@@ -1,16 +1,16 @@
 #!/usr/bin/env python3
-"""bench.py -- measurement of the protected-region hot path on B200.
+"""bench.py -- measurement of the protected-region hot path on H100.
 
 Headline workload (BASELINE.json configs[1]): SHA-256 under TMR, 2^20 x 64-byte messages per GPU, warp-shuffle
 select voter, -countErrors -countSyncs.  Metric: MB/s of VOTED OUTPUT.  One "step" = one protected launch over the
 whole batch.  The same JSON line carries the other BASELINE configs under "also" (each timed in the same process
 with its own roofline / e2e / cpu_baseline):
     N = 1 : aes (configs[2]), gemm (configs[3]), crc16 (config-1 timing shape), crc16_cpu_1thread (configs[0]),
-            sha256_2p30 (configs[4] on one GPU)
-    N > 1 : sha256_2p30 strong-scaled over the ranks (configs[4]), gemm sharded by C row-blocks (configs[3])
+            sha256_2p29 (configs[4], 2^29 messages: what 80 GB hold, on one GPU)
+    N > 1 : sha256_2p29 strong-scaled over the ranks (configs[4]), gemm sharded by C row-blocks (configs[3])
 
   python bench.py [--gpus N --steps K --warmup W]          # this repo's CUDA path
-  python bench.py --workload aes|gemm|crc16|sha256_2p30     # one workload as its own line
+  python bench.py --workload aes|gemm|crc16|sha256_2p29     # one workload as its own line
   python bench.py --impl reference ...                      # the reference's own C sources (oracle/_ref, else the
                                                             # oracle port) under CPU xMR, all host threads
 Under torchrun (N>1) every rank works on its own shard (no data-path collective).  The ranks rendezvous ON THE GPU
@@ -19,7 +19,9 @@ counters -- is done BY THE KERNELS: ranks 1..N-1 map rank 0's counter block over
 kernel's closing tally is a handful of system-scope atomics into it, so the timed region holds no collective at all and
 rank 0's coast_sync() reads the whole job's TMR_ERROR_CNT / __SYNC_COUNT.  (Without peer access the fallback is ONE NCCL
 all-reduce of the 4 counters per timed region, inside the region; `collectives.counter_fold` says which ran.)
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes, after the timed steps, the voted output of the last timed step of
+every workload measured as DIR/<workload>.npy (float64 for 32-bit words, float32 otherwise; an output of more than 2^19 elements
+as a fixed seeded sample, whose element indices go to DIR/<workload>_index.npy).
 """
 from __future__ import annotations
 
@@ -35,23 +37,22 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 METRIC = "protected-kernel throughput (MB/s voted output), sha256 TMR"
-SM_COUNT = 148
 
 # one name per workload, shared by both arms so that `config` is identical in the two JSON lines the driver compares
 WORKLOAD_NAMES = {
     "sha256": "sha256 TMR, 2^20 x 64-byte messages per GPU (BASELINE configs[1])",
-    "sha256_2p30": "batched sha256 TMR, 2^30 x 64-byte messages sharded over the GPUs (BASELINE configs[4])",
+    "sha256_2p29": "batched sha256 TMR, 2^29 x 64-byte messages sharded over the GPUs (BASELINE configs[4], sized for 80 GB)",
     "aes": "aes-128 ECB encrypt DWC, 2^24 x 16-byte blocks, Bernoulli(2^-10) single-bit flips (BASELINE configs[2])",
     "crc16": "crc16 TMR, 2^20 x 64-byte messages (SURVEY.md 8d config 1 timing shape)",
-    "gemm": "matmul TMR 4096x4096x4096 fp32 on tcgen05 kind::tf32, three TMEM accumulator replicas + voter (BASELINE configs[3])",
+    "gemm": "matmul TMR 4096x4096x4096 fp32 on wgmma tf32, three register accumulator replicas + voter (BASELINE configs[3])",
 }
-PROTECTION = {"sha256": "-TMR -countErrors -countSyncs", "sha256_2p30": "-TMR -countErrors -countSyncs",
+PROTECTION = {"sha256": "-TMR -countErrors -countSyncs", "sha256_2p29": "-TMR -countErrors -countSyncs",
               "aes": "-DWC + single-bit-flip injector", "crc16": "-TMR -countErrors -countSyncs",
               "gemm": "-TMR -countErrors -countSyncs"}
-FULL_UNITS = {"sha256": 1 << 20, "sha256_2p30": 1 << 30, "aes": 1 << 24, "crc16": 1 << 20, "gemm": 4096 * 4096}
-OUT_B = {"sha256": 32, "sha256_2p30": 32, "aes": 16, "crc16": 2, "gemm": 4}
-DTYPE = {"sha256": "u32", "sha256_2p30": "u32", "aes": "u8", "crc16": "u16", "gemm": "f32(tf32 mma)"}
-STRONG = {"sha256_2p30", "gemm"}
+FULL_UNITS = {"sha256": 1 << 20, "sha256_2p29": 1 << 29, "aes": 1 << 24, "crc16": 1 << 20, "gemm": 4096 * 4096}
+OUT_B = {"sha256": 32, "sha256_2p29": 32, "aes": 16, "crc16": 2, "gemm": 4}
+DTYPE = {"sha256": "u32", "sha256_2p29": "u32", "aes": "u8", "crc16": "u16", "gemm": "f32(tf32 mma)"}
+STRONG = {"sha256_2p29", "gemm"}
 
 
 def metric_name(wl):
@@ -64,7 +65,7 @@ def config_for(wl: str, n_gpus: int) -> dict:
             "units": FULL_UNITS[wl], "units_are": "in total, sharded over the GPUs" if wl in STRONG else "per GPU",
             "protection": PROTECTION[wl], "voter": "select (r0==r1?r0:r2), one vote per stored element",
             "inputs": "Philox4x32-10 counter stream, identical bytes in both arms",
-            "l2": "rotating in/out buffer sets larger than the 126 MB L2 (one set when a set alone is larger)",
+            "l2": "rotating in/out buffer sets larger than the 50 MB L2 (one set when a set alone is larger)",
             "parallelism": f"shard{n_gpus}" if n_gpus > 1 else "1gpu"}
 
 
@@ -80,7 +81,7 @@ def hbm_peak():
     pj = measured_peaks()
     if "hbm_gbs" in pj:
         return float(pj["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -335,49 +336,46 @@ def workload_table(cb):
     F = cb.F_COUNT_ERRORS | cb.F_COUNT_SYNCS
     return {
         "sha256": dict(kernel=cb.K_SHA256, nc=3, flags=F, unit_bytes=64, in_b=64, alg_b=96, plan=None,
-                       kname="xmr_sha256_b64_seg_nc3_inj0", bound="hbm", sets=4, profile="r01_sha256_tmr_seg.json",
-                       profile_units=1 << 20, traffic="r01_sha256_tmr_traffic.json"),
-        "sha256_2p30": dict(kernel=cb.K_SHA256, nc=3, flags=F, unit_bytes=64, in_b=64, alg_b=96, plan=None,
-                            kname="xmr_sha256_b64_seg_nc3_inj0", bound="hbm", sets=1, profile="r01_sha256_tmr_seg.json",
-                            profile_units=1 << 20, traffic=None),
+                       kname="xmr_sha256_b64_seg_nc3_inj0", bound="hbm", sets=4),
+        "sha256_2p29": dict(kernel=cb.K_SHA256, nc=3, flags=F, unit_bytes=64, in_b=64, alg_b=96, plan=None,
+                            kname="xmr_sha256_b64_seg_nc3_inj0", bound="hbm", sets=1),
         "aes": dict(kernel=cb.K_AES128, nc=2, flags=0, unit_bytes=0, in_b=16, alg_b=32,
                     plan=dict(seed=33, p=2.0 ** -10), key=bytes(16),
-                    kname="xmr_aes128_enc_nc2_inj1", bound="hbm", sets=2, profile="r02_aes_nc2_inj1.json", profile_units=1 << 24,
-                    traffic="r02_aes_traffic.json"),
+                    kname="xmr_aes128_enc_nc2_inj1", bound="hbm", sets=2),
         "crc16": dict(kernel=cb.K_CRC16, nc=3, flags=F, unit_bytes=64, in_b=64, alg_b=66, plan=None,
-                      kname="xmr_crc16_b64_nc3_inj0", bound="hbm", sets=4, profile="r01_crc16_nc3_v2.json", profile_units=1 << 20,
-                      traffic="r01_crc16_traffic.json"),
+                      kname="xmr_crc16_b64_nc3_inj0", bound="hbm", sets=4),
         "gemm": dict(kernel=cb.K_GEMM_TF32, nc=3, flags=F, side=4096, plan=None,
-                     kname="xmr_gemm_tf32_nc3_inj0", bound="tensor", sets=2, profile="r02_gemm_nc3.json", profile_units=4096 * 4096,
-                     traffic="r02_gemm_traffic.json"),
+                     kname="xmr_gemm_tf32_nc3_inj0", bound="tensor", sets=2),
     }
-
-
-def static_profile(name):
-    """ncu numbers that are properties of the CODE (instruction count per launch, pipe shares), read from the committed
-    summary under profiles/ and labelled as static wherever they are used."""
-    if not name:
-        return None
-    fallbacks = {"r02_aes_nc2_inj1.json": "r01_aes_nc2_inj.json", "r02_gemm_nc3.json": "r01_gemm_nc3_final.json"}
-    for cand in (name, fallbacks.get(name, name)):
-        p = os.path.join(ROOT, "profiles", cand)
-        if os.path.exists(p):
-            try:
-                with open(p) as f:
-                    d = json.load(f)
-                d = d[0] if isinstance(d, list) else d
-                d["_file"] = f"profiles/{cand}"
-                return d
-            except Exception:
-                return None
-    return None
 
 
 class Ctx:
     pass
 
 
-def measure(cx, wl: str, steps: int, warmup: int, *, cpu_budget_s: float = 0.0, e2e_cap_units: int = 1 << 24):
+DUMP_SAMPLE = 1 << 19
+DUMP_VIEW = {"sha256": "u32", "sha256_2p29": "u32", "aes": "u8", "crc16": "u16", "gemm": "f32"}
+
+
+def dump_output(dump_dir, name, out, view):
+    """The voted output of one step (a device tensor) as DIR/<name>.npy: 32-bit words as float64 (exact), bytes, halves and fp32 as
+    float32.  More than DUMP_SAMPLE elements: a fixed seeded sample (sorted indices in DIR/<name>_index.npy)."""
+    import numpy as np
+    import torch
+    x = out.view({"f32": torch.float32, "u32": torch.int32, "u16": torch.int16, "u8": torch.uint8}[view])
+    n = x.numel()
+    os.makedirs(dump_dir, exist_ok=True)
+    if n > DUMP_SAMPLE:
+        idx = np.sort(np.random.default_rng(20240601).integers(0, n, DUMP_SAMPLE, dtype=np.int64))
+        x = x[torch.from_numpy(idx).to(x.device)]
+        np.save(os.path.join(dump_dir, f"{name}_index.npy"), idx.astype(np.float64))
+    x = x.cpu().numpy()
+    if view in ("u32", "u16"):
+        x = x.view(np.uint32 if view == "u32" else np.uint16)
+    np.save(os.path.join(dump_dir, f"{name}.npy"), x.astype(np.float64 if view == "u32" else np.float32))
+
+
+def measure(cx, wl: str, steps: int, warmup: int, *, cpu_budget_s: float = 0.0, e2e_cap_units: int = 1 << 24, dump_dir=None):
     """One workload on this rank's GPU: device-timed region, single-launch loop, end-to-end host call.  Returns the
     JSON-line dict on rank 0 (None elsewhere).  Every rank must call it with the same arguments."""
     torch, cb, rt, dist = cx.torch, cx.cb, cx.rt, cx.dist
@@ -418,8 +416,8 @@ def measure(cx, wl: str, steps: int, warmup: int, *, cpu_budget_s: float = 0.0, 
         if wl in STRONG:                                     # config 5: a fixed 2^30-message batch, contiguous shards
             lo, hi = shard_range(FULL_UNITS[wl], rank, world)
             n, unit_base, scaling = hi - lo, lo, "strong"
-            if n * 96 > 150 * (1 << 30):
-                raise SystemExit(f"{wl}: {n} messages per GPU do not fit 180 GB; use more GPUs")
+            if n * 96 > 64 * (1 << 30):
+                raise SystemExit(f"{wl}: {n} messages per GPU do not fit 80 GB; use more GPUs")
         else:
             n = FULL_UNITS[wl]                               # weak scaling: the same shard size on every GPU
             unit_base = rank * n
@@ -489,6 +487,8 @@ def measure(cx, wl: str, steps: int, warmup: int, *, cpu_budget_s: float = 0.0, 
         rt.clock_probe(probe1)
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1)
+    if dump_dir and descs:                                 # what the last timed step computed (outside the timed region)
+        dump_output(dump_dir, wl if world == 1 else f"{wl}_rank{rank}", outs[(steps - 1) % nsets], DUMP_VIEW[wl])
     timed_launches = launches
     # the SM clock the region REALLY ran at: cycles / nanoseconds between the two probes, per SM that answered both, median
     p0, p1 = probe0.view(-1, 2).cpu(), probe1.view(-1, 2).cpu()
@@ -638,44 +638,24 @@ def measure(cx, wl: str, steps: int, warmup: int, *, cpu_budget_s: float = 0.0, 
     # the dominant kernel's average launch duration over the TIMED REGION (one launch per step, back to back on the
     # launching stream, CUDA events); the per-launch event pairs measured after it (k_ms) are kept as a cross-check
     k_reg = ms / max(1, timed_launches)
-    prof = static_profile(W.get("profile"))
-    sm_hz = (clocks.get("sm_mhz_in_timed_region") or clocks.get("sm_mhz") or 1965.0) * 1e6   # the delivered clock when the probes answered
+    sm_hz = (clocks.get("sm_mhz_in_timed_region") or clocks.get("sm_mhz") or 1755.0) * 1e6   # the delivered clock when the probes answered
     sm_hz_how = "SM clock delivered in the timed region (clock64/globaltimer probes)" if clocks.get("sm_mhz_in_timed_region") else "NVML-sampled SM clock"
     if W["bound"] == "hbm":
         peak, peak_src = hbm_peak()
         achieved, unit = alg_bytes / (k_reg * 1e-3) / 1e9, "GB/s"
         rl_extra = {"algorithmic_bytes_per_launch": alg_bytes,
-                    "note": "integer-issue / shared-memory bound, not HBM bound (DESIGN.md section 5): alu_frac and issue_frac say how "
-                            "close the kernel is to the SM's integer ceiling"}
+                    "note": "integer-issue / shared-memory bound, not HBM bound (DESIGN.md section 5)"}
     else:
         pj = measured_peaks()
-        peak = float(pj.get("bf16_tflops", 1590.0)) / 2.0
-        peak_src = "measured bf16 cuBLAS burst / 2 (TF32 runs at half the bf16 rate)" if pj else "fallback 1590/2"
+        peak = float(pj.get("bf16_tflops", 989.0)) / 2.0
+        peak_src = ("measured bf16 cuBLAS burst / 2 (TF32 runs at half the bf16 rate)" if pj else
+                    "H100 SXM data sheet: 989 TFLOP/s dense bf16 / 2 = TF32 dense, at 700 W; not measured")
         achieved, unit = flops_issued / (k_reg * 1e-3) / 1e12, "TFLOP/s"
-        hw = 4096.0 * SM_COUNT * sm_hz / 1e12                # tcgen05 kind::tf32: 4096 dense FLOP / clk / SM
+        hw = 2048.0 * n_sm * sm_hz / 1e12                   # TF32 wgmma: 2048 dense FLOP / clk / SM
         rl_extra = {"issued_flops_per_launch": flops_issued, "useful_flops_per_launch": flops_issued / 3,
                     "frac_of_clock_scaled_hw_rate": round(achieved / hw, 5),
-                    "clock_scaled_hw_rate": {"value": round(hw, 1), "unit": "TFLOP/s", "how": "4096 FLOP/clk/SM x 148 SMs x " + sm_hz_how},
+                    "clock_scaled_hw_rate": {"value": round(hw, 1), "unit": "TFLOP/s", "how": f"2048 FLOP/clk/SM x {n_sm} SMs x " + sm_hz_how},
                     "note": "issued = 3 replicas x 2MNK; useful = one replica"}
-    if prof and prof.get("kernel") == W["kname"] and "warp_insts" in prof:
-        # instructions per launch are a property of the CODE (static, from the committed ncu summary, scaled to this launch's
-        # unit count); the time is live
-        wi = prof["warp_insts"] * (n / float(W["profile_units"]))
-        rl_extra["issue_frac"] = round(wi / (k_reg * 1e-3) / (SM_COUNT * 4 * sm_hz), 4)
-        rl_extra["issue_frac_how"] = (f"warp instructions per launch ({prof['_file']}, static) / live kernel time / "
-                                      "(148 SMs x 4 schedulers x 1 warp instruction per clock x " + sm_hz_how + ")")
-        if W["bound"] == "hbm" and "pipe_alu_pct" in prof:
-            rl_extra["alu_frac"] = round(prof["pipe_alu_pct"] / 100.0, 4)
-            rl_extra["alu_frac_source"] = f"{prof['_file']} (static): ncu sm__inst_executed_pipe_alu, pct of peak sustained active"
-    traffic, traffic_src = None, None
-    if W.get("traffic"):
-        tp = os.path.join(ROOT, "profiles", W["traffic"])
-        if os.path.exists(tp):
-            with open(tp) as f:
-                tj = json.load(f)
-            if tj.get("kernel", W["kname"]) == W["kname"]:
-                traffic = tj.get("dram_bytes_per_launch")
-                traffic_src = f"profiles/{W['traffic']} (static: one ncu --set full capture of this kernel at this size, not measured in this run)"
     bound_s = max(h2d / (pcie_h2d * 1e9), d2h / (pcie_d2h * 1e9))
     line = {
         "metric": metric_name(wl),
@@ -684,7 +664,7 @@ def measure(cx, wl: str, steps: int, warmup: int, *, cpu_budget_s: float = 0.0, 
         "vs_baseline": None, "dtype": DTYPE[wl], "data": "synthetic",
         "config": config_for(wl, world),
         "roofline": dict({"bound": W["bound"], "achieved": round(achieved, 2), "peak": peak, "unit": unit,
-                          "frac": round(achieved / peak, 5), "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                          "frac": round(achieved / peak, 5), "peak_source": peak_src,
                           "kernel": W["kname"], "kernel_ms": round(k_reg, 5),
                           "kernel_ms_source": "timed region / launches (CUDA events on the launching stream)",
                           "kernel_ms_single_launch_events": round(k_ms, 5)}, **rl_extra),
@@ -720,7 +700,7 @@ def measure(cx, wl: str, steps: int, warmup: int, *, cpu_budget_s: float = 0.0, 
     return line
 
 
-ALSO_STEPS = {"aes": 20, "gemm": 40, "crc16": 200, "sha256_2p30": 3}
+ALSO_STEPS = {"aes": 20, "gemm": 40, "crc16": 200, "sha256_2p29": 3}
 
 
 def run_ours(args):
@@ -755,14 +735,14 @@ def run_ours(args):
                                                       log=lambda m: print("bench: " + m, file=sys.stderr))
 
     main_cpu = 0.0 if args.no_cpu_baseline else 10.0
-    line = measure(cx, args.workload, args.steps, args.warmup, cpu_budget_s=main_cpu)
+    line = measure(cx, args.workload, args.steps, args.warmup, cpu_budget_s=main_cpu, dump_dir=args.dump_outputs)
     if args.workload == "sha256" and not args.no_also:
         also = {}
-        wls = ["aes", "gemm", "crc16", "sha256_2p30"] if cx.world == 1 else ["sha256_2p30", "gemm"]
+        wls = ["aes", "gemm", "crc16", "sha256_2p29"] if cx.world == 1 else ["sha256_2p29", "gemm"]
         for wl in wls:
             t0 = time.perf_counter()
             try:
-                sub = measure(cx, wl, ALSO_STEPS[wl], 3, cpu_budget_s=0.0 if args.no_cpu_baseline else 3.0)
+                sub = measure(cx, wl, ALSO_STEPS[wl], 3, cpu_budget_s=0.0 if args.no_cpu_baseline else 3.0, dump_dir=args.dump_outputs)
             except Exception as exc:                       # an extra workload must never cost the headline line
                 sub = {"error": repr(exc)[:300]}
                 if cx.dist is not None:
@@ -793,9 +773,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-also", action="store_true", help="headline workload only (skip the other BASELINE configs)")
     ap.add_argument("--host-path", choices=["staged", "hybrid", "zerocopy", "one-shot"], default=None, help="force the host-call path of the e2e measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the voted output of the last timed step of each workload as DIR/<workload>.npy")
     ap.add_argument("--ref-budget-s", type=float, default=90.0, help="--impl reference: CPU seconds the whole run may take")
     ap.add_argument("--threads", type=int, default=0, help="--impl reference: host threads (default: all; config 1 is 1 thread)")
-    ap.add_argument("--workload", choices=["sha256", "sha256_2p30", "aes", "crc16", "gemm"], default="sha256",
+    ap.add_argument("--workload", choices=["sha256", "sha256_2p29", "aes", "crc16", "gemm"], default="sha256",
                     help="default sha256 = BASELINE configs[1], the headline line (with the other configs under `also`)")
     args = ap.parse_args()
     if args.warmup < 3:

@@ -1,6 +1,6 @@
-"""coast_b200 -- B200-native redundant execution (TMR/DWC) behind the COAST annotation surface.
+"""coast_b200 -- H100-native redundant execution (TMR/DWC) behind the COAST annotation surface.
 
-The product is the C-ABI library ``libcoast_rt.so`` (include/coast_rt.h): hand-written sm_100a
+The product is the C-ABI library ``libcoast_rt.so`` (include/coast_rt.h): hand-written sm_90a
 kernels in which every live value of a protected region is computed by 2 (DWC) or 3 (TMR)
 replicas on adjacent lanes and voted at the sphere-of-replication exit.  This package is the
 thin Python host mirror used by the tests and bench.py; PyTorch supplies device memory,

@@ -1,4 +1,4 @@
-"""In-tree build of libcoast_rt.so (nvcc cross-compiles sm_100a without a GPU)."""
+"""In-tree build of libcoast_rt.so (nvcc cross-compiles sm_90a without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -19,7 +19,7 @@ def _stale() -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Compile coast_kernels.cu -> sm_100a cubin and link libcoast_rt.so next to this file."""
+    """Compile coast_kernels.cu -> sm_90a cubin and link libcoast_rt.so next to this file."""
     if force or _stale():
         cmd = ["make", "-C", CSRC] + (["-B"] if force else [])
         res = subprocess.run(cmd, capture_output=not verbose, text=True)

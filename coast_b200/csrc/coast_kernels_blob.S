@@ -1,4 +1,4 @@
-/* Embeds the sm_100a device module (coast_kernels.cubin) into libcoast_rt.so. */
+/* Embeds the sm_90a device module (coast_kernels.cubin) into libcoast_rt.so. */
     .section .rodata
     .balign 64
     .global coast_kernels_cubin

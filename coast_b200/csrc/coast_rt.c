@@ -4,7 +4,7 @@
  * Replaces, at run time, what byuccl/coast does at compile time:
  *   projects/dataflowProtection (run(M, numClones), dataflowProtection.cpp:63-164),
  *   projects/TMR (TMR.cpp:29-36) and projects/DWC (DWC.cpp:29-36)
- * by launching a hand-written sm_100a kernel in which every live value of the protected
+ * by launching a hand-written sm_90a kernel in which every live value of the protected
  * region is computed by num_clones replicas and voted at the SoR exit.
  *
  * libcuda.so.1 is bound lazily with dlopen() so that this library LOADS without a GPU
@@ -153,7 +153,7 @@ static int drv_fail(CUresult r, const char* what) {
 #define DRV(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) return drv_fail(r_, #call); } while (0)
 
 const char* coast_last_error(void) { return G.err; }
-const char* coast_version(void) { return "coast_rt 0.1 (sm_100a)"; }
+const char* coast_version(void) { return "coast_rt 0.1 (sm_90a)"; }
 
 static int bind_driver(void) {
     if (G.libcuda) return COAST_OK;
@@ -175,9 +175,8 @@ static int bind_driver(void) {
 /* NUMA placement                                                        */
 /* ------------------------------------------------------------------ */
 /* The host-call path (coast_run_host) is PCIe-bound; on a two-socket box a process that runs -- and first-touches its
- * pinned buffers -- on the socket the GPU is NOT attached to loses up to half of the copy bandwidth (measured r01: 1.69 vs
- * 3.16 ms per 96 MiB step on two boxes).  coast_init() therefore moves the calling thread (threads it creates later inherit
- * it) onto the CPUs of the GPU's NUMA node and makes that node the preferred one for its memory.  Plain syscalls, no
+ * pinned buffers -- on the socket the GPU is NOT attached to can lose up to half of the copy
+ * bandwidth.  coast_init() therefore moves the calling thread (threads it creates later inherit it) onto the CPUs of the GPU's NUMA node and makes that node the preferred one for its memory.  Plain syscalls, no
  * libnuma.  COAST_NUMA_BIND=0 leaves the process alone.  Best effort: any failure leaves things as they were. */
 #ifndef MPOL_PREFERRED
 #define MPOL_PREFERRED 1
@@ -287,15 +286,15 @@ static int init_impl(int device) {
     int major = 0, minor = 0;
     p_cuDeviceGetAttribute(&major, CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MAJOR, G.dev);
     p_cuDeviceGetAttribute(&minor, CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MINOR, G.dev);
-    if (major != 10) {
+    if (major != 9 || minor != 0) {
         p_cuDevicePrimaryCtxRelease_v2(G.dev);
-        return fail(COAST_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library carries sm_100a code only", device, major, minor);
+        return fail(COAST_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library carries sm_90a code only", device, major, minor);
     }
     p_cuDeviceGetAttribute(&G.sm_count, CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT, G.dev);
     numa_bind_to_gpu();
-    G.host_path_default = 0;        /* measured r02 (profiles/r02_e2e_zero_copy_experiment.md) */
+    G.host_path_default = 0;        /* staged: the copy engines move the bytes */
     r = p_cuModuleLoadData(&G.mod, coast_kernels_cubin);
-    if (r != CUDA_SUCCESS) { p_cuDevicePrimaryCtxRelease_v2(G.dev); return drv_fail(r, "cuModuleLoadData(sm_100a cubin)"); }
+    if (r != CUDA_SUCCESS) { p_cuDevicePrimaryCtxRelease_v2(G.dev); return drv_fail(r, "cuModuleLoadData(sm_90a cubin)"); }
     DRV(p_cuMemAlloc_v2(&G.counters, XMR_CTR_COUNT * sizeof(uint64_t)));
     {
         CUmemPoolProps pp; memset(&pp, 0, sizeof pp);
@@ -369,7 +368,7 @@ int coast_parse_opt_passes(const char* s, uint32_t* num_clones, uint32_t* flags)
             fprintf(stderr, "coast_rt: -reportErrors is deprecated in the reference (counts AGREEING syncs, "
                             "synchronization.cpp:1323-1350) and is not emulated; use -countErrors\n");
         }
-        else fprintf(stderr, "coast_rt: OPT_PASSES token '%s' has no effect on the B200 runtime (ignored)\n", tok);
+        else fprintf(stderr, "coast_rt: OPT_PASSES token '%s' has no effect on the GPU runtime (ignored)\n", tok);
     }
     if (tmr && dwc) return fail(COAST_ERR_BAD_ARG, "-TMR and -DWC are mutually exclusive");
     if (tmr) nc = COAST_TMR; else if (dwc) nc = COAST_DWC;
@@ -488,40 +487,42 @@ static int encode_rows_map(CUtensorMap* map, const void* base, uint32_t row_byte
     return COAST_OK;
 }
 
-/* tcgen05 TF32 GEMM: A through a 2-D map (box 32 k x 128 m), B (row-major K x N, N contiguous) through a 3-D view
- * {32 n, K, N/32} (box 32 x 32 x 4) so one TMA lands the [n-chunk][k][128 B] layout the MN-major UMMA descriptor reads. */
-/* tile geometry mirrors xmr::gemm::Geom<NC>: unprotected 128 x 256 tiles on 4 stages, DWC/TMR 128 x 128 on 6 stages */
-static int launch_gemm_tf32(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream) {
+/* TF32 GEMM on wgmma (xmr_gemm_tf32.cuh): B (row-major K x N) is transposed into stream-ordered scratch first, because TF32
+ * wgmma reads both operands K-major; A and B^T then go through 2-D maps with the 128-byte swizzle (box 32 k x 128 rows; the
+ * CTA-pair kernels load B^T in 64-row boxes, half of a 128-column block per CTA, multicast to both).
+ * Tile geometry mirrors xmr::gemm::Geom<NC>: unprotected 128 x 256 tiles on 4 stages, DWC/TMR 128 x 128 on 6 stages. */
+static int launch_gemm_tf32_bt(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream, CUdeviceptr bt) {
     char name[64];
     const int wide = d->num_clones == 1 && d->N % 256u == 0;
     if (d->num_clones == 1 && !wide) snprintf(name, sizeof name, "xmr_gemm_tf32n_nc1_inj%d", inj);
     else snprintf(name, sizeof name, "xmr_gemm_tf32_nc%u_inj%d", d->num_clones, inj);
     unsigned bn = wide ? 256u : 128u, stages = wide ? 4u : 6u;
-    unsigned GEMM_SMEM = stages * (16384u + 32u * bn * 4u) + 1024u + 256u;
-    /* CTA-pair kernels (xmr_gemm_tf32_pair.cuh, tcgen05 cta_group::2): 256 x BN pair tiles, each CTA stages half of B.  Bit-identical
-     * to the single-CTA kernels; measured at 4096^3: unprotected 0.190 vs 0.201 ms, DWC 0.320 vs 0.328 ms, TMR 0.465 vs 0.463 ms
-     * (profiles/r02_gemm_pair_timings.txt).  Default: pairs for the unprotected and DWC kernels when the shape allows (M % 256,
-     * N % BN), the single-CTA kernel for TMR; COAST_GEMM_PAIR=0 / 1 forces one or the other for every replica count. */
-    unsigned b_box_chunks = 4u;
+    /* CTA-pair kernels (cluster 2 x 1 x 1, 256 x BN pair tiles, B multicast): bit-identical to the single-CTA kernels.  Default:
+     * pairs for the unprotected and DWC kernels when the shape allows (M % 256, N % BN), the single-CTA kernel for TMR;
+     * COAST_GEMM_PAIR=0 / 1 forces one or the other for every replica count. */
+    unsigned b_box = 128u;
     int pair = 0;
     { const char* e = getenv("COAST_GEMM_PAIR");
       const unsigned pbn = d->num_clones == 1 ? 256u : 128u;
       const int want = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : d->num_clones < 3;
       if (want && d->M % 256u == 0 && d->N % pbn == 0 && G.sm_count >= 2) {
-          pair = 1; bn = pbn; stages = d->num_clones == 1 ? 6u : 8u; b_box_chunks = 2u;
-          GEMM_SMEM = stages * (16384u + 32u * (bn / 2u) * 4u) + 1024u + 256u;
+          pair = 1; bn = pbn; stages = d->num_clones == 1 ? 4u : 6u; b_box = 64u;
           snprintf(name, sizeof name, "xmr_gemm_tf32p_nc%u_inj%d", d->num_clones, inj);
       } }
+    const unsigned GEMM_SMEM = stages * (16384u + 32u * bn * 4u) + 1024u + 256u;
     { const char* g = getenv("COAST_GEMM_GROUP_M"); if (g && atoi(g) > 0 && atoi(g) < 256) a->mode = (a->mode & ~0xFFu) | (unsigned)atoi(g); }
-    /* L2 eviction priorities (A evict_last, B and C evict_first): 5 % fewer DRAM reads at 4096^3, same time (profiles/r02_gemm_l2_sweep.txt) */
+    /* L2 eviction priorities: A evict_last, B and C evict_first; COAST_GEMM_L2_HINTS=0 loads and stores with the normal policy */
     { const char* h = getenv("COAST_GEMM_L2_HINTS"); if (!(h && !strcmp(h, "0"))) a->mode |= 0x100u; }
     /* the unprotected kernel halves the tiles of a short last round (xmr_gemm_tf32.cuh); COAST_GEMM_TAIL_SPLIT=0 keeps whole tiles */
     { const char* h = getenv("COAST_GEMM_TAIL_SPLIT"); if (h && !strcmp(h, "0")) a->mode |= 0x200u; }
-    /* DWC / TMR: the A operand stays in the tensor core's collector across the replicas of a k-step (tcgen05.mma collector::a::fill /
-     * use / lastuse); COAST_GEMM_KEEP_A=0 re-reads it from shared memory for every replica */
-    { const char* h = getenv("COAST_GEMM_KEEP_A"); if (h && !strcmp(h, "0")) a->mode |= 0x400u; }
     CUfunction fn; int occ = 1;
-    int rc = get_fn(name, GEMM_SMEM, &fn, &occ); if (rc) return rc;
+    int rc = get_fn("xmr_gemm_bt", 0, &fn, NULL); if (rc) return rc;
+    {
+        const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N;
+        void* params[] = { &B, &bt, &k32, &n32 };
+        DRV(p_cuLaunchKernel(fn, (unsigned)G.sm_count * 8u, 1, 1, 256, 1, 1, 0, stream, params, NULL));
+    }
+    rc = get_fn(name, GEMM_SMEM, &fn, &occ); if (rc) return rc;
     CUtensorMap ma, mb;
     {
         cuuint64_t gdim[2] = { d->K, d->M };
@@ -533,12 +534,12 @@ static int launch_gemm_tf32(const coast_launch_desc* d, xmr_args* a, int inj, CU
                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
     }
     {
-        cuuint64_t gdim[3] = { 32, d->K, d->N / 32u };
-        cuuint64_t gstr[2] = { (cuuint64_t)d->N * 4u, 128u };
-        cuuint32_t box[3] = { 32, 32, b_box_chunks };       /* 128 columns per load; a 256-wide tile takes two (pair kernels: one half tile) */
-        cuuint32_t estr[3] = { 1, 1, 1 };
-        DRV(p_cuTensorMapEncodeTiled(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)d->d_aux, gdim, gstr, box, estr,
-                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B,
+        cuuint64_t gdim[2] = { d->K, d->N };
+        cuuint64_t gstr[1] = { (cuuint64_t)d->K * 4u };
+        cuuint32_t box[2] = { 32, b_box };
+        cuuint32_t estr[2] = { 1, 1 };
+        DRV(p_cuTensorMapEncodeTiled(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)bt, gdim, gstr, box, estr,
+                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
     }
     unsigned tiles = (d->M / 128u) * (d->N / bn);           /* pair kernels: CTAs = 2 x pair tiles, an even grid (cluster 2 x 1 x 1) */
@@ -549,11 +550,19 @@ static int launch_gemm_tf32(const coast_launch_desc* d, xmr_args* a, int inj, CU
     DRV(p_cuLaunchKernel(fn, grid, 1, 1, 384, 1, 1, GEMM_SMEM, stream, params, NULL));
     return COAST_OK;
 }
+/* B^T is per-launch scratch from the stream-ordered pool, like the limb planes below */
+static int launch_gemm_tf32(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream) {
+    CUdeviceptr bt = 0;
+    DRV(p_cuMemAllocFromPoolAsync(&bt, (size_t)d->K * d->N * 4u, G.pool, stream));
+    int rc = launch_gemm_tf32_bt(d, a, inj, stream, bt);
+    p_cuMemFreeAsync(bt, stream);
+    return rc;
+}
 
-/* Exact integer matmul on tcgen05 kind::i8 (xmr_mm_tc.cuh): split A and B into u8 limb planes (library scratch),
- * then ten u8 GEMMs per replica into four s32 TMEM accumulators, recombined modulo 2^32 in the epilogue. */
-static int launch_mm_tc_planes(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream, int atmem, CUdeviceptr pa, CUdeviceptr pb) {
-    const uint32_t nc = d->num_clones, bn = atmem ? (nc == 1 ? 64u : 32u) : (nc == 3 ? 32u : 64u);
+/* Exact integer matmul on wgmma u8 (xmr_mm_tc.cuh): split A and B into u8 limb planes (library scratch),
+ * then ten u8 GEMMs per replica into four s32 register accumulators, recombined modulo 2^32 in the epilogue. */
+static int launch_mm_tc_planes(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream, CUdeviceptr pa, CUdeviceptr pb) {
+    const uint32_t nc = d->num_clones, bn = nc == 1 ? 64u : 32u;
     {
         CUfunction f; int rc = get_fn("xmr_mm_split_a", 0, &f, NULL); if (rc) return rc;
         unsigned long long rows = d->M, K = d->K; const void* A = d->d_in;
@@ -564,11 +573,9 @@ static int launch_mm_tc_planes(const coast_launch_desc* d, xmr_args* a, int inj,
         void* params2[] = { &B, &pb, &k32, &n32 };
         DRV(p_cuLaunchKernel(f, (unsigned)G.sm_count * 8u, 1, 1, 256, 1, 1, 0, stream, params2, NULL));
     }
-    /* the MMAs that share an A limb keep it in the tensor core's collector (xmr_mm_tc.cuh); COAST_MM_KEEP_A=0 issues them plain */
-    { const char* h = getenv("COAST_MM_KEEP_A"); if (h && !strcmp(h, "0")) a->mode |= 0x400u; else a->mode &= ~0x400u; }
     const unsigned smem = 2u * (65536u + 4u * bn * 128u) + 1024u + 256u;
     char name[64];
-    snprintf(name, sizeof name, "xmr_mm_u32_%s_nc%u_inj%d", atmem ? "tct" : "tc", nc, inj);
+    snprintf(name, sizeof name, "xmr_mm_u32_tc_nc%u_inj%d", nc, inj);
     CUfunction fn; int occ = 1;
     int rc = get_fn(name, smem, &fn, &occ); if (rc) return rc;
     CUtensorMap ma, mb;
@@ -594,17 +601,17 @@ static int launch_mm_tc_planes(const coast_launch_desc* d, xmr_args* a, int inj,
     unsigned grid = tiles < (unsigned)G.sm_count ? tiles : (unsigned)G.sm_count;
     void* params[3] = { a, &ma, &mb };
     if (d->flags & COAST_F_VERBOSE) fprintf(stderr, "coast_rt: %s grid=%u smem=%u tiles=%u\n", name, grid, smem, tiles);
-    DRV(p_cuLaunchKernel(fn, grid, 1, 1, 256, 1, 1, smem, stream, params, NULL));
+    DRV(p_cuLaunchKernel(fn, grid, 1, 1, 384, 1, 1, smem, stream, params, NULL));
     return COAST_OK;
 }
 /* The limb planes (4 x u8 per element of A and of B^T) are per-launch scratch from the stream-ordered pool, like the
  * quicksort replicas: allocated on the launch's stream, released on it after the kernel, so launches on different
  * streams never share planes.  The pool keeps released memory cached, so steady state costs no driver allocation. */
-static int launch_mm_tc(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream, int atmem) {
+static int launch_mm_tc(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream) {
     const size_t a_bytes = (size_t)d->M * d->K * 4u, b_bytes = (size_t)d->K * d->N * 4u;   /* 4 planes of 1 byte per element */
     CUdeviceptr planes = 0;
     DRV(p_cuMemAllocFromPoolAsync(&planes, a_bytes + b_bytes, G.pool, stream));
-    int rc = launch_mm_tc_planes(d, a, inj, stream, atmem, planes, planes + a_bytes);
+    int rc = launch_mm_tc_planes(d, a, inj, stream, planes, planes + a_bytes);
     p_cuMemFreeAsync(planes, stream);
     return rc;
 }
@@ -705,14 +712,13 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "MM needs A (d_in), B (d_aux) and M,N,K");
         if (d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "MM: n_units must be M*N");
         snprintf(name, sizeof name, "xmr_mm_u32_nc%u_inj%d", nc, inj);
-        {   /* tensor-core path (exact, u8 limbs on kind::i8) for tile-aligned problems; COAST_MM_PATH=tiled|naive overrides */
+        {   /* tensor-core path (exact, u8 limbs on wgmma) for tile-aligned problems; COAST_MM_PATH=tiled|naive overrides */
             const char* path = getenv("COAST_MM_PATH");
-            const int want_tc = !path || !strcmp(path, "tc") || !strcmp(path, "tct");
+            const int want_tc = !path || !strcmp(path, "tc");
             if (store_votes) break;                              /* per-k votes on `sum`: the plain kernel (one lane per replica per element) */
             if (want_tc && d->M % 128u == 0 && d->N % 64u == 0 && d->K % 128u == 0 && aligned16 &&
                 !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u))
-                /* measured at 4096^3: A staged in TMEM wins for TMR (1.54 vs 2.45 ms); smem operands win for 1-2 replicas */
-                return launch_mm_tc(d, &a, inj, (CUstream)stream, path ? !strcmp(path, "tct") : nc == 3);
+                return launch_mm_tc(d, &a, inj, (CUstream)stream);
             if (path && !strcmp(path, "naive")) break;
         }
         /* register-tiled fast path: 64 x 128 x 16 tiles, NC x 128 threads (replicas on adjacent warps) */
@@ -969,8 +975,7 @@ static int run_host_staged(const coast_launch_desc* d, uint64_t ib, uint64_t ob,
     const uint64_t ibs = ib ? ib : 1;                          /* divisor of the chunk schedule */
     /* each chunk is its own launch (own tensor map); the fault plan is keyed by the global unit index so
      * chunking never changes results */
-    /* Chunk schedule measured on the B200 box (tools/e2e_chunk_sweep.py): 8-16 MiB chunks stream best (~12 us of driver
-     * work per chunk), but a fixed size leaves the copy engines idle while the first chunk goes up and the last comes
+    /* Chunk schedule (tools/e2e_chunk_sweep.py sweeps it): large chunks amortise the driver work of each chunk, but a fixed size leaves the copy engines idle while the first chunk goes up and the last comes
      * down.  So chunks ramp 1,2,4,8,16,16,... MiB and shrink again towards the end (each at most half of what remains).
      * Chunks are bounded in BYTES: a unit larger than the bound (a long CHStone stream, a long SHA message) is a chunk
      * of its own, so the staging slots never exceed max(16 MiB, one unit) each. */
@@ -1095,13 +1100,13 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
      *   hybrid  : pinned input + a kernel that reads each input byte once: the chunks' kernels read mapped host memory
      *             directly through the TMA ring (no upload copies, no input staging), outputs are staged and downloaded
      *             per chunk;
-     *   zerocopy: ONE launch reads and WRITES mapped host memory.  Measured r02: SM stores of 16-32 bytes per lane to host
-     *             memory lose to the copy engine (profiles/r02_e2e_zero_copy_experiment.md); kept for small calls. */
+     *   zerocopy: ONE launch reads and WRITES mapped host memory: SM stores of 16-32 bytes per lane to host memory
+     *             are small PCIe writes, so it is meant for calls whose output is small. */
     const char* hp = getenv("COAST_HOST_PATH");
     const int streams_once = d->kernel == COAST_K_CRC16 || d->kernel == COAST_K_SHA256 || d->kernel == COAST_K_AES128 ||
                              d->kernel == COAST_K_CHSTONE_SHA || d->kernel == COAST_K_CHSTONE_AES;
-    /* default (measured, profiles/r02_e2e_*.json): staged -- except when the output is tiny next to the input (crc16: 2 of 64 bytes,
-     * CHStone sha: 20 bytes per stream), where one zero-copy launch on pinned buffers beats the chunk pipeline (1.59 vs 2.77 ms) */
+    /* default: staged -- except when the output is tiny next to the input (crc16: 2 of 64 bytes, CHStone sha: 20 bytes per
+     * stream), where one zero-copy launch on pinned buffers reads each input byte once and saves the chunk pipeline's copies */
     const int tiny_out = ob * 8u <= ib;
     const int want = hp ? (!strcmp(hp, "zerocopy") ? 2 : !strcmp(hp, "hybrid") ? 1 : 0) : (tiny_out ? 2 : G.host_path_default);
     CUdeviceptr zin = 0;

@@ -1,6 +1,6 @@
 /*
  * xmr_args.h -- kernel argument block shared by the host runtime (coast_rt.c, plain C)
- * and the sm_100a kernels (coast_kernels.cu).  Plain C layout, no CUDA types.
+ * and the sm_90a kernels (coast_kernels.cu).  Plain C layout, no CUDA types.
  */
 #ifndef XMR_ARGS_H_
 #define XMR_ARGS_H_

@@ -1,4 +1,4 @@
-// xmr_common.cuh -- device-side building blocks of the redundant-execution engine (sm_100a).
+// xmr_common.cuh -- device-side building blocks of the redundant-execution engine (sm_90a).
 //
 //   replica layout : NC (1/2/3) replicas of a unit sit on ADJACENT LANES of one warp
 //                    (lane = NC*u + r).  This is the analogue of cloneInsns putting I.DWC/I.TMR
@@ -193,7 +193,7 @@ struct Tally {
     }
 };
 
-// ---------------------------------------------------------------- mbarrier / TMA (sm_90+ PTX, sm_100a SASS: UTMALDG / SYNCS)
+// ---------------------------------------------------------------- mbarrier / TMA (sm_90 PTX; SASS UTMALDG / SYNCS)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

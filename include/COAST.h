@@ -1,5 +1,5 @@
 /*
- * COAST.h -- the in-code directive surface of COAST, as honoured by the B200 runtime.
+ * COAST.h -- the in-code directive surface of COAST, as honoured by the GPU runtime.
  *
  * Same 17 macro names, same spelling of every annotation string as byuccl/coast
  * tests/COAST.h:11-67 (strings must match projects/dataflowProtection/dataflowProtection.h:69-79),
@@ -21,7 +21,7 @@
  *       - an explicit __xMR on a function with no kernel that calls none FAILS THE BUILD, naming it.
  *     What the directives MEAN for the runtime:
  *
- *   directive                        reference meaning (interface.cpp:364-601)          B200 runtime
+ *   directive                        reference meaning (interface.cpp:364-601)          GPU runtime
  *   -------------------------------  -------------------------------------------------  ---------------------------------
  *   __xMR / __NO_xMR                 put fn/global/local in / out of the SoR            SoR = the offloaded kernel body
  *   __DEFAULT_xMR / __DEFAULT_NO_xMR default scope; both DECLARE an int (:20-21)        same declaration is emitted

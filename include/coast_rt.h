@@ -1,5 +1,5 @@
 /*
- * coast_rt.h -- C ABI of libcoast_rt.so, the B200 redundant-execution runtime.
+ * coast_rt.h -- C ABI of libcoast_rt.so, the H100 redundant-execution runtime.
  *
  * The reference (byuccl/coast) has NO run-time library: `opt -TMR/-DWC` inlines
  * replicas, voters and counters into the program.  The only run-time symbols it
@@ -11,7 +11,7 @@
  *     dataflowProtection::run(M, numClones)   dataflowProtection.cpp:63-164
  *     TMR::runOnModule  -> run(M,3)           projects/TMR/TMR.cpp:29-36
  *     DWC::runOnModule  -> run(M,2)           projects/DWC/DWC.cpp:29-36
- * with a runtime "triplicate-and-vote" launch of a hand-written sm_100a kernel.
+ * with a runtime "triplicate-and-vote" launch of a hand-written sm_90a kernel.
  *
  * Plain C, plain pointers and sizes.  No CUDA / torch types in any signature:
  * device pointers are `void*` (CUdeviceptr-compatible), streams are `void*`
@@ -63,7 +63,7 @@ typedef enum coast_kernel_id {
     COAST_K_AES128    = 2, /* tests/aes/TI_aes_128.c:107-231                   */
     COAST_K_MM_U32    = 3, /* tests/mm_common/mm_common_tmr.c:3-20 (exact, mod 2^32;
                               same low 32 bits as matrixMultiply.c:95-112)      */
-    COAST_K_GEMM_TF32 = 4, /* BASELINE config 4: fp32 in/out, tcgen05 kind::tf32 */
+    COAST_K_GEMM_TF32 = 4, /* BASELINE config 4: fp32 in/out, wgmma tf32 */
     COAST_K_QSORT     = 5, /* tests/quicksort/quicksort.c:121-136 (SURVEY.md 8f-4): data-dependent branches -> the
                               branch conditions are the sync points, voted inside the loops */
     COAST_K_CHSTONE_SHA = 6, /* tests/chstone/sha/sha.c:93-193 (SURVEY.md 8f-4): the CHStone `sha` benchmark -- one unit
@@ -155,7 +155,7 @@ typedef struct coast_fault_plan {
  *                 always the ORIGINAL cipher key, :112-129).
  *   MM_U32   in : A, M x K uint32 row-major; aux: B, K x N uint32 row-major
  *            out: C, M x N uint32; a unit is one C element, n_units must be M*N.  Exact modulo 2^32 on every
- *            path: tcgen05 kind::i8 on u8 limbs when M%128 == N%64 == K%128 == 0 (limb planes are per-launch scratch
+ *            path: wgmma u8 x u8 on u8 limbs when M%128 == N%64 == K%128 == 0 (limb planes are per-launch scratch
  *            from a stream-ordered pool: any number of streams), register-tiled CUDA cores when M%64 == N%128 ==
  *            K%16 == 0, a plain kernel otherwise (e.g. the 9 x 9 tests).  COAST_MM_PATH=tc|tiled|naive overrides.
  *   GEMM_TF32 same with float.
@@ -211,7 +211,7 @@ typedef struct coast_stats {
 #define COAST_ERR_BUSY        (-100005) /* another host thread is inside the library (single caller, see Thread-safety) */
 
 /* --- lifetime ------------------------------------------------------ */
-int  coast_init(int device);          /* bind libcuda, retain device's primary context, load the sm_100a module; moves the
+int  coast_init(int device);          /* bind libcuda, retain device's primary context, load the sm_90a module; moves the
                                          calling thread onto the CPUs of the GPU's NUMA node and prefers that node for its
                                          memory (the host-call path is PCIe-bound); COAST_NUMA_BIND=0 disables that */
 int  coast_numa_node(void);           /* the node coast_init bound to, or -1 */

@@ -477,7 +477,7 @@ uint32_t orc_mm_u32_elem(const uint32_t* A, const uint32_t* B, uint32_t K, uint3
     return sum;
 }
 
-/* BASELINE config 4 (fp32 on tensor cores): tcgen05 kind::tf32 reads the top 19 bits
+/* BASELINE config 4 (fp32 on tensor cores): wgmma tf32 reads the top 19 bits
  * of each fp32 operand; accumulation order inside the tensor core is unspecified, so
  * this is a TOLERANCE oracle (exact products of the truncated operands, summed in
  * double, rounded once). */

@@ -3,7 +3,7 @@
  *
  * TEST INFRASTRUCTURE ONLY (tests/test_host_logic.py builds it into a temp dir and puts that dir on LD_LIBRARY_PATH of a
  * child process).  It executes NO workload: kernels are recorded, not run.  What it does check, the way the real driver
- * would fail: every copy stays inside a live allocation, launch geometry and dynamic shared memory are within sm_100
+ * would fail: every copy stays inside a live allocation, launch geometry and dynamic shared memory are within sm_90
  * limits, tensor maps obey the cuTensorMapEncodeTiled constraints, nothing leaks at exit.  Every call that matters is
  * appended as one JSON line to $MOCK_CUDA_LOG.
  */
@@ -69,9 +69,9 @@ CUresult cuDeviceGet(CUdevice* d, int ord) { if (ord != 0) return CUDA_ERROR_INV
 CUresult cuDeviceGetAttribute(int* v, CUdevice_attribute a, CUdevice d) {
     (void)d;
     switch (a) {
-    case CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MAJOR: *v = getenv("MOCK_CUDA_CC_MAJOR") ? atoi(getenv("MOCK_CUDA_CC_MAJOR")) : 10; break;
+    case CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MAJOR: *v = getenv("MOCK_CUDA_CC_MAJOR") ? atoi(getenv("MOCK_CUDA_CC_MAJOR")) : 9; break;
     case CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MINOR: *v = 0; break;
-    case CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT: *v = 148; break;
+    case CU_DEVICE_ATTRIBUTE_MULTIPROCESSOR_COUNT: *v = 132; break;
     default: *v = 0;
     }
     return CUDA_SUCCESS;

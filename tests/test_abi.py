@@ -30,11 +30,11 @@ def test_library_exports_everything_the_header_declares(built_lib):
     assert C.c_uint64.in_dll(L, "__SYNC_COUNT").value == 0
 
 
-def test_sm100a_cubin_is_embedded(built_lib):
+def test_sm90a_cubin_is_embedded(built_lib):
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")],
                          capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     blob = open(built_lib, "rb").read()
     cubin = open(os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin"), "rb").read()
     assert cubin[:4] == b"\x7fELF" and cubin in blob
@@ -53,7 +53,7 @@ def test_every_kernel_the_host_code_can_name_is_in_the_cubin(built_lib):
     fmts = (fmts - stems) | {s + "_nc%u_inj%d" for s in stems}
     names = set()
     for f in fmts:
-        opts = [["tc", "tct"] if tok == "%s" else ["1", "2", "3"] if tok == "%u" else ["0", "1"] for tok in re.findall(r"%[sud]", f)]
+        opts = [["tc"] if tok == "%s" else ["1", "2", "3"] if tok == "%u" else ["0", "1"] for tok in re.findall(r"%[sud]", f)]
         for combo in itertools.product(*opts):
             it = iter(combo)
             names.add(re.sub(r"%[sud]", lambda m: next(it), f))
@@ -182,18 +182,17 @@ def _sass(fun):
     return subprocess.run(["cuobjdump", "-sass", "-fun", fun, cubin], capture_output=True, text=True, timeout=300).stdout
 
 
-def test_sass_carries_the_blackwell_instructions_the_design_claims(built_lib):
-    """cuobjdump of the embedded sm_100a cubin: tcgen05 MMAs (UTCHMMA / UTCIMMA), TMA loads (UTMALDG), TMEM loads (LDTM); the
-    replicated TF32 MMAs keep A in the collector (A_KEEP / A_REUSE); the CTA-pair kernels issue .2CTA MMAs, .2CTA TMA loads and multicast
-    commits; the headline SHA-256 kernel has no local-memory traffic"""
+def test_sass_carries_the_hopper_instructions_the_design_claims(built_lib):
+    """cuobjdump of the embedded sm_90a cubin: warpgroup MMAs (HGMMA, TF32 and u8), TMA loads (UTMALDG), register reallocation between
+    the producer and consumer warpgroups (USETMAXREG); the CTA-pair kernels multicast B (UTMALDG.2D.MULTICAST) and synchronise the cluster
+    (UCGABAR); the headline SHA-256 kernel has no local-memory traffic"""
     tmr = _sass("xmr_gemm_tf32_nc3_inj0")
-    assert tmr.count("UTCHMMA") >= 12 and "UTMALDG" in tmr and "LDTM" in tmr
-    assert "A_KEEP" in tmr and "A_REUSE" in tmr and ".2CTA" not in tmr
+    assert tmr.count("HGMMA.64x128x8.F32.TF32") >= 12 and "UTMALDG" in tmr and "USETMAXREG" in tmr and "MULTICAST" not in tmr
     pair = _sass("xmr_gemm_tf32p_nc2_inj0")
-    assert "UTCHMMA.2CTA" in pair and "UTMALDG.2D.2CTA" in pair and "UTMALDG.3D.2CTA" in pair and "UTCBAR.2CTA.MULTICAST" in pair
-    assert "UCGABAR_ARV" in pair and "UCGABAR_WAIT" in pair                     # the cluster barrier around TMEM allocation / teardown
+    assert "HGMMA.64x128x8.F32.TF32" in pair and "UTMALDG.2D.MULTICAST" in pair
+    assert "UCGABAR_ARV" in pair and "UCGABAR_WAIT" in pair                     # the cluster barrier around start-up / teardown
     limb = _sass("xmr_mm_u32_tc_nc3_inj0")
-    assert limb.count("UTCIMMA") >= 120 and "A_KEEP" in limb
+    assert limb.count("IGMMA.64x32x32.U8.U8") >= 120
     sha = _sass("xmr_sha256_b64_seg_nc3_inj1")
     assert "UTMALDG" in sha and "STL" not in sha and "LDL" not in sha
     aes = _sass("xmr_aes128_enc_nc2_inj1")

@@ -1,4 +1,4 @@
-"""GPU (B200): seeded differential fuzzing of the whole C ABI against the oracle -- random kernel, clone count, size,
+"""GPU (H100): seeded differential fuzzing of the whole C ABI against the oracle -- random kernel, clone count, size,
 flag combination, fault-plan kind (none / Bernoulli / explicit table with deliberately invalid entries), unit_base.
 Every case must agree bit for bit in output AND counters."""
 import numpy as np

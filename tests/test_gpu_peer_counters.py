@@ -1,4 +1,4 @@
-"""GPU (two B200s of one box): the multi-GPU fold of TMR_ERROR_CNT / __SYNC_COUNT / DWC / injected / first_fault_unit done BY THE
+"""GPU (two H100s of one box): the multi-GPU fold of TMR_ERROR_CNT / __SYNC_COUNT / DWC / injected / first_fault_unit done BY THE
 KERNELS over peer memory (coast_counters_export / _attach, include/coast_rt.h) instead of a collective: a second process on GPU 1
 tallies into GPU 0's counter block, and GPU 0's coast_sync() reads what the oracle counts for the WHOLE unit range."""
 import json
@@ -18,7 +18,7 @@ STAT_KEYS = ("errors_corrected", "dwc_detected", "syncs", "injected", "first_fau
 def test_second_gpu_tallies_into_the_owners_counter_block(rt, oracle, tmp_path, nc):
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs of one box (gpurun --gpus 2)")
+        pytest.skip("needs two GPUs of one box")
     n, half, seed, threshold = 6000, 2500, 5, 2 ** 32 // 40
     m = oracle.fill_philox(n * 16, 0, 9).view(np.uint8).copy()
     oplan = oracle.make_plan(oracle.PLAN_BERNOULLI, seed=seed, threshold=threshold)

@@ -1,8 +1,8 @@
 """Host logic of libcoast_rt.so (coast_b200/csrc/coast_rt.c) on a GPU-less box, against a MOCK driver
 (tests/mock_cuda/mock_cuda.c, test infrastructure: it runs no workload, it records and bounds-checks driver calls):
-launch geometry and shared memory within sm_100 limits, tensor maps inside the caller's buffers, the argument block every
+launch geometry and shared memory within sm_90 limits, tensor maps inside the caller's buffers, the argument block every
 kernel receives, the chunk schedule of coast_run_host() (every byte copied exactly once, per-chunk unit_base), scratch and
-staging memory released, loud failures for bad arguments and for a non-sm_100 device."""
+staging memory released, loud failures for bad arguments and for a non-sm_90 device."""
 import ctypes as C
 import json
 import os
@@ -78,11 +78,11 @@ def test_launch_geometry_and_argument_block(mock_dir, tmp_path, kernel, nc, n, u
     assert len(launches) == 1
     la = launches[0]
     name, block, tile_rows = want
-    assert la["name"] == name and la["block"] == block and la["smem"] <= 232448 and 1 <= la["grid"] <= 148 * 32 * 4
+    assert la["name"] == name and la["block"] == block and la["smem"] <= 232448 and 1 <= la["grid"] <= 132 * 32 * 4
     a = args_of(la)
     assert a.n_units == n and a.unit_base == 0 and a.unit_bytes == ub and a.flags == 3 and a.plan_mode == 0
     if tile_rows:                                           # TMA-tiled kernels: one tensor map over exactly the caller's rows
-        assert a.n_tiles == -(-n // tile_rows) and la["grid"] <= 148 * 8
+        assert a.n_tiles == -(-n // tile_rows) and la["grid"] <= 132 * 8
         tm = [e for e in ev if e["op"] == "tmap"]
         pack = tm[0]["dim0"] * 4 // (16 if kernel == K_AES128 else ub)      # AES: the same dense bytes as 64- or 256-byte rows
         assert (pack == 16 and (a.mode >> 8) & 15 == 4) if kernel == K_AES128 else pack == 1
@@ -150,13 +150,13 @@ def test_unaligned_sha_input_takes_the_general_kernel(mock_dir, tmp_path):
     assert not [e for e in ev if e["op"] == "tmap"]
 
 
-def test_a_device_that_is_not_sm100_is_refused(mock_dir, tmp_path):
-    res, ev = run_child(mock_dir, tmp_path, [], env_extra={"MOCK_CUDA_CC_MAJOR": "9"})
-    assert res["init"] != 0 and "sm_100a code only" in res["error"]
+def test_a_device_that_is_not_sm90_is_refused(mock_dir, tmp_path):
+    res, ev = run_child(mock_dir, tmp_path, [], env_extra={"MOCK_CUDA_CC_MAJOR": "10"})
+    assert res["init"] != 0 and "sm_90a code only" in res["error"]
 
 
 @pytest.mark.parametrize("M,N,K,nc,env,want", [
-    (256, 128, 256, 3, {}, ["xmr_mm_split_a", "xmr_mm_split_bt", "xmr_mm_u32_tct_nc3_inj0"]),       # TMR: A limb planes staged in TMEM
+    (256, 128, 256, 3, {}, ["xmr_mm_split_a", "xmr_mm_split_bt", "xmr_mm_u32_tc_nc3_inj0"]),
     (256, 128, 256, 2, {}, ["xmr_mm_split_a", "xmr_mm_split_bt", "xmr_mm_u32_tc_nc2_inj0"]),
     (256, 128, 256, 3, {"COAST_MM_PATH": "tiled"}, ["xmr_mm_u32_tiled_nc3_inj0"]),
     (64, 128, 48, 3, {}, ["xmr_mm_u32_tiled_nc3_inj0"]),                                              # not 128/64/128-aligned
@@ -173,7 +173,7 @@ def test_exact_matmul_path_selection_and_tensor_maps(mock_dir, tmp_path, M, N, K
         tm = [e for e in ev if e["op"] == "tmap"]
         assert len(tm) == 2 and all(t["elem"] == 1 and t["rank"] == 3 and t["box0"] == 128 for t in tm)   # u8 limb planes, 128-byte k rows
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]][0]
-    assert la["smem"] <= 232448 and la["grid"] <= max(148, (M // 64) * (N // 128))
+    assert la["smem"] <= 232448 and la["grid"] <= max(132, (M // 64) * (N // 128))
     assert ev[-1] == {"op": "exit", "live_allocations": 0}
 
 
@@ -185,7 +185,8 @@ def test_tf32_gemm_launch(mock_dir, tmp_path):
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]][0]
     assert la["name"] == "xmr_gemm_tf32_nc3_inj0" and la["block"] == 384 and la["grid"] == 16 and la["smem"] <= 232448
     tm = [e for e in ev if e["op"] == "tmap"]
-    assert [t["rank"] for t in tm] == [2, 3] and tm[1]["swizzle"] != tm[0]["swizzle"]      # B: the 32-byte-atom swizzle of the MN-major operand
+    assert [t["rank"] for t in tm] == [2, 2] and tm[1]["swizzle"] == tm[0]["swizzle"]      # A and B^T: both K-major, 128-byte swizzle
+    assert [e["name"] for e in ev if e["op"] == "launch" and e["name"] != "xmr_counters_reset"][0] == "xmr_gemm_bt"   # B transposed first
     bad, _ = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=3, n=100 * 128, M=100, N=128, K=64, in_bytes=100 * 64 * 4,
                                                   aux_bytes=64 * 128 * 4, out_bytes=100 * 128 * 4)])
     assert bad["ops"][0]["rc"] != 0 and "multiples of 128" in bad["ops"][0]["err"]
@@ -217,20 +218,19 @@ def test_tf32_gemm_kernel_selection_pairs_and_single(mock_dir, tmp_path, nc, M, 
 
 
 def test_gemm_tuning_switches_reach_the_kernel_as_mode_bits(mock_dir, tmp_path):
-    """COAST_GEMM_GROUP_M / _L2_HINTS / _TAIL_SPLIT / _KEEP_A (TF32) and COAST_MM_KEEP_A (integer limb kernel) are read per launch and
-    travel in xmr_args.mode: bits 0-7 group, 0x100 hints on, 0x200 tail split off, 0x400 collector reuse off"""
+    """COAST_GEMM_GROUP_M / _L2_HINTS / _TAIL_SPLIT (TF32) are read per launch and travel in xmr_args.mode: bits 0-7 group,
+    0x100 hints on, 0x200 tail split off; the integer limb kernel has no mode bits"""
     s = 512
     gemm = dict(op="launch", kernel=K_GEMM_TF32, nc=3, n=s * s, M=s, N=s, K=64, in_bytes=s * 64 * 4, aux_bytes=64 * s * 4, out_bytes=s * s * 4, flags=3)
     mm = dict(op="launch", kernel=K_MM_U32, nc=3, n=s * s, M=s, N=s, K=128, in_bytes=s * 128 * 4, aux_bytes=128 * s * 4, out_bytes=s * s * 4, flags=3)
     res, ev = run_child(mock_dir, tmp_path, [gemm, mm], env_extra={"COAST_MM_PATH": "tc"})
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert [x["name"] for x in la] == ["xmr_gemm_tf32_nc3_inj0", "xmr_mm_u32_tc_nc3_inj0"]
-    assert args_of(la[0]).mode == 0x100 and args_of(la[1]).mode & 0x400 == 0
-    env = {"COAST_GEMM_GROUP_M": "8", "COAST_GEMM_L2_HINTS": "0", "COAST_GEMM_TAIL_SPLIT": "0", "COAST_GEMM_KEEP_A": "0", "COAST_MM_KEEP_A": "0",
-           "COAST_MM_PATH": "tc"}
+    assert args_of(la[0]).mode == 0x100 and args_of(la[1]).mode == 0
+    env = {"COAST_GEMM_GROUP_M": "8", "COAST_GEMM_L2_HINTS": "0", "COAST_GEMM_TAIL_SPLIT": "0", "COAST_MM_PATH": "tc"}
     res, ev = run_child(mock_dir, tmp_path, [gemm, mm], env_extra=env)
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
-    assert args_of(la[0]).mode == 8 | 0x200 | 0x400 and args_of(la[1]).mode & 0x400
+    assert args_of(la[0]).mode == 8 | 0x200 and args_of(la[1]).mode == 0
 
 
 def test_quicksort_through_the_host_call_uses_one_scratch_slot_per_chunk(mock_dir, tmp_path):

@@ -5,6 +5,7 @@ function on the CPU, and an explicit __xMR that cannot be honoured fails the bui
 The programs below are this repo's own (written for the test), built in a temp directory with the same Makefile contract
 as the reference's test directories.  No GPU: the cases that run a binary are the ones whose protected region stays on the CPU."""
 import os
+import tempfile
 import re
 import subprocess
 
@@ -90,7 +91,7 @@ def test_an_xmr_wrapper_around_a_kernel_entry_is_accepted_and_reported(tmp_path,
 
 
 def scan(src):
-    tool = "/tmp/coast_scope_test"
+    tool = os.path.join(tempfile.mkdtemp(), "coast_scope")
     subprocess.run(["gcc", "-O1", "-o", tool, os.path.join(LEVEL, "makefiles", "coast_scope.c")], check=True)
     pre = subprocess.run(["gcc", "-E", "-w", "-DCOAST_SCOPE_SCAN", "-include", os.path.join(LEVEL, "coast_shim.h"), "-I", LEVEL, "-x", "c", "-"],
                          input=src, capture_output=True, text=True, check=True).stdout
