@@ -8,7 +8,7 @@ pytestmark = pytest.mark.gpu
 
 
 def _case(rng, oracle):
-    k = int(rng.integers(0, 5))
+    k = int(rng.integers(0, 8))
     nc = int(rng.integers(1, 4))
     flags = int(rng.choice([0, 1, 3, 3 | 0x100, 3 | 0x8, 3 | 0x10, 0x20 & 0]))
     kw = {}
@@ -32,6 +32,26 @@ def _case(rng, oracle):
         n = M * N
         kernel, inp = oracle.K_MM_U32, rng.integers(0, 2 ** 32, M * K, dtype=np.uint64).astype(np.uint32)
         kw = dict(M=M, N=N, K=K, aux=rng.integers(0, 2 ** 32, K * N, dtype=np.uint64).astype(np.uint32))
+    elif k == 5:    # TF32 GEMM on integer operands: exact, so bit-exact with the oracle (test_gpu_wgmma_exact.py)
+        M, N, K = [(128, 128, 32), (128, 256, 64), (256, 128, 96), (256, 256, 32), (128, 384, 224), (256, 512, 64)][int(rng.integers(0, 6))]
+        n = M * N
+        amax = int(rng.choice([1, 8, 64]))
+        kernel = oracle.K_GEMM_TF32
+        inp = rng.integers(-amax, amax + 1, M * K).astype(np.float32)
+        kw = dict(M=M, N=N, K=K, aux=rng.integers(-amax, amax + 1, K * N).astype(np.float32))
+    elif k == 6:    # CHStone sha: whole 64-byte blocks
+        L = 64 * int(rng.integers(1, 17))
+        n = int(rng.integers(1, 120))
+        kernel, inp, kw = oracle.K_CHSTONE_SHA, rng.integers(0, 256, n * L, dtype=np.uint8), dict(unit_bytes=L)
+    elif k == 7:    # CHStone aes: one int per state byte; per-unit keys (mode 2 | dec) or one shared key
+        n = int(rng.integers(1, 1500))
+        mode = int(rng.choice([0, 1, 2, 3]))
+        kernel, inp = oracle.K_CHSTONE_AES, rng.integers(0, 256, n * 16).astype(np.int32)
+        kw = dict(mode=mode)
+        if mode & 2:
+            kw["aux"] = rng.integers(0, 256, n * 16).astype(np.int32)
+        else:
+            kw["key"] = bytes(rng.integers(0, 256, 16, dtype=np.uint8))
     else:           # quicksort
         L = int(rng.choice([1, 2, 3, 16, 100, 580]))
         n = int(rng.integers(1, 120))

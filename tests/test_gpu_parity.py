@@ -547,9 +547,11 @@ def test_mm_tiled_kernel_exact_and_faults(rt, oracle, nc, M, N, K):
 
 def test_mm_full_size_properties(rt, oracle):
     """4096^3 exact integer TMR (the reference's own arithmetic at BASELINE config-4 size): voted output == unprotected output
-    bit for bit under a fault plan; spot elements equal the oracle's dot products; XOR-fold check as mm_common_tmr.c:23-32."""
+    bit for bit under a fault plan; every element equals the exact mod-2^32 product (mm_u32_ref, fp64 on 16-bit limbs on the
+    device); XOR-fold check as mm_common_tmr.c:23-32."""
     import torch
     import coast_b200 as cb
+    from test_gpu_wgmma_exact import mm_u32_ref
     n = 4096
     A = torch.empty(n * n, dtype=torch.int32, device="cuda")
     B = torch.empty(n * n, dtype=torch.int32, device="cuda")
@@ -560,15 +562,9 @@ def test_mm_full_size_properties(rt, oracle):
     rt.run(cb.K_MM_U32, 1, A, n * n, M=n, N=n, K=n, aux=B, out=o1)
     _, st = rt.run(cb.K_MM_U32, 3, A, n * n, M=n, N=n, K=n, aux=B, flags=3, out=o3, plan=cb.FaultPlan(mode=cb.PLAN_BERNOULLI, seed=8, p=2 ** -12))
     assert torch.equal(o1, o3) and st.errors_corrected == st.injected > 3000
-    hA = oracle.fill_philox(n * n, 0, 4)
-    hB = oracle.fill_philox(n * n, 0, 44)
-    C = o3.cpu().numpy().view(np.uint32).reshape(n, n)
-    for (i, j) in [(0, 0), (1, 4095), (2047, 1234), (4095, 4095), (63, 64), (64, 127)]:
-        ref = int(np.sum(hA[i * n:(i + 1) * n].astype(np.uint64) * hB[j::n].astype(np.uint64)) & np.uint64(0xFFFFFFFF)) & 0xFFFFFFFF
-        exact = 0
-        for k in range(n):
-            exact = (exact + int(hA[i * n + k]) * int(hB[k * n + j])) & 0xFFFFFFFF
-        assert int(C[i, j]) == exact
+    assert torch.equal(o3.view(n, n).to(torch.int64) & 0xFFFFFFFF, mm_u32_ref(A.view(n, n), B.view(n, n)))
+    assert (A.cpu().numpy().view(np.uint32) == oracle.fill_philox(n * n, 0, 4)).all()      # the device fill is the oracle's
+    C = o3.cpu().numpy().view(np.uint32)
     assert int(np.bitwise_xor.reduce(C.ravel())) == int(np.bitwise_xor.reduce(o1.cpu().numpy().view(np.uint32)))
 
 
