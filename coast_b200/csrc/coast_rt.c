@@ -14,6 +14,7 @@
 #define _GNU_SOURCE
 #include "../../include/coast_rt.h"
 #include "xmr_args.h"
+#include "xmr_geom.h"
 
 #include <cuda.h>
 #include <ctype.h>
@@ -90,6 +91,19 @@ __attribute__((weak)) void FAULT_DETECTED_DWC(void) { /* synchronization.cpp:125
 DRV_FUNCS(X)
 #undef X
 
+/* A tiled tensor map as the launch wants it.  `base` is an offset into the launch's scratch when in_scratch is set.
+ * No padding: the map cache compares descriptions with memcmp. */
+typedef struct {
+    uintptr_t base;
+    cuuint64_t dim[3], stride[2];
+    cuuint32_t box[3], rank;
+    CUtensorMapDataType dtype;
+    CUtensorMapSwizzle swz;
+    CUtensorMapL2promotion l2;
+    int in_scratch;
+} map_desc;
+_Static_assert(sizeof(map_desc) == 80, "map_desc has no padding");
+
 #define MAX_FN 128
 static struct {
     int inited;
@@ -115,9 +129,8 @@ static struct {
     CUdeviceptr h_b; size_t h_b_cap; CUevent ev_b;   /* matmul host call: the replicated operand B and "B has landed" */
     int numa_node;                   /* NUMA node the process was bound to by coast_init (-1: not bound) */
     int busy;                        /* one host thread at a time (the reference is single-threaded); others fail loudly */
-    /* tensor maps of the row-tiled kernels, keyed by (base, row bytes, rows, box rows, swizzle): coast_run_host re-encodes the
-     * same few maps every call */
-    struct { const void* base; uint32_t row_bytes, box_rows; uint64_t rows; int swz; CUtensorMap map; } tmaps[16];
+    /* tensor maps of the row-tiled kernels: coast_run_host re-encodes the same few maps every call */
+    struct { map_desc key; CUtensorMap map; } tmaps[16];
     int n_tmaps, tmap_next;
     unsigned warned_store_votes;     /* one warning per kernel and process */
     int host_path_default;           /* host-call path for pinned buffers: 0 = staged, 1 = hybrid, 2 = zero-copy */
@@ -229,7 +242,7 @@ static int ensure_ctx(void) {
     return COAST_OK;
 }
 
-static int get_fn_b(const char* name, unsigned smem, int block, CUfunction* fn, int* ctas_per_sm) {
+static int get_fn(const char* name, unsigned smem, unsigned block, CUfunction* fn, int* ctas_per_sm) {
     for (int i = 0; i < G.n_fns; ++i)
         if (!strcmp(G.fns[i].name, name) && G.fns[i].smem == smem) { *fn = G.fns[i].fn; if (ctas_per_sm) *ctas_per_sm = G.fns[i].ctas_per_sm; return COAST_OK; }
     CUfunction f = NULL;
@@ -237,7 +250,7 @@ static int get_fn_b(const char* name, unsigned smem, int block, CUfunction* fn, 
     if (r != CUDA_SUCCESS) return drv_fail(r, name);
     if (smem > 48 * 1024) DRV(p_cuFuncSetAttribute(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem));
     int occ = 1;
-    DRV(p_cuOccupancyMaxActiveBlocksPerMultiprocessor(&occ, f, block, smem));
+    DRV(p_cuOccupancyMaxActiveBlocksPerMultiprocessor(&occ, f, (int)block, smem));
     if (occ < 1) occ = 1;
     if (G.n_fns < MAX_FN) {
         snprintf(G.fns[G.n_fns].name, sizeof G.fns[0].name, "%s", name);
@@ -248,12 +261,8 @@ static int get_fn_b(const char* name, unsigned smem, int block, CUfunction* fn, 
     return COAST_OK;
 }
 
-static int get_fn(const char* name, unsigned smem, CUfunction* fn, int* ctas_per_sm) {
-    return get_fn_b(name, smem, XMR_CTA_THREADS, fn, ctas_per_sm);
-}
-
 static int launch_small(const char* name, unsigned grid, unsigned block, void** params, CUstream s) {
-    CUfunction f; int rc = get_fn(name, 0, &f, NULL);
+    CUfunction f; int rc = get_fn(name, 0, block, &f, NULL);
     if (rc) return rc;
     DRV(p_cuLaunchKernel(f, grid, 1, 1, block, 1, 1, 0, s, params, NULL));
     return COAST_OK;
@@ -377,10 +386,33 @@ int coast_parse_opt_passes(const char* s, uint32_t* num_clones, uint32_t* flags)
     return COAST_OK;
 }
 
+/* ------------------------------------------------------------------ */
+/* per-kernel facts                                                     */
+/* ------------------------------------------------------------------ */
+#define IN_UNIT_BYTES 0xFFFFFFFFu           /* kernel_info.in_bytes: the descriptor's unit_bytes */
+static const struct kernel_info {
+    const char* name;                       /* in messages */
+    uint32_t out_bytes;                     /* per unit; QSORT: 0, the output is the unit's array */
+    uint32_t votes;                         /* SoR-exit votes per unit */
+    uint32_t in_bytes;                      /* per unit, staged by the host call; 0: the matmuls (operands, not units) */
+    uint32_t key_bytes;                     /* per-unit key bytes with COAST_AES_KEY_PER_UNIT */
+    int store_votes;                        /* in-loop store votes are built (coast_rt.h) */
+    int streams_once;                       /* reads each input byte once: may read mapped host memory directly */
+} KINFO[COAST_K_COUNT_] = {
+    [COAST_K_CRC16]       = { "crc16",       2,  1,  IN_UNIT_BYTES, 0,  1, 1 },
+    [COAST_K_SHA256]      = { "sha256",      32, 32, IN_UNIT_BYTES, 0,  1, 1 },
+    [COAST_K_AES128]      = { "aes128",      16, 16, 16,            16, 0, 1 },
+    [COAST_K_MM_U32]      = { "mm_u32",      4,  1,  0,             0,  1, 0 },
+    [COAST_K_GEMM_TF32]   = { "gemm_tf32",   4,  1,  0,             0,  0, 0 },
+    [COAST_K_QSORT]       = { "qsort",       0,  0,  IN_UNIT_BYTES, 0,  0, 0 },
+    [COAST_K_CHSTONE_SHA] = { "chstone_sha", 20, 5,  IN_UNIT_BYTES, 0,  0, 1 },
+    [COAST_K_CHSTONE_AES] = { "chstone_aes", 64, 16, 64,            64, 0, 1 },
+};
+
 static int store_votes_wanted(uint32_t fl) {
     return (fl & (COAST_F_STORE_DATA_SYNC | COAST_F_NO_MEM_REPLICATION)) && !(fl & COAST_F_NO_STORE_DATA_SYNC);
 }
-static int store_votes_built(uint32_t kernel) { return kernel == COAST_K_CRC16 || kernel == COAST_K_MM_U32 || kernel == COAST_K_SHA256; }
+static int store_votes_built(uint32_t kernel) { return kernel < COAST_K_COUNT_ && KINFO[kernel].store_votes; }
 
 uint32_t coast_flags_honoured(uint32_t kernel, uint32_t nc, uint32_t fl) {
     uint32_t h = fl & (COAST_F_COUNT_ERRORS | COAST_F_COUNT_SYNCS | COAST_F_VERBOSE | COAST_F_MAJORITY_VOTER);
@@ -426,193 +458,123 @@ uint32_t coast_fault_site_bits(uint32_t kernel, uint32_t unit_bytes, uint32_t K,
     if (kernel == COAST_K_AES128 || kernel == COAST_K_CHSTONE_AES) return 8u;
     return 32u;
 }
-uint32_t coast_out_bytes_per_unit(uint32_t kernel) {
-    static const uint32_t ob[COAST_K_COUNT_] = { 2, 32, 16, 4, 4, 0, 20, 64 };
-    return kernel < COAST_K_COUNT_ ? ob[kernel] : 0;
-}
-uint32_t coast_votes_per_unit(uint32_t kernel) {
-    static const uint32_t nv[COAST_K_COUNT_] = { 1, 32, 16, 1, 1, 0, 5, 16 };
-    return kernel < COAST_K_COUNT_ ? nv[kernel] : 0;
-}
+uint32_t coast_out_bytes_per_unit(uint32_t kernel) { return kernel < COAST_K_COUNT_ ? KINFO[kernel].out_bytes : 0; }
+uint32_t coast_votes_per_unit(uint32_t kernel) { return kernel < COAST_K_COUNT_ ? KINFO[kernel].votes : 0; }
 uint32_t coast_out_bytes(uint32_t kernel, uint32_t unit_bytes) {
     return kernel == COAST_K_QSORT ? unit_bytes : coast_out_bytes_per_unit(kernel);
 }
 static uint64_t in_bytes_per_unit(const coast_launch_desc* d) {
-    switch (d->kernel) {
-    case COAST_K_CRC16: case COAST_K_SHA256: case COAST_K_QSORT: case COAST_K_CHSTONE_SHA: return d->unit_bytes;
-    case COAST_K_AES128: return 16;
-    case COAST_K_CHSTONE_AES: return 64;
-    default: return 0;
-    }
+    if (d->kernel >= COAST_K_COUNT_) return 0;
+    return KINFO[d->kernel].in_bytes == IN_UNIT_BYTES ? d->unit_bytes : KINFO[d->kernel].in_bytes;
 }
 /* bytes of per-unit aux data the host call stages next to the input (AES keys) */
 static uint64_t aux_bytes_per_unit(const coast_launch_desc* d) {
-    if (!(d->mode & COAST_AES_KEY_PER_UNIT)) return 0;
-    return d->kernel == COAST_K_AES128 ? 16 : d->kernel == COAST_K_CHSTONE_AES ? 64 : 0;
+    return d->kernel < COAST_K_COUNT_ && (d->mode & COAST_AES_KEY_PER_UNIT) ? KINFO[d->kernel].key_bytes : 0;
 }
 
 /* ------------------------------------------------------------------ */
 /* the launch                                                           */
 /* ------------------------------------------------------------------ */
-static unsigned ring_smem(unsigned tile_rows, unsigned row_bytes) {
-    unsigned tile = tile_rows * row_bytes;
-    unsigned stride = (tile + 1023u) & ~1023u;
-    return XMR_STAGES * stride + 64u;
-}
-
-static int encode_rows_map_uncached(CUtensorMap* map, const void* base, uint32_t row_bytes, uint64_t rows, uint32_t box_rows,
-                                    CUtensorMapSwizzle swz) {
-    cuuint64_t gdim[2] = { row_bytes / 4u, rows };
-    cuuint64_t gstr[1] = { row_bytes };
-    cuuint32_t box[2] = { row_bytes / 4u, box_rows };
-    cuuint32_t estr[2] = { 1, 1 };
-    DRV(p_cuTensorMapEncodeTiled(map, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void*)base, gdim, gstr, box, estr,
-                                 CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
+/* A tensor map is a pure function of its description.  The host-call path re-creates the same handful of row maps every call,
+ * so `cached` maps are looked up among the last 16 (round-robin replacement). */
+static int encode_map(const map_desc* want, CUdeviceptr scratch, int cached, CUtensorMap* map) {
+    map_desc m = *want;
+    if (m.in_scratch) { m.base += scratch; m.in_scratch = 0; }
+    if (cached)
+        for (int i = 0; i < G.n_tmaps; ++i)
+            if (!memcmp(&G.tmaps[i].key, &m, sizeof m)) { *map = G.tmaps[i].map; return COAST_OK; }
+    static const cuuint32_t estr[3] = { 1, 1, 1 };
+    DRV(p_cuTensorMapEncodeTiled(map, m.dtype, m.rank, (void*)m.base, m.dim, m.stride, m.box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                 m.swz, m.l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
+    if (cached) {
+        const int n_slots = (int)(sizeof G.tmaps / sizeof G.tmaps[0]);
+        int k = G.n_tmaps < n_slots ? G.n_tmaps++ : (G.tmap_next++ % n_slots);
+        G.tmaps[k].key = m; G.tmaps[k].map = *map;
+    }
     return COAST_OK;
 }
 
-/* A tensor map is a pure function of (base, geometry); the host-call path re-creates the same handful every call, so the
- * last 16 are kept (round-robin replacement). */
-static int encode_rows_map(CUtensorMap* map, const void* base, uint32_t row_bytes, uint64_t rows, uint32_t box_rows,
-                           CUtensorMapSwizzle swz) {
-    for (int i = 0; i < G.n_tmaps; ++i)
-        if (G.tmaps[i].base == base && G.tmaps[i].rows == rows && G.tmaps[i].row_bytes == row_bytes &&
-            G.tmaps[i].box_rows == box_rows && G.tmaps[i].swz == (int)swz) { *map = G.tmaps[i].map; return COAST_OK; }
-    int rc = encode_rows_map_uncached(map, base, row_bytes, rows, box_rows, swz); if (rc) return rc;
-    const int n_slots = (int)(sizeof G.tmaps / sizeof G.tmaps[0]);
-    int k = G.n_tmaps < n_slots ? G.n_tmaps++ : (G.tmap_next++ % n_slots);
-    G.tmaps[k].base = base; G.tmaps[k].rows = rows; G.tmaps[k].row_bytes = row_bytes; G.tmaps[k].box_rows = box_rows;
-    G.tmaps[k].swz = (int)swz; G.tmaps[k].map = *map;
-    return COAST_OK;
-}
-
-/* TF32 GEMM on wgmma (xmr_gemm_tf32.cuh): B (row-major K x N) is transposed into stream-ordered scratch first, because TF32
- * wgmma reads both operands K-major; A and B^T then go through 2-D maps with the 128-byte swizzle (box 32 k x 128 rows; the
- * CTA-pair kernels load B^T in 64-row boxes, half of a 128-column block per CTA, multicast to both).
- * Tile geometry mirrors xmr::gemm::Geom<NC>: unprotected 128 x 256 tiles on 4 stages, DWC/TMR 128 x 128 on 6 stages. */
-static int launch_gemm_tf32_bt(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream, CUdeviceptr bt) {
+/* What kernel selection decides about a launch; run_plan() does the rest. */
+typedef struct {
     char name[64];
-    const int wide = d->num_clones == 1 && d->N % 256u == 0;
-    if (d->num_clones == 1 && !wide) snprintf(name, sizeof name, "xmr_gemm_tf32n_nc1_inj%d", inj);
-    else snprintf(name, sizeof name, "xmr_gemm_tf32_nc%u_inj%d", d->num_clones, inj);
-    unsigned bn = wide ? 256u : 128u, stages = wide ? 4u : 6u;
-    /* CTA-pair kernels (cluster 2 x 1 x 1, 256 x BN pair tiles, B multicast): bit-identical to the single-CTA kernels.  Default:
-     * pairs for the unprotected and DWC kernels when the shape allows (M % 256, N % BN), the single-CTA kernel for TMR;
-     * COAST_GEMM_PAIR=0 / 1 forces one or the other for every replica count. */
-    unsigned b_box = 128u;
-    int pair = 0;
-    { const char* e = getenv("COAST_GEMM_PAIR");
-      const unsigned pbn = d->num_clones == 1 ? 256u : 128u;
-      const int want = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : d->num_clones < 3;
-      if (want && d->M % 256u == 0 && d->N % pbn == 0 && G.sm_count >= 2) {
-          pair = 1; bn = pbn; stages = d->num_clones == 1 ? 4u : 6u; b_box = 64u;
-          snprintf(name, sizeof name, "xmr_gemm_tf32p_nc%u_inj%d", d->num_clones, inj);
-      } }
-    const unsigned GEMM_SMEM = stages * (16384u + 32u * bn * 4u) + 1024u + 256u;
-    { const char* g = getenv("COAST_GEMM_GROUP_M"); if (g && atoi(g) > 0 && atoi(g) < 256) a->mode = (a->mode & ~0xFFu) | (unsigned)atoi(g); }
-    /* L2 eviction priorities: A evict_last, B and C evict_first; COAST_GEMM_L2_HINTS=0 loads and stores with the normal policy */
-    { const char* h = getenv("COAST_GEMM_L2_HINTS"); if (!(h && !strcmp(h, "0"))) a->mode |= 0x100u; }
-    /* the unprotected kernel halves the tiles of a short last round (xmr_gemm_tf32.cuh); COAST_GEMM_TAIL_SPLIT=0 keeps whole tiles */
-    { const char* h = getenv("COAST_GEMM_TAIL_SPLIT"); if (h && !strcmp(h, "0")) a->mode |= 0x200u; }
-    CUfunction fn; int occ = 1;
-    int rc = get_fn("xmr_gemm_bt", 0, &fn, NULL); if (rc) return rc;
-    {
-        const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N;
-        void* params[] = { &B, &bt, &k32, &n32 };
-        DRV(p_cuLaunchKernel(fn, (unsigned)G.sm_count * 8u, 1, 1, 256, 1, 1, 0, stream, params, NULL));
-    }
-    rc = get_fn(name, GEMM_SMEM, &fn, &occ); if (rc) return rc;
-    CUtensorMap ma, mb;
-    {
-        cuuint64_t gdim[2] = { d->K, d->M };
-        cuuint64_t gstr[1] = { (cuuint64_t)d->K * 4u };
-        cuuint32_t box[2] = { 32, 128 };
-        cuuint32_t estr[2] = { 1, 1 };
-        DRV(p_cuTensorMapEncodeTiled(&ma, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)d->d_in, gdim, gstr, box, estr,
-                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
-    }
-    {
-        cuuint64_t gdim[2] = { d->K, d->N };
-        cuuint64_t gstr[1] = { (cuuint64_t)d->K * 4u };
-        cuuint32_t box[2] = { 32, b_box };
-        cuuint32_t estr[2] = { 1, 1 };
-        DRV(p_cuTensorMapEncodeTiled(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)bt, gdim, gstr, box, estr,
-                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
-    }
-    unsigned tiles = (d->M / 128u) * (d->N / bn);           /* pair kernels: CTAs = 2 x pair tiles, an even grid (cluster 2 x 1 x 1) */
-    unsigned grid = tiles < (unsigned)G.sm_count ? tiles : (unsigned)G.sm_count;
-    if (pair) grid &= ~1u;
-    void* params[3] = { a, &ma, &mb };
-    if (d->flags & COAST_F_VERBOSE) fprintf(stderr, "coast_rt: %s grid=%u smem=%u tiles=%u\n", name, grid, GEMM_SMEM, tiles);
-    DRV(p_cuLaunchKernel(fn, grid, 1, 1, 384, 1, 1, GEMM_SMEM, stream, params, NULL));
-    return COAST_OK;
-}
-/* B^T is per-launch scratch from the stream-ordered pool, like the limb planes below */
-static int launch_gemm_tf32(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream) {
-    CUdeviceptr bt = 0;
-    DRV(p_cuMemAllocFromPoolAsync(&bt, (size_t)d->K * d->N * 4u, G.pool, stream));
-    int rc = launch_gemm_tf32_bt(d, a, inj, stream, bt);
-    p_cuMemFreeAsync(bt, stream);
-    return rc;
+    unsigned block, smem;
+    uint64_t ctas;                /* CTAs the work needs (0: one warp per 32/nc units, the lane-interleaved kernels) */
+    unsigned waves;               /* the grid is at most this many waves of resident CTAs; 0: all ctas */
+    unsigned cluster;             /* CTAs per cluster: the grid is a multiple of it */
+    int n_maps, cache_maps;       /* tensor maps: kernel parameters 2 and 3 */
+    map_desc map[2];
+    size_t scratch;               /* stream-ordered scratch for the pre-pass and the maps */
+    size_t scratch_per_cta;       /* plus this much per CTA of the grid, handed to the kernel as xmr_args.aux */
+    int (*prepass)(const coast_launch_desc* d, CUdeviceptr scratch, CUstream s);
+} launch_plan;
+
+/* The TMA-ring kernels: tiles of tile_rows units of row_bytes each, loaded as equal boxes of at most 256 rows.  With a row
+ * pack shift p the same dense bytes are described as rows 2^p times longer. */
+static void plan_ring(launch_plan* L, xmr_args* a, unsigned tile_rows, unsigned row_bytes, unsigned pack, CUtensorMapSwizzle swz) {
+    L->ctas = (a->n_units + tile_rows - 1) / tile_rows;
+    L->waves = 1;
+    a->n_tiles = (unsigned)L->ctas;
+    L->n_maps = 1; L->cache_maps = 1;
+    map_desc* m = &L->map[0];
+    m->dtype = CU_TENSOR_MAP_DATA_TYPE_UINT32; m->rank = 2; m->base = (uintptr_t)a->in;
+    m->dim[0] = m->box[0] = (row_bytes << pack) / 4u;
+    m->dim[1] = a->n_units >> pack;
+    m->stride[0] = row_bytes << pack;
+    m->box[1] = (tile_rows / xmr_ring_loads(tile_rows)) >> pack;
+    m->swz = swz; m->l2 = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
 }
 
-/* Exact integer matmul on wgmma u8 (xmr_mm_tc.cuh): split A and B into u8 limb planes (library scratch),
- * then ten u8 GEMMs per replica into four s32 register accumulators, recombined modulo 2^32 in the epilogue. */
-static int launch_mm_tc_planes(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream, CUdeviceptr pa, CUdeviceptr pb) {
-    const uint32_t nc = d->num_clones, bn = nc == 1 ? 64u : 32u;
-    {
-        CUfunction f; int rc = get_fn("xmr_mm_split_a", 0, &f, NULL); if (rc) return rc;
-        unsigned long long rows = d->M, K = d->K; const void* A = d->d_in;
-        void* params[] = { &A, &pa, &rows, &K };
-        DRV(p_cuLaunchKernel(f, (unsigned)G.sm_count * 8u, 1, 1, 256, 1, 1, 0, stream, params, NULL));
-        rc = get_fn("xmr_mm_split_bt", 0, &f, NULL); if (rc) return rc;
-        unsigned int k32 = d->K, n32 = d->N; const void* B = d->d_aux;
-        void* params2[] = { &B, &pb, &k32, &n32 };
-        DRV(p_cuLaunchKernel(f, (unsigned)G.sm_count * 8u, 1, 1, 256, 1, 1, 0, stream, params2, NULL));
-    }
-    const unsigned smem = 2u * (65536u + 4u * bn * 128u) + 1024u + 256u;
-    char name[64];
-    snprintf(name, sizeof name, "xmr_mm_u32_tc_nc%u_inj%d", nc, inj);
-    CUfunction fn; int occ = 1;
-    int rc = get_fn(name, smem, &fn, &occ); if (rc) return rc;
-    CUtensorMap ma, mb;
-    {
-        cuuint64_t gdim[3] = { d->K, d->M, 4 };
-        cuuint64_t gstr[2] = { (cuuint64_t)d->K, (cuuint64_t)d->M * d->K };
-        cuuint32_t box[3] = { 128, 128, 4 };
-        cuuint32_t estr[3] = { 1, 1, 1 };
-        DRV(p_cuTensorMapEncodeTiled(&ma, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)pa, gdim, gstr, box, estr,
-                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
-    }
-    {
-        cuuint64_t gdim[3] = { d->K, d->N, 4 };
-        cuuint64_t gstr[2] = { (cuuint64_t)d->K, (cuuint64_t)d->N * d->K };
-        cuuint32_t box[3] = { 128, bn, 4 };
-        cuuint32_t estr[3] = { 1, 1, 1 };
-        DRV(p_cuTensorMapEncodeTiled(&mb, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)pb, gdim, gstr, box, estr,
-                                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
-    }
-    unsigned tiles = (d->M / 128u) * (d->N / bn);
-    unsigned grid = tiles < (unsigned)G.sm_count ? tiles : (unsigned)G.sm_count;
-    void* params[3] = { a, &ma, &mb };
-    if (d->flags & COAST_F_VERBOSE) fprintf(stderr, "coast_rt: %s grid=%u smem=%u tiles=%u\n", name, grid, smem, tiles);
-    DRV(p_cuLaunchKernel(fn, grid, 1, 1, 384, 1, 1, smem, stream, params, NULL));
-    return COAST_OK;
+/* A K-major operand of the wgmma kernels, 128-byte swizzle: rows x K elements of esize bytes, in `planes` planes. */
+static void plan_wg_map(map_desc* m, CUtensorMapDataType dtype, unsigned esize, uintptr_t base, int in_scratch, uint32_t K,
+                        uint32_t rows, unsigned planes, unsigned box_rows) {
+    m->dtype = dtype; m->rank = planes > 1 ? 3 : 2; m->base = base; m->in_scratch = in_scratch;
+    m->dim[0] = K; m->dim[1] = rows; m->dim[2] = planes;
+    m->stride[0] = (cuuint64_t)K * esize; m->stride[1] = (cuuint64_t)rows * K * esize;
+    m->box[0] = 128u / esize; m->box[1] = box_rows; m->box[2] = planes;
+    m->swz = CU_TENSOR_MAP_SWIZZLE_128B; m->l2 = CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
 }
-/* The limb planes (4 x u8 per element of A and of B^T) are per-launch scratch from the stream-ordered pool, like the
- * quicksort replicas: allocated on the launch's stream, released on it after the kernel, so launches on different
- * streams never share planes.  The pool keeps released memory cached, so steady state costs no driver allocation. */
-static int launch_mm_tc(const coast_launch_desc* d, xmr_args* a, int inj, CUstream stream) {
-    const size_t a_bytes = (size_t)d->M * d->K * 4u, b_bytes = (size_t)d->K * d->N * 4u;   /* 4 planes of 1 byte per element */
-    CUdeviceptr planes = 0;
-    DRV(p_cuMemAllocFromPoolAsync(&planes, a_bytes + b_bytes, G.pool, stream));
-    int rc = launch_mm_tc_planes(d, a, inj, stream, planes, planes + a_bytes);
-    p_cuMemFreeAsync(planes, stream);
+
+/* Pre-passes of the wgmma kernels: TF32 wgmma reads both operands K-major, so B (K x N, row-major) is transposed into scratch;
+ * the limb kernel splits A and B into u8 limb planes ([plane][M][K] and, transposed, [plane][N][K]). */
+static int prepass_transpose_b(const coast_launch_desc* d, CUdeviceptr bt, CUstream s) {
+    const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N;
+    void* params[] = { &B, &bt, &k32, &n32 };
+    return launch_small("xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
+}
+static int prepass_split_limbs(const coast_launch_desc* d, CUdeviceptr pa, CUstream s) {
+    unsigned long long rows = d->M, K = d->K; const void* A = d->d_in;
+    void* params_a[] = { &A, &pa, &rows, &K };
+    int rc = launch_small("xmr_mm_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_a, s); if (rc) return rc;
+    CUdeviceptr pb = pa + (size_t)d->M * d->K * 4u;
+    unsigned int k32 = d->K, n32 = d->N; const void* B = d->d_aux;
+    void* params_b[] = { &B, &pb, &k32, &n32 };
+    return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
+}
+
+/* Scratch comes from the stream-ordered pool: allocated on the launch's stream and released on it after the kernel, so launches
+ * on different streams never share it, and the pool keeps released memory cached (no driver allocation in steady state). */
+static int run_plan(const launch_plan* L, const coast_launch_desc* d, xmr_args* a, CUstream stream) {
+    CUfunction fn; int occ = 1;
+    int rc = get_fn(L->name, L->smem, L->block, &fn, &occ); if (rc) return rc;
+    const uint64_t cap = (uint64_t)G.sm_count * (unsigned)occ * L->waves;
+    unsigned grid = (unsigned)(L->waves && L->ctas > cap ? cap : L->ctas);
+    grid -= grid % L->cluster;
+    const size_t bytes = L->scratch + (size_t)grid * L->scratch_per_cta;
+    CUdeviceptr scratch = 0;
+    if (bytes) DRV(p_cuMemAllocFromPoolAsync(&scratch, bytes, G.pool, stream));
+    if (L->scratch_per_cta) a->aux = (const void*)scratch;
+    CUtensorMap maps[2];
+    rc = L->prepass ? L->prepass(d, scratch, stream) : COAST_OK;
+    for (int i = 0; i < L->n_maps && !rc; ++i) rc = encode_map(&L->map[i], scratch, L->cache_maps, &maps[i]);
+    if (!rc) {
+        void* params[3] = { a, &maps[0], &maps[1] };
+        if (d->flags & COAST_F_VERBOSE)
+            fprintf(stderr, "coast_rt: %s grid=%u block=%u smem=%u units=%llu\n", L->name, grid, L->block, L->smem,
+                    (unsigned long long)d->n_units);
+        CUresult r = p_cuLaunchKernel(fn, grid, 1, 1, L->block, 1, 1, L->smem, stream, params, NULL);
+        if (r != CUDA_SUCCESS) rc = drv_fail(r, "cuLaunchKernel");
+    }
+    if (scratch) p_cuMemFreeAsync(scratch, stream);
     return rc;
 }
 
@@ -624,7 +586,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     if (d->n_units == 0) return COAST_OK;
     if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null device buffer");
     const uint32_t nc = d->num_clones;
-    const uint32_t upw = 32u / nc;
+    const uint32_t upw = xmr_units_per_warp(nc);
     const int inj = d->plan && d->plan->mode != COAST_PLAN_NONE;
 
     xmr_args a; memset(&a, 0, sizeof a);
@@ -642,173 +604,166 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         if (a.plan_mode > COAST_PLAN_TABLE) return fail(COAST_ERR_BAD_ARG, "unknown fault plan mode %u", a.plan_mode);
     }
     a.n_sites = coast_fault_sites(d->kernel, d->unit_bytes, d->K);
-    /* in-loop store votes (-storeDataSync / -noMemReplication): built for CRC16 and MM_U32, loud everywhere else */
+    /* in-loop store votes (-storeDataSync / -noMemReplication): built for CRC16, SHA256 and MM_U32, loud everywhere else */
     const int store_votes = store_votes_wanted(d->flags) && nc > 1;
     if (store_votes && !store_votes_built(d->kernel)) {
-        static const char* const kname[COAST_K_COUNT_] = { "crc16", "sha256", "aes128", "mm_u32", "gemm_tf32", "qsort", "chstone_sha", "chstone_aes" };
         const char* strict = getenv("COAST_STRICT_FLAGS");
         if (strict && strcmp(strict, "0"))
             return fail(COAST_ERR_UNSUPPORTED, "-noMemReplication / -storeDataSync: the %s kernel has no in-loop store votes "
-                                               "(COAST_STRICT_FLAGS is set)", kname[d->kernel]);
+                                               "(COAST_STRICT_FLAGS is set)", KINFO[d->kernel].name);
         if (!(G.warned_store_votes & (1u << d->kernel))) {
             G.warned_store_votes |= 1u << d->kernel;
             fprintf(stderr, "coast_rt: WARNING: -noMemReplication / -storeDataSync are NOT honoured by the %s kernel: it has no in-loop "
                             "store votes and runs the default sync set (SoR-exit votes only).  COAST_STRICT_FLAGS=1 makes this an error.\n",
-                    kname[d->kernel]);
+                    KINFO[d->kernel].name);
         }
     }
     if (store_votes && store_votes_built(d->kernel)) a.flags |= XMR_F_STORE_VOTES;
 
-    char name[64];
-    unsigned smem = 0; int tma = 0; int block = XMR_CTA_THREADS; int mm_tiled = 0; int qs_scratch = 0;
-    unsigned tile_rows = 0, row_bytes = 0; CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_NONE;
+    /* kernel selection: name, CTA, shared memory, grid rule, tensor maps, pre-pass and scratch (xmr_geom.h) */
+    launch_plan L; memset(&L, 0, sizeof L);
+    L.block = XMR_CTA_THREADS; L.waves = 4; L.cluster = 1;
     const int aligned16 = (((uintptr_t)d->d_in) & 15u) == 0;
+    const int ring_ok = d->unit_bytes == 64 && aligned16 && d->n_units < 0x7FFFFF00ull && !store_votes;   /* 64-byte rows through TMA */
     switch (d->kernel) {
     case COAST_K_SHA256:
-        if (d->unit_bytes == 64 && aligned16 && d->n_units < 0x7FFFFF00ull && !store_votes) {
-            tma = 1; tile_rows = XMR_WARPS * upw; row_bytes = 64; swz = CU_TENSOR_MAP_SWIZZLE_64B;
-            smem = ring_smem(tile_rows, row_bytes);
-            snprintf(name, sizeof name, "xmr_sha256_b64_nc%u_inj%d", nc, inj);
+        if (((uintptr_t)d->d_out) & 15u) return fail(COAST_ERR_BAD_ARG, "SHA output must be 16-byte aligned");
+        if (!ring_ok) {
+            snprintf(L.name, sizeof L.name, "xmr_sha256_gen_nc%u_inj%d", nc, inj);
+        } else if (nc == 3 && !(d->flags & COAST_F_INTERLEAVE)) {
             /* TMR replica scheduling: -s (segmented, the reference default, interface.cpp:245-247) = replicas on
              * adjacent warps; -i (interleaved) = replicas on adjacent lanes.  Results are identical. */
-            if (nc == 3 && !(d->flags & COAST_F_INTERLEAVE)) {
-                block = 384; tile_rows = 128;
-                smem = ((ring_smem(tile_rows, row_bytes) + 127u) & ~127u) + 2u * 4u * 2u * 8u * 32u * 4u;
-                snprintf(name, sizeof name, "xmr_sha256_b64_seg_nc3_inj%d", inj);
-            }
+            snprintf(L.name, sizeof L.name, "xmr_sha256_b64_seg_nc3_inj%d", inj);
+            L.block = XMR_SHA_SEG_THREADS; L.smem = xmr_sha_seg_smem();
+            plan_ring(&L, &a, XMR_SHA_SEG_TILE_ROWS, 64, 0, CU_TENSOR_MAP_SWIZZLE_64B);
         } else {
-            snprintf(name, sizeof name, "xmr_sha256_gen_nc%u_inj%d", nc, inj);
+            snprintf(L.name, sizeof L.name, "xmr_sha256_b64_nc%u_inj%d", nc, inj);
+            L.smem = xmr_sha_smem(nc);
+            plan_ring(&L, &a, xmr_sha_tile_rows(nc), 64, 0, CU_TENSOR_MAP_SWIZZLE_64B);
         }
         break;
     case COAST_K_CRC16:
         if (d->unit_bytes < 1 || d->unit_bytes > 255) return fail(COAST_ERR_BAD_ARG, "crc16 length is an unsigned char (1..255)");
-        if (d->unit_bytes == 64 && aligned16 && d->n_units < 0x7FFFFF00ull && !store_votes) {
-            /* table kernel: 1024-thread CTAs (768 unprotected), shared window = [.., 0x10000) unused | 64 KiB byte-step
-             * table | tile ring at 0x20000 (CrcGeom in xmr_crc16.cuh) */
-            tma = 1; block = nc == 1 ? 768 : 1024; tile_rows = (unsigned)(block / 32) * upw; row_bytes = 64;
-            swz = CU_TENSOR_MAP_SWIZZLE_64B;
-            smem = 0x20000u + ring_smem(tile_rows, row_bytes);
-            snprintf(name, sizeof name, "xmr_crc16_b64_nc%u_inj%d", nc, inj);
+        if (ring_ok) {                                       /* table kernel: byte-step table and tile ring in shared memory */
+            snprintf(L.name, sizeof L.name, "xmr_crc16_b64_nc%u_inj%d", nc, inj);
+            L.block = xmr_crc_threads(nc); L.smem = xmr_crc_smem(nc);
+            plan_ring(&L, &a, xmr_crc_tile_rows(nc), 64, 0, CU_TENSOR_MAP_SWIZZLE_64B);
         } else {
-            snprintf(name, sizeof name, "xmr_crc16_gen_nc%u_inj%d", nc, inj);
+            snprintf(L.name, sizeof L.name, "xmr_crc16_gen_nc%u_inj%d", nc, inj);
         }
         break;
-    case COAST_K_AES128:
-        if ((d->mode & COAST_AES_KEY_PER_UNIT) && !d->d_aux) return fail(COAST_ERR_BAD_ARG, "per-unit keys need d_aux");
+    case COAST_K_AES128: {
+        const int dec = (d->mode & COAST_AES_DECRYPT) != 0, perkey = (d->mode & COAST_AES_KEY_PER_UNIT) != 0;
+        if (perkey && !d->d_aux) return fail(COAST_ERR_BAD_ARG, "per-unit keys need d_aux");
         if (!aligned16 || (((uintptr_t)d->d_out) & 15u)) return fail(COAST_ERR_BAD_ARG, "AES buffers must be 16-byte aligned");
-        if ((d->mode & COAST_AES_KEY_PER_UNIT) && (((uintptr_t)d->d_aux) & 15u)) return fail(COAST_ERR_BAD_ARG, "AES per-unit keys must be 16-byte aligned");
+        if (perkey && (((uintptr_t)d->d_aux) & 15u)) return fail(COAST_ERR_BAD_ARG, "AES per-unit keys must be 16-byte aligned");
         if (d->n_units >= 0x7FFFFF00ull) return fail(COAST_ERR_UNSUPPORTED, "AES: at most 2^31 - 257 blocks per launch (split the batch)");
-        {
-            /* one table-driven body (xmr_aes128.cuh): enc / dec with one ECB key, enck / deck with per-unit keys.  512-thread CTAs;
-             * the shared window holds the ring, the two 64 KiB-aligned T-tables and, for decrypt, the 32 KiB (InvS, S) table */
-            const int dec = (d->mode & COAST_AES_DECRYPT) != 0, perkey = (d->mode & COAST_AES_KEY_PER_UNIT) != 0;
-            tma = 1; block = 512; tile_rows = 16u * upw * (nc == 1 ? 2u : 4u); row_bytes = 16;
-            smem = dec ? 0x38000u : 0x30000u;
-            static const char* const stem[4] = { "xmr_aes128_enc", "xmr_aes128_dec", "xmr_aes128_enck", "xmr_aes128_deck" };
-            snprintf(name, sizeof name, "%s_nc%u_inj%d", stem[dec + 2 * perkey], nc, inj);
-        }
+        /* one table-driven body (xmr_aes128.cuh): enc / dec with one ECB key, enck / deck with per-unit keys */
+        static const char* const stem[4] = { "xmr_aes128_enc", "xmr_aes128_dec", "xmr_aes128_enck", "xmr_aes128_deck" };
+        snprintf(L.name, sizeof L.name, "%s_nc%u_inj%d", stem[dec + 2 * perkey], nc, inj);
+        L.block = XMR_AES_THREADS; L.smem = xmr_aes_smem(dec);
+        /* the same dense bytes as 256- or 64-byte rows when the count allows */
+        const unsigned tile_rows = xmr_aes_tile_rows(nc), box_rows = tile_rows / xmr_ring_loads(tile_rows);
+        unsigned pack = d->n_units % 16u == 0 ? 4u : d->n_units % 4u == 0 ? 2u : 0u;
+        while (pack && box_rows % (1u << pack)) pack -= 2u;
+        a.mode = (a.mode & ~(XMR_MODE_AES_ROWPACK_MASK << XMR_MODE_AES_ROWPACK_SHIFT)) | (pack << XMR_MODE_AES_ROWPACK_SHIFT);
+        plan_ring(&L, &a, tile_rows, 16, pack, CU_TENSOR_MAP_SWIZZLE_NONE);
         break;
-    case COAST_K_MM_U32:
+    }
+    case COAST_K_MM_U32: {
         if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "MM needs A (d_in), B (d_aux) and M,N,K");
         if (d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "MM: n_units must be M*N");
-        snprintf(name, sizeof name, "xmr_mm_u32_nc%u_inj%d", nc, inj);
-        {   /* tensor-core path (exact, u8 limbs on wgmma) for tile-aligned problems; COAST_MM_PATH=tiled|naive overrides */
-            const char* path = getenv("COAST_MM_PATH");
-            const int want_tc = !path || !strcmp(path, "tc");
-            if (store_votes) break;                              /* per-k votes on `sum`: the plain kernel (one lane per replica per element) */
-            if (want_tc && d->M % 128u == 0 && d->N % 64u == 0 && d->K % 128u == 0 && aligned16 &&
-                !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u))
-                return launch_mm_tc(d, &a, inj, (CUstream)stream);
-            if (path && !strcmp(path, "naive")) break;
-        }
-        /* register-tiled fast path: 64 x 128 x 16 tiles, NC x 128 threads (replicas on adjacent warps) */
-        if (!store_votes && d->M % 64u == 0 && d->N % 128u == 0 && d->K % 16u == 0 && aligned16 && !(((uintptr_t)d->d_aux) & 15u) &&
-            !(((uintptr_t)d->d_out) & 15u)) {
-            mm_tiled = 1; block = (int)nc * 128; smem = 64u * 1024u;
-            snprintf(name, sizeof name, "xmr_mm_u32_tiled_nc%u_inj%d", nc, inj);
+        /* the plain kernel (one lane per replica per element) takes any shape and the per-k votes on `sum`; tile-aligned problems
+         * go to the tensor cores (exact, u8 limbs on wgmma) or the register-tiled kernel; COAST_MM_PATH=tc|tiled|naive overrides */
+        snprintf(L.name, sizeof L.name, "xmr_mm_u32_nc%u_inj%d", nc, inj);
+        const char* path = getenv("COAST_MM_PATH");
+        const int aligned = aligned16 && !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u);
+        if (store_votes || !aligned) break;
+        if ((!path || !strcmp(path, "tc")) && d->M % XMR_WG_BM == 0 && d->N % xmr_mmtc_bn(1) == 0 && d->K % XMR_MMTC_BK == 0) {
+            const unsigned bn = xmr_mmtc_bn(nc);
+            snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_nc%u_inj%d", nc, inj);
+            L.block = XMR_WG_THREADS; L.smem = xmr_mmtc_smem(nc);
+            L.ctas = (d->M / XMR_WG_BM) * (d->N / bn); L.waves = 1;
+            L.scratch = ((size_t)d->M * d->K + (size_t)d->K * d->N) * 4u;          /* 4 planes of 1 byte per element */
+            L.prepass = prepass_split_limbs;
+            L.n_maps = 2;
+            plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, d->M, 4, XMR_WG_BM);
+            plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)d->M * d->K * 4u, 1, d->K, d->N, 4, bn);
+        } else if (!(path && !strcmp(path, "naive")) && d->M % XMR_MMT_BM == 0 && d->N % XMR_MMT_BN == 0 && d->K % XMR_MMT_BK == 0) {
+            snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_nc%u_inj%d", nc, inj);
+            L.block = xmr_mmt_threads(nc); L.smem = XMR_MMT_SMEM;
+            L.ctas = (d->M / XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;
         }
         break;
+    }
     case COAST_K_QSORT:
         if (d->unit_bytes < 4 || (d->unit_bytes & 3u) || d->unit_bytes > 4096u)
             return fail(COAST_ERR_BAD_ARG, "quicksort arrays are 1..1024 int32 (unit_bytes = 4*L, got %u)", d->unit_bytes);
-        block = 128; qs_scratch = 1;
         {   /* two schedulings of the same algorithm (xmr_qsort.cuh): per-unit state machine (default) or nested loops */
             const char* path = getenv("COAST_QSORT_PATH");
-            snprintf(name, sizeof name, "%s_nc%u_inj%d", path && !strcmp(path, "nested") ? "xmr_qsortn" : "xmr_qsort", nc, inj);
+            snprintf(L.name, sizeof L.name, "%s_nc%u_inj%d", path && !strcmp(path, "nested") ? "xmr_qsortn" : "xmr_qsort", nc, inj);
         }
+        /* one resident wave of persistent warps, each with a private copy of every replica's array, lane-major and CONTIGUOUS
+         * per lane (a scan walks one cache line per 32 elements; thread-local memory would put a lane's elements 128 bytes apart) */
+        L.block = XMR_QSORT_THREADS; L.waves = 1;
+        L.scratch_per_cta = (size_t)XMR_QSORT_THREADS * d->unit_bytes;
         break;
     case COAST_K_CHSTONE_SHA:
         if (d->unit_bytes < 64u || (d->unit_bytes & 63u) || d->unit_bytes >= (1u << 29))
             return fail(COAST_ERR_BAD_ARG, "CHStone sha streams are whole 64-byte blocks, 64 <= unit_bytes < 2^29 (got %u)", d->unit_bytes);
         if (!aligned16 || (((uintptr_t)d->d_out) & 3u)) return fail(COAST_ERR_BAD_ARG, "CHStone sha: d_in must be 16-byte and d_out 4-byte aligned");
-        snprintf(name, sizeof name, "xmr_chsha_nc%u_inj%d", nc, inj);
+        snprintf(L.name, sizeof L.name, "xmr_chsha_nc%u_inj%d", nc, inj);
         break;
-    case COAST_K_CHSTONE_AES:
+    case COAST_K_CHSTONE_AES: {
+        const int dec = (d->mode & COAST_AES_DECRYPT) != 0;
         if ((d->mode & COAST_AES_KEY_PER_UNIT) && !d->d_aux) return fail(COAST_ERR_BAD_ARG, "per-unit keys need d_aux");
         if (!aligned16 || (((uintptr_t)d->d_out) & 15u) || ((d->mode & COAST_AES_KEY_PER_UNIT) && (((uintptr_t)d->d_aux) & 15u)))
             return fail(COAST_ERR_BAD_ARG, "CHStone aes buffers must be 16-byte aligned");
-        block = 512; smem = (d->mode & COAST_AES_DECRYPT) ? 0x38000u : 0x30000u;        /* same shared-memory tables as the TI kernels */
-        {
-            static const char* const stem[2] = { "xmr_chaes_enc", "xmr_chaes_dec" };
-            snprintf(name, sizeof name, "%s_nc%u_inj%d", stem[(d->mode & COAST_AES_DECRYPT) ? 1 : 0], nc, inj);
-        }
+        static const char* const stem[2] = { "xmr_chaes_enc", "xmr_chaes_dec" };
+        snprintf(L.name, sizeof L.name, "%s_nc%u_inj%d", stem[dec], nc, inj);
+        L.block = XMR_AES_THREADS; L.smem = xmr_aes_smem(dec);               /* the same shared-memory tables as the TI kernels */
         break;
-    case COAST_K_GEMM_TF32:
+    }
+    case COAST_K_GEMM_TF32: {
         if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "GEMM needs A (d_in), B (d_aux) and M,N,K");
         if (d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "GEMM: n_units must be M*N");
-        if (d->M % 128u || d->N % 128u || d->K % 32u)
+        if (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % XMR_GEMM_BK)
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_TF32 tiles are 128x128x32: M,N must be multiples of 128 and K of 32 (got %u,%u,%u)", d->M, d->N, d->K);
         if (!aligned16 || (((uintptr_t)d->d_aux) & 15u) || (((uintptr_t)d->d_out) & 15u)) return fail(COAST_ERR_BAD_ARG, "GEMM buffers must be 16-byte aligned");
-        return launch_gemm_tf32(d, &a, inj, (CUstream)stream);
+        /* xmr_gemm_tf32.cuh: unprotected 128 x 256 tiles when N allows (wide), else 128 x 128.  CTA-pair kernels (cluster 2 x 1 x 1,
+         * 256-row pair tiles, B multicast) are bit-identical to the single-CTA kernels.  Default: pairs for the unprotected and
+         * DWC kernels when the shape allows, the single-CTA kernel for TMR; COAST_GEMM_PAIR=0 / 1 forces one or the other. */
+        const int wide = nc == 1 && d->N % xmr_gemm_bn(1) == 0;
+        const char* e = getenv("COAST_GEMM_PAIR");
+        const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
+        const int pair = want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
+        if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32p_nc%u_inj%d", nc, inj);
+        else if (nc == 1 && !wide) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32n_nc1_inj%d", inj);
+        else snprintf(L.name, sizeof L.name, "xmr_gemm_tf32_nc%u_inj%d", nc, inj);
+        { const char* g = getenv("COAST_GEMM_GROUP_M");
+          if (g && atoi(g) > 0 && atoi(g) <= (int)XMR_MODE_GROUP_M_MASK) a.mode = (a.mode & ~XMR_MODE_GROUP_M_MASK) | (unsigned)atoi(g); }
+        /* L2 eviction priorities: A evict_last, B and C evict_first; COAST_GEMM_L2_HINTS=0 loads and stores with the normal policy */
+        { const char* h = getenv("COAST_GEMM_L2_HINTS"); if (!(h && !strcmp(h, "0"))) a.mode |= XMR_MODE_L2_HINTS; }
+        /* the unprotected kernel halves the tiles of a short last round; COAST_GEMM_TAIL_SPLIT=0 keeps whole tiles */
+        { const char* h = getenv("COAST_GEMM_TAIL_SPLIT"); if (h && !strcmp(h, "0")) a.mode |= XMR_MODE_NO_TAIL_SPLIT; }
+        /* persistent CTAs, one per SM (their shared memory allows no second); pairs: an even grid */
+        L.block = XMR_WG_THREADS; L.smem = xmr_gemm_smem(wide);
+        L.ctas = (d->M / XMR_WG_BM) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = pair ? 2 : 1;
+        L.scratch = (size_t)d->K * d->N * 4u;                                   /* B^T */
+        L.prepass = prepass_transpose_b;
+        L.n_maps = 2;
+        plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uintptr_t)d->d_in, 0, d->K, d->M, 1, XMR_WG_BM);
+        plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, d->N, 1, xmr_gemm_b_box(pair));
+        break;
+    }
     default:
         return fail(COAST_ERR_UNSUPPORTED, "kernel %u is not built into this library yet", d->kernel);
     }
-    if (d->kernel == COAST_K_SHA256 && (((uintptr_t)d->d_out) & 15u)) return fail(COAST_ERR_BAD_ARG, "SHA output must be 16-byte aligned");
-
-    CUfunction fn; int occ = 1;
-    rc = get_fn_b(name, smem, block, &fn, &occ); if (rc) return rc;
-    unsigned grid;
-    CUtensorMap map;
-    void* params[2] = { &a, &map };
-    if (tma) {
-        uint64_t n_tiles = (d->n_units + tile_rows - 1) / tile_rows;
-        a.n_tiles = (unsigned)n_tiles;
-        unsigned loads = (tile_rows + 255u) / 256u;
-        while (tile_rows % loads) ++loads;                        /* mirrors TileRing::pick_loads() */
-        unsigned pack = 0;                                        /* AES: the same dense bytes as 256- or 64-byte rows when the count allows */
-        if (d->kernel == COAST_K_AES128) {
-            pack = d->n_units % 16u == 0 ? 4u : d->n_units % 4u == 0 ? 2u : 0u;
-            while (pack && (tile_rows / loads) % (1u << pack)) pack -= 2u;
-            a.mode = (a.mode & ~0xF00u) | (pack << 8);
-        }
-        rc = encode_rows_map(&map, d->d_in, row_bytes << pack, d->n_units >> pack, (tile_rows / loads) >> pack, swz); if (rc) return rc;
-        uint64_t cap = (uint64_t)G.sm_count * (unsigned)occ;
-        grid = (unsigned)(n_tiles < cap ? n_tiles : cap);
-    } else if (mm_tiled) {
-        grid = (d->M / 64u) * (d->N / 128u);
-    } else {
-        uint64_t warps = (d->n_units + upw - 1) / upw;
-        uint64_t wpc = (uint64_t)block / 32u;
-        uint64_t ctas = (warps + wpc - 1) / wpc;
-        /* quicksort: one resident wave (persistent warps), because every warp owns a scratch slot */
-        uint64_t cap = (uint64_t)G.sm_count * (unsigned)occ * (qs_scratch ? 1u : 4u);
-        grid = (unsigned)(ctas < cap ? ctas : cap);
+    if (!L.ctas) {                                           /* lane-interleaved kernels: each warp takes 32/nc units */
+        const uint64_t warps = (d->n_units + upw - 1) / upw, wpc = L.block / 32u;
+        L.ctas = (warps + wpc - 1) / wpc;
     }
-    CUdeviceptr scratch = 0;
-    if (qs_scratch) {
-        /* private copy of every replica's array, lane-major and CONTIGUOUS per lane (a scan walks one cache line per 32
-         * elements; thread-local memory would put consecutive elements of a lane 128 bytes apart) */
-        size_t bytes = (size_t)grid * (size_t)(block / 32) * 32u * (size_t)d->unit_bytes;
-        DRV(p_cuMemAllocFromPoolAsync(&scratch, bytes ? bytes : 4, G.pool, (CUstream)stream));
-        a.aux = (const void*)scratch;
-    }
-    if (d->flags & COAST_F_VERBOSE)
-        fprintf(stderr, "coast_rt: %s grid=%u block=%d smem=%u units=%llu\n", name, grid, block, smem,
-                (unsigned long long)d->n_units);
-    CUresult lr = p_cuLaunchKernel(fn, grid, 1, 1, (unsigned)block, 1, 1, smem, (CUstream)stream, params, NULL);
-    if (scratch) p_cuMemFreeAsync(scratch, (CUstream)stream);           /* stream-ordered: released after the kernel */
-    if (lr != CUDA_SUCCESS) return drv_fail(lr, "cuLaunchKernel");
-    return COAST_OK;
+    return run_plan(&L, d, &a, (CUstream)stream);
 }
 
 /* ------------------------------------------------------------------ */
@@ -962,10 +917,13 @@ static CUdeviceptr host_alias(const void* h, size_t bytes) {
     return d0;
 }
 
-static int drain_host_streams(void) {
-    CUresult r0 = p_cuStreamSynchronize(G.hs[0]), r1 = p_cuStreamSynchronize(G.hs[1]), r2 = p_cuStreamSynchronize(G.hs[2]);
-    CUresult r = r0 != CUDA_SUCCESS ? r0 : r1 != CUDA_SUCCESS ? r1 : r2;
-    return r == CUDA_SUCCESS ? COAST_OK : drv_fail(r, "cuStreamSynchronize(host-call streams)");
+/* A host call failed with `rc`: copies of earlier chunks may still be in flight on the caller's buffers, so wait for the three
+ * host-call streams before returning -- and keep the error text of the failure, not of the wait. */
+static int drain_host_streams(int rc) {
+    char keep[sizeof G.err]; memcpy(keep, G.err, sizeof keep);
+    for (int i = 0; i < 3; ++i) p_cuStreamSynchronize(G.hs[i]);
+    memcpy(G.err, keep, sizeof keep);
+    return rc;
 }
 
 /* Chunked pipeline: H2D -> kernel -> D2H per chunk, chunks round-robin over 3 streams / 3 staging slots. */
@@ -1017,19 +975,14 @@ static int run_host_staged(const coast_launch_desc* d, uint64_t ib, uint64_t ob,
         rc = launch_impl(&c, G.hs[slot]); if (rc) goto fail;
         STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + done * ob, G.h_out[slot], (size_t)(n * ob), G.hs[slot]));
         if (per_unit_key && d->kernel == COAST_K_AES128 && (d->mode & COAST_AES_KEY_WRITEBACK))
-            STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_aux + done * 16, G.h_aux[slot], (size_t)(n * 16), G.hs[slot]));
+            STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_aux + done * ab, G.h_aux[slot], (size_t)(n * ab), G.hs[slot]));
         if (d->d_status) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_status + done, G.h_stat[slot], (size_t)n, G.hs[slot]));
         done += n; slot = (slot + 1) % 3;
     }
 #undef STEP
     return COAST_OK;
 fail:
-    {   /* copies of earlier chunks may still be in flight on the caller's buffers: never return before they have landed */
-        char keep[sizeof G.err]; memcpy(keep, G.err, sizeof keep);
-        drain_host_streams();
-        memcpy(G.err, keep, sizeof keep);
-    }
-    return rc;
+    return drain_host_streams(rc);
 }
 
 /* Matmul host call.  B (replicated operand) goes up once; C is produced in row blocks: block i's rows of A upload, its
@@ -1074,8 +1027,7 @@ static int run_host_matmul(const coast_launch_desc* d, coast_stats* out, int* dw
     DRV(p_cuStreamSynchronize(G.hs[0])); DRV(p_cuStreamSynchronize(G.hs[1]));
     return sync_impl(G.hs[2], out, dwc_fired);
 fail:
-    { char keep[sizeof G.err]; memcpy(keep, G.err, sizeof keep); drain_host_streams(); memcpy(G.err, keep, sizeof keep); }
-    return rc;
+    return drain_host_streams(rc);
 }
 
 /* `d_in` / `d_out` / `d_aux` / `d_status` of the descriptor are HOST pointers here. */
@@ -1103,8 +1055,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
      *   zerocopy: ONE launch reads and WRITES mapped host memory: SM stores of 16-32 bytes per lane to host memory
      *             are small PCIe writes, so it is meant for calls whose output is small. */
     const char* hp = getenv("COAST_HOST_PATH");
-    const int streams_once = d->kernel == COAST_K_CRC16 || d->kernel == COAST_K_SHA256 || d->kernel == COAST_K_AES128 ||
-                             d->kernel == COAST_K_CHSTONE_SHA || d->kernel == COAST_K_CHSTONE_AES;
+    const int streams_once = KINFO[d->kernel].streams_once;
     /* default: staged -- except when the output is tiny next to the input (crc16: 2 of 64 bytes, CHStone sha: 20 bytes per
      * stream), where one zero-copy launch on pinned buffers reads each input byte once and saves the chunk pipeline's copies */
     const int tiny_out = ob * 8u <= ib;

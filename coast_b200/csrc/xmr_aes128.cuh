@@ -37,10 +37,15 @@ namespace xmr {
 //   addr = PRMT(t, lanebase) = lanebase.b3 : lanebase.b2 : byte_k(t) : lanebase.b0,  lanebase = table | half | lane*4
 // and bank = lane for every lane whatever the data -> no shared-memory bank conflicts, no rotates, no LEA.  The 128-byte
 // rows of the third window cost one extra shift: addr = PRMT(t, 2*lanebase) >> 1.
-constexpr int AES_THREADS = 512, AES_WARPS = 16;
-constexpr uint32_t AES_TAB01 = 0x10000u, AES_TAB23 = 0x20000u, AES_SIS = 0x30000u;
-constexpr uint32_t AES_WINDOW_END_ENC = 0x30000u, AES_WINDOW_END_DEC = 0x38000u;
-template <int NC> struct AesGeom { static constexpr int J = NC == 1 ? 2 : 4; static constexpr int TROWS = AES_WARPS * Lanes<NC>::kUnitsPerWarp * J; };
+constexpr int AES_THREADS = XMR_AES_THREADS, AES_WARPS = XMR_AES_WARPS;
+constexpr uint32_t AES_TAB01 = XMR_AES_TAB01, AES_TAB23 = XMR_AES_TAB23, AES_SIS = XMR_AES_SIS;
+static_assert(AES_TAB01 + 256u * 64u * 4u <= AES_TAB23 && AES_TAB23 + 256u * 64u * 4u <= xmr_aes_smem(false) &&
+              AES_SIS + 256u * 32u * 4u <= xmr_aes_smem(true), "the tables fit the launch's shared memory");
+template <int NC> struct AesGeom {
+    static constexpr int J = (int)xmr_aes_blocks_per_lane(NC);
+    static constexpr int TROWS = AES_WARPS * Lanes<NC>::kUnitsPerWarp * J;
+    static_assert(TROWS == xmr_aes_tile_rows(NC), "the host's tile");
+};
 
 // Input ring of the AES kernels: 3 stages, full[] (TMA -> warps) and empty[] (warps -> the issuing thread) mbarriers and NO
 // CTA-wide barrier in the tile loop.  r02 ablation (profiles/r02_aes_injector_ablation.txt): with the r01 ring's __syncthreads()
@@ -51,12 +56,12 @@ template <int NC> struct AesGeom { static constexpr int J = NC == 1 ? 2 : 4; sta
 constexpr int AES_STAGES = 3;
 template <int TILE_ROWS>
 struct AesRing {
-    static constexpr int pick_loads() { int l = (TILE_ROWS + 255) / 256; while (TILE_ROWS % l) ++l; return l; }
-    static constexpr int LOADS = pick_loads();
+    static constexpr int LOADS = (int)xmr_ring_loads(TILE_ROWS);
     static constexpr int BOX_ROWS = TILE_ROWS / LOADS;
     static constexpr uint32_t TILE_BYTES = (uint32_t)TILE_ROWS * 16u;
-    static constexpr uint32_t STAGE_STRIDE = (TILE_BYTES + 1023u) & ~1023u;
-    static constexpr uint32_t SMEM_BYTES = AES_STAGES * STAGE_STRIDE + 128;
+    static constexpr uint32_t STAGE_STRIDE = xmr_ring_stride(TILE_ROWS, 16u);
+    static constexpr uint32_t SMEM_BYTES = xmr_ring_smem(AES_STAGES, TILE_ROWS, 16u, 128u);
+    static_assert(2 * AES_STAGES * sizeof(uint64_t) <= 128u, "full and empty barriers fit behind the tiles");
     uint8_t* tiles; uint64_t* full; uint64_t* empty; const CUtensorMap* tmap; uint32_t pack_shift;
     __device__ __forceinline__ void init(uint8_t* smem, const CUtensorMap* map, uint32_t row_pack_shift) {
         tiles = smem; tmap = map; pack_shift = row_pack_shift;
@@ -161,7 +166,7 @@ __device__ __forceinline__ void aes_round_cols(const AesLaneBases& L, const uint
 template <int NC>
 __device__ __forceinline__ void aes_vote_store(const uint32_t (&c)[4], uint8_t* out, unsigned long long local,
                                                unsigned long long gunit, bool valid, int lane, uint32_t flags, Tally& tally) {
-    const bool majority = flags & COAST_F_MAJORITY_D;
+    const bool majority = flags & COAST_F_MAJORITY_VOTER;
     uint32_t o[4], bad = 0;
 #pragma unroll
     for (int i = 0; i < 4; ++i) { Voted v = vote_u32<NC, 1>(c[i], majority); o[i] = v.vote; bad += v.bad; }
@@ -312,7 +317,7 @@ __device__ __forceinline__ void aes128_body(const xmr_args& a, const CUtensorMap
     const uint32_t win = smem_u32(smem_raw);                    // shared-window address of the dynamic region
     uint8_t* ring_mem = smem_raw + ((1024u - (win & 1023u)) & 1023u);
     Ring ring;
-    ring.init(ring_mem, tmap, (a.mode >> 8) & 15u);             // XMR_AES_ROWPACK: 16-byte blocks described as 64- or 256-byte rows
+    ring.init(ring_mem, tmap, (a.mode >> XMR_MODE_AES_ROWPACK_SHIFT) & XMR_MODE_AES_ROWPACK_MASK);   // 16-byte blocks as 64- or 256-byte rows
     // per-warp queue of deferred units (INJECT, one-key kernels): {unit, fault} pairs right after the ring, still below the tables
     constexpr uint32_t Q_OFF = (Ring::SMEM_BYTES + 127u) & ~127u;
     static_assert(Q_OFF + (uint32_t)AES_WARPS * AES_QCAP * 8u + 2048u + 1024u <= AES_TAB01, "ring + queues must end below the first table window");
@@ -480,7 +485,7 @@ __device__ __forceinline__ void aes128_body(const xmr_args& a, const CUtensorMap
 #pragma unroll
         for (int j = 0; j < J; ++j) {
             aes_vote_store<NC>(s[j], static_cast<uint8_t*>(a.out), local[j], a.unit_base + local[j], valid[j] && !((defer >> j) & 1u), lane, a.flags, tally);
-            if (PERKEY && (a.mode & 4u) && valid[j] && Lanes<NC>::voter(lane))       // COAST_AES_KEY_WRITEBACK: replica 0's mutated key[]
+            if (PERKEY && (a.mode & COAST_AES_KEY_WRITEBACK) && valid[j] && Lanes<NC>::voter(lane))   // replica 0's mutated key[]
                 *reinterpret_cast<uint4*>(static_cast<uint8_t*>(const_cast<void*>(a.aux)) + local[j] * 16ull) = make_uint4(k[j][0], k[j][1], k[j][2], k[j][3]);
         }
         if (INJECT && !PERKEY && q_count > (uint32_t)(AES_QCAP - J * UPW)) {        // the next tile might not fit: drain now (rare)
@@ -516,8 +521,8 @@ __device__ __forceinline__ void chstone_aes_body(const xmr_args& a) {
     const unsigned long long gwarp = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const unsigned long long nwarps = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
     const unsigned long long n_wtiles = (a.n_units + UPW - 1) / UPW;
-    const bool per_unit = a.mode & 2u;
-    const bool majority = a.flags & COAST_F_MAJORITY_D;
+    const bool per_unit = a.mode & COAST_AES_KEY_PER_UNIT;
+    const bool majority = a.flags & COAST_F_MAJORITY_VOTER;
     const uint32_t rk_unused[4] = {0u, 0u, 0u, 0u};
     Tally tally(a);
     for (unsigned long long wt = gwarp; wt < n_wtiles; wt += nwarps) {

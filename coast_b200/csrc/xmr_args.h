@@ -16,7 +16,7 @@ typedef struct xmr_args {
     unsigned char* status;            /* optional: per-unit count of disagreeing votes (saturating u8) */
     unsigned int unit_bytes;
     unsigned int flags;               /* COAST_F_*                                  */
-    unsigned int mode;                /* COAST_AES_*                                */
+    unsigned int mode;                /* per kernel: AES, COAST_AES_* and the row pack (XMR_MODE_AES_ROWPACK_*); TF32 GEMM, XMR_MODE_* */
     unsigned int M, N, K;
     unsigned int plan_mode, seed_lo, seed_hi, threshold;
     unsigned int n_sites;
@@ -28,6 +28,13 @@ typedef struct xmr_args {
 #define XMR_F_STORE_VOTES 0x8000u
 /* AES: bits 8..11 of xmr_args.mode = log2 of the blocks per tensor-map row (the host describes the dense 16-byte blocks as
  * 64- or 256-byte rows when the count allows) */
+#define XMR_MODE_AES_ROWPACK_SHIFT 8
+#define XMR_MODE_AES_ROWPACK_MASK  0xFu
+/* TF32 GEMM (set by the host from COAST_GEMM_*): tile-rows per rasterisation group (0 = the kernel's default), L2 eviction
+ * hints on, no splitting of a short last round's tiles */
+#define XMR_MODE_GROUP_M_MASK  0xFFu
+#define XMR_MODE_L2_HINTS      0x100u
+#define XMR_MODE_NO_TAIL_SPLIT 0x200u
 
 /* counter slots (mirror coast_stats) */
 #define XMR_CTR_ERRORS   0
@@ -36,10 +43,5 @@ typedef struct xmr_args {
 #define XMR_CTR_INJECTED 3
 #define XMR_CTR_FIRST    4
 #define XMR_CTR_COUNT    5
-
-/* tile geometry of the TMA-staged kernels: CTA = 8 warps, each warp owns 32/NC units */
-#define XMR_CTA_THREADS 256
-#define XMR_WARPS       8
-#define XMR_STAGES      2
 
 #endif

@@ -96,7 +96,7 @@ __device__ __forceinline__ void chsha_body(const xmr_args& a) {
     const unsigned long long n_wtiles = (a.n_units + UPW - 1) / UPW;
     const uint32_t len = a.unit_bytes;
     const uint32_t nblk = len >> 6;                            // data blocks; the final block is compression #nblk
-    const bool majority = a.flags & COAST_F_MAJORITY_D;
+    const bool majority = a.flags & COAST_F_MAJORITY_VOTER;
     Tally tally(a);
     for (unsigned long long wt = gwarp; wt < n_wtiles; wt += nwarps) {
         const unsigned long long local = wt * UPW + Lanes<NC>::unit(lane);

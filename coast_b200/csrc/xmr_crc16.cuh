@@ -18,7 +18,7 @@ __device__ __forceinline__ uint32_t crc16_step(uint32_t crc, uint32_t b) {
 template <int NC>
 __device__ __forceinline__ void crc_vote_store(uint32_t crc, uint16_t* out, unsigned long long local, unsigned long long gunit,
                                                bool valid, int lane, uint32_t flags, Tally& tally) {
-    Voted v = vote_u32<NC, 4>(crc, flags & COAST_F_MAJORITY_D);   // one element (the u16 lives alone in the register)
+    Voted v = vote_u32<NC, 4>(crc, flags & COAST_F_MAJORITY_VOTER);   // one element (the u16 lives alone in the register)
     if (valid && Lanes<NC>::voter(lane)) {
         out[local] = (uint16_t)v.vote;
         tally.unit_exit<NC>(v.bad, 1u, flags, gunit);
@@ -41,10 +41,11 @@ __device__ __forceinline__ void crc_vote_store(uint32_t crc, uint16_t* out, unsi
 // this form 2 + LDS; 0.394 -> 0.244 -> see profiles/ for the current time of 2^22 TMR messages).
 // 64 KiB of table leaves one CTA per SM, so the CTA is 1024 threads (768 for the unprotected run, whose 64 B x 1024
 // tile ring would not fit next to the table).
-constexpr uint32_t CRC_TAB = 0x10000u, CRC_RING = 0x20000u;
+constexpr uint32_t CRC_TAB = XMR_CRC_TAB, CRC_RING = XMR_CRC_RING;
+static_assert(CRC_TAB + 256u * 64u * 4u <= CRC_RING, "the table ends below the ring");
 template <int NC> struct CrcGeom {
-    static constexpr int WARPS = NC == 1 ? 24 : 32;
-    static constexpr int THREADS = WARPS * 32;
+    static constexpr int THREADS = (int)xmr_crc_threads(NC);
+    static constexpr int WARPS = THREADS / 32;
     static constexpr int TU = WARPS * Lanes<NC>::kUnitsPerWarp;
 };
 template <int OFF>
@@ -72,6 +73,7 @@ __device__ __forceinline__ void crc16_b64_body(const xmr_args& a, const CUtensor
     static_assert(XMR_STAGES == CRC_J, "one ring stage per in-flight message of a lane");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     using Ring = TileRing<TU, 64>;
+    static_assert(TU == xmr_crc_tile_rows(NC) && CRC_RING + Ring::SMEM_BYTES <= xmr_crc_smem(NC), "ring fits the launch's shared memory");
     const uint32_t win = smem_u32(smem_raw);                    // shared-window address of the dynamic region
     Ring ring;
     ring.init(smem_raw + (CRC_RING - win), tmap);
@@ -211,7 +213,7 @@ __device__ __forceinline__ void crc16_gen_body(const xmr_args& a) {
         } else {
             // -storeDataSync / -noMemReplication: the three assignments of the loop body are voted (crc16.c:26-28), the
             // replicas continue with the voted value; 3 votes per byte + the SoR exit
-            const bool majority = a.flags & COAST_F_MAJORITY_D;
+            const bool majority = a.flags & COAST_F_MAJORITY_VOTER;
             uint32_t bad = 0;
             for (uint32_t i = 0; i < len; ++i) {
                 uint32_t b = __ldg(msg + i);

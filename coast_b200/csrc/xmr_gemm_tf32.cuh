@@ -28,17 +28,19 @@
 namespace xmr {
 namespace gemm {
 
-constexpr int BM = 128, BK = 32;                     // BK fp32 = 128 bytes = one swizzle row
+constexpr int BM = XMR_WG_BM, BK = XMR_GEMM_BK;      // BK fp32 = 128 bytes = one swizzle row
 constexpr int WG_K = 8;                              // one wgmma consumes 8 tf32 = 32 bytes of K
 constexpr int WG_N = 128;                            // wgmma N per instruction
 constexpr uint32_t A_STAGE = BM * BK * 4;            // 16 KiB
-constexpr int CTA_THREADS = 384;                     // warpgroup 0 = producer, 1-2 = consumers
+constexpr int CTA_THREADS = XMR_WG_THREADS;          // warpgroup 0 = producer, 1-2 = consumers
 template <int NC, bool WIDE = (NC == 1)> struct Geom {         // WIDE: 128 x 256 tiles (unprotected, N % 256 == 0)
-    static constexpr int BN = WIDE ? 256 : 128;
+    static constexpr int BN = (int)xmr_gemm_bn(WIDE);
     static constexpr int NSUB = BN / WG_N;
-    static constexpr int STAGES = WIDE ? 4 : 6;                  // 192 KiB of operand stages either way
+    static constexpr int STAGES = (int)xmr_gemm_stages(WIDE);   // 192 KiB of operand stages either way
     static constexpr uint32_t B_STAGE = BK * BN * 4;             // [BN rows of B^T][128 B]
-    static constexpr uint32_t SMEM_BYTES = STAGES * (A_STAGE + B_STAGE) + 1024 /*align slack*/ + 256 /*barriers*/;
+    // 1 KiB alignment slack, the stages, then full[] and empty[]
+    static_assert(1023u + STAGES * (A_STAGE + B_STAGE) + 2u * STAGES * sizeof(uint64_t) <= xmr_gemm_smem(WIDE),
+                  "stages and barriers fit the launch's shared memory");
 };
 constexpr uint32_t GROUP_M_DEFAULT = 16;             // tile rasterisation: 16 tile-rows per group, column-major inside
 constexpr uint32_t GROUP_M = GROUP_M_DEFAULT;        // (xmr_mm_tc.cuh uses the fixed value)
@@ -150,7 +152,7 @@ template <int NC, int NSUB, bool INJECT>
 __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float (&acc)[NC][NSUB][64], uint32_t row0, uint32_t n0, uint32_t nsub_t,
                                          bool hints, uint64_t pol_c) {
     const uint32_t flags = a.flags;
-    const bool majority = flags & COAST_F_MAJORITY_D;
+    const bool majority = flags & COAST_F_MAJORITY_VOTER;
     float* C = static_cast<float*>(a.out);
     const uint32_t lane = threadIdx.x & 31;
 #pragma unroll
@@ -203,7 +205,7 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
     using G = Geom<NC, WIDE>;
     constexpr int BN = G::BN, NSUB = G::NSUB, STAGES = G::STAGES;
     constexpr uint32_t B_STAGE = G::B_STAGE;
-    constexpr int B_BOX = PAIR ? 64 : 128;                      // B^T rows per TMA box
+    constexpr int B_BOX = (int)xmr_gemm_b_box(PAIR);            // B^T rows per TMA box
     constexpr uint32_t CTAS = PAIR ? 2u : 1u;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023u) & ~(uintptr_t)1023u);
@@ -217,16 +219,16 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
     const uint32_t worker = blockIdx.x / CTAS, n_workers = gridDim.x / CTAS;
     const uint32_t TM = BM * CTAS;                              // rows of a (pair) tile
     const uint32_t tiles_n = a.N / BN, tiles_m = a.M / TM, n_tiles = tiles_m * tiles_n, kblocks = a.K / BK;
-    const uint32_t gm1 = (a.mode & 0xFFu) ? (a.mode & 0xFFu) : GROUP_M_DEFAULT;
+    const uint32_t gm1 = (a.mode & XMR_MODE_GROUP_M_MASK) ? (a.mode & XMR_MODE_GROUP_M_MASK) : GROUP_M_DEFAULT;
     const uint32_t group_m = PAIR ? (gm1 > 1u ? gm1 / 2u : 1u) : gm1;   // pair tiles are 256 rows: half as many tile-rows per group
-    const bool hints = (a.mode & 0x100u) != 0;
+    const bool hints = (a.mode & XMR_MODE_L2_HINTS) != 0;
     // Wave quantisation (WIDE only): e.g. 512 tiles on 132 CTAs are 3.9 rounds.  When the last, partial round holds at most half
     // the workers, each of its tiles is split into two 128-column halves, so the tail costs half a round: virtual tile ids
     // [0, sched_full) are whole tiles, [sched_full, n_virtual) are halves (two consecutive ids per tile).
     uint32_t sched_full = n_tiles, n_virtual = n_tiles;
     if (WIDE) {
         const uint32_t whole = (n_tiles / n_workers) * n_workers, rem = n_tiles - whole;
-        if (rem && 2u * rem <= n_workers && !(a.mode & 0x200u)) { sched_full = whole; n_virtual = whole + 2u * rem; }
+        if (rem && 2u * rem <= n_workers && !(a.mode & XMR_MODE_NO_TAIL_SPLIT)) { sched_full = whole; n_virtual = whole + 2u * rem; }
     }
     auto decode = [&](uint32_t v, uint32_t& tm, uint32_t& n_off, uint32_t& bn_t) {
         uint32_t w = v, h = 0, tn;
@@ -334,7 +336,7 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
 }  // namespace xmr
 
 // B (K x N, row-major) -> B^T (N x K): the K-major operand TF32 wgmma reads.  32 x 32 tiles through shared memory.
-extern "C" __global__ void __launch_bounds__(256)
+extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
 xmr_gemm_bt(const float* __restrict__ B, float* __restrict__ Bt, unsigned int K, unsigned int N) {
     __shared__ float tile[32][33];
     const unsigned int tiles_n = N / 32u, tiles_k = K / 32u;

@@ -48,7 +48,7 @@ __device__ __forceinline__ void mm_u32_body(const xmr_args& a) {
                 sum += __ldg(ap + k) * __ldg(bp + (size_t)k * N);
                 if (INJECT && fsite == k) sum ^= fmask;
             }
-            Voted v = vote_u32<NC, 4>(sum, a.flags & COAST_F_MAJORITY_D);
+            Voted v = vote_u32<NC, 4>(sum, a.flags & COAST_F_MAJORITY_VOTER);
             if (valid && Lanes<NC>::voter(lane)) {
                 C[local] = v.vote;                              // :16
                 tally.unit_exit<NC>(v.bad, 1u, a.flags, a.unit_base + local);
@@ -56,7 +56,7 @@ __device__ __forceinline__ void mm_u32_body(const xmr_args& a) {
         } else {
             // -storeDataSync / -noMemReplication: `sum += ...` (:13) is voted at every k, the replicas continue with the voted
             // value; K votes + the SoR-exit store (:16)
-            const bool majority = a.flags & COAST_F_MAJORITY_D;
+            const bool majority = a.flags & COAST_F_MAJORITY_VOTER;
             uint32_t bad = 0;
             for (uint32_t k = 0; k < K; ++k) {
                 sum += __ldg(ap + k) * __ldg(bp + (size_t)k * N);

@@ -22,14 +22,16 @@ namespace mmtc {
 
 using namespace xmr::gemm;
 
-constexpr int TBM = 128, TBK = 128;                 // 128 u8 of K = one 128-byte swizzle row = 4 wgmmas of K = 32
+constexpr int TBM = XMR_WG_BM, TBK = XMR_MMTC_BK;    // 128 u8 of K = one 128-byte swizzle row = 4 wgmmas of K = 32
 // register accumulators per consumer thread: NC x 4 x BN / 2 (TMR: 3 x 4 x 16 = 192)
 template <int NC> struct Geom {
-    static constexpr int BN = NC == 1 ? 64 : 32;
+    static constexpr int BN = (int)xmr_mmtc_bn(NC);
     static constexpr uint32_t A_STAGE_B = 4u * TBM * TBK;            // 64 KiB: [plane][row][128 B]
     static constexpr uint32_t B_STAGE_B = 4u * BN * TBK;             // 32 / 16 KiB
-    static constexpr int STAGES_ = 2;
-    static constexpr uint32_t SMEM = STAGES_ * (A_STAGE_B + B_STAGE_B) + 1024 + 256;
+    static constexpr int STAGES_ = (int)XMR_MMTC_STAGES;
+    // 1 KiB alignment slack, the stages, then full[] and empty[]
+    static_assert(1023u + STAGES_ * (A_STAGE_B + B_STAGE_B) + 2u * STAGES_ * sizeof(uint64_t) <= xmr_mmtc_smem(NC),
+                  "stages and barriers fit the launch's shared memory");
 };
 template <int BN> __device__ __forceinline__ void wgmma_u8(uint32_t (&d)[BN / 2], uint64_t da, uint64_t db);
 template <> __device__ __forceinline__ void wgmma_u8<32>(uint32_t (&d)[16], uint64_t da, uint64_t db) { wgmma_u8_m64n32k32(d, da, db); }
@@ -79,7 +81,7 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
         const uint32_t t = threadIdx.x & 127, lane = t & 31;
         const uint32_t a_off = (uint32_t)(wg - 1) * 64u * 128u;
         const uint32_t flags = a.flags;
-        const bool majority = flags & COAST_F_MAJORITY_D;
+        const bool majority = flags & COAST_F_MAJORITY_VOTER;
         uint32_t* C = static_cast<uint32_t*>(a.out);
         const uint32_t* __restrict__ A32 = static_cast<const uint32_t*>(a.in);
         const uint32_t* __restrict__ B32 = static_cast<const uint32_t*>(a.aux);
@@ -174,7 +176,7 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
 
 // ---- limb-split pre-pass ---------------------------------------------------------------------------------------
 // A (u32, rows x K, row-major) -> planes[l][row][k] (u8).  One thread = 4 consecutive k of one row.
-extern "C" __global__ void __launch_bounds__(256)
+extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
 xmr_mm_split_a(const uint32_t* __restrict__ A, uint8_t* __restrict__ planes, unsigned long long rows, unsigned long long K) {
     const unsigned long long quads = rows * K / 4ull, stride = (unsigned long long)gridDim.x * blockDim.x;
     for (unsigned long long q = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; q < quads; q += stride) {
@@ -191,7 +193,7 @@ xmr_mm_split_a(const uint32_t* __restrict__ A, uint8_t* __restrict__ planes, uns
     }
 }
 // B (u32, K x N, row-major) -> planes[l][n][k] (u8, TRANSPOSED so the MMA's B operand is K-major).  32 x 32 tiles via smem.
-extern "C" __global__ void __launch_bounds__(256)
+extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
 xmr_mm_split_bt(const uint32_t* __restrict__ B, uint8_t* __restrict__ planes, unsigned int K, unsigned int N) {
     __shared__ uint32_t tile[32][33];
     const unsigned int tiles_n = N / 32u, tiles_k = K / 32u;

@@ -14,7 +14,7 @@
 namespace xmr {
 namespace mmt {
 
-constexpr int BM = 64, BN = 128, BK = 16, VT = 128;
+constexpr int BM = XMR_MMT_BM, BN = XMR_MMT_BN, BK = XMR_MMT_BK, VT = XMR_MMT_VT;
 
 __device__ __forceinline__ Voted vote3(uint32_t x, uint32_t r1, uint32_t r2, int nc, bool majority) {
     Voted v{x, 0u};
@@ -32,7 +32,9 @@ __device__ __forceinline__ void body(const xmr_args& a) {
     extern __shared__ __align__(16) uint32_t smem[];
     uint32_t* As = smem;                        // [2][BK][BM]   (k-major: transposed on the way in)
     uint32_t* Bs = smem + 2 * BK * BM;          // [2][BK][BN]
-    uint32_t* ex = smem;                        // epilogue: [NC-1][64][VT], reuses the operand buffers (64 KiB)
+    uint32_t* ex = smem;                        // epilogue: [NC-1][64][VT], reuses the operand buffers
+    static_assert(2u * BK * (BM + BN) * 4u <= XMR_MMT_SMEM && (NC - 1u) * 64u * VT * 4u <= XMR_MMT_SMEM,
+                  "operand tiles and epilogue buffer fit the launch's shared memory");
     const int tid = threadIdx.x, r = tid / VT, vt = tid % VT;
     const int tx = vt & 15, ty = vt >> 4;        // micro-tile: rows {ty*4+i, 32+ty*4+i}, cols {tx*4+j, 64+tx*4+j}
     const uint32_t M = a.M, N = a.N, K = a.K;
@@ -104,7 +106,7 @@ __device__ __forceinline__ void body(const xmr_args& a) {
     }
 
     Tally tally(a);
-    const bool majority = a.flags & COAST_F_MAJORITY_D;
+    const bool majority = a.flags & COAST_F_MAJORITY_VOTER;
     auto row_of = [&](int i) { return m0 + (i < 4 ? ty * 4 + i : 32 + ty * 4 + (i - 4)); };
     auto col_of = [&](int j) { return n0 + (j < 4 ? tx * 4 + j : 64 + tx * 4 + (j - 4)); };
 
@@ -163,7 +165,7 @@ __device__ __forceinline__ void body(const xmr_args& a) {
 }  // namespace xmr
 
 #define XMR_MMT_KERNEL(NC, INJ)                                                                          \
-    extern "C" __global__ void __launch_bounds__(NC * 128)                                               \
+    extern "C" __global__ void __launch_bounds__(xmr_mmt_threads(NC))                                             \
     xmr_mm_u32_tiled_nc##NC##_inj##INJ(const __grid_constant__ xmr_args a) { xmr::mmt::body<NC, INJ != 0>(a); }
 XMR_MMT_KERNEL(1, 0) XMR_MMT_KERNEL(2, 0) XMR_MMT_KERNEL(3, 0)
 XMR_MMT_KERNEL(1, 1) XMR_MMT_KERNEL(2, 1) XMR_MMT_KERNEL(3, 1)

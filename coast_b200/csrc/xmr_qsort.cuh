@@ -69,7 +69,7 @@ __device__ __forceinline__ void qsort_nested_body(const xmr_args& a) {
                 }
                 if (fsite >= 32u * L && fsite != 0xFFFFFFFFu) at(fsite - 32u * L) ^= (int32_t)fmask;
             }
-            QsVote<NC> vote{gmask, base, (a.flags & COAST_F_MAJORITY_D) != 0, r == 0};
+            QsVote<NC> vote{gmask, base, (a.flags & COAST_F_MAJORITY_VOTER) != 0, r == 0};
             uint32_t ev = 0;
             int sp = 0;
             stack[sp++] = L;                                    // off = 0
@@ -120,7 +120,7 @@ __device__ __forceinline__ void qsort_nested_body(const xmr_args& a) {
                     else {
                         const int32_t r2 = __shfl_sync(gmask, x, base + 2);
                         const bool c01 = r0 == r1, c02 = r0 == r2;
-                        v = (a.flags & COAST_F_MAJORITY_D) ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
+                        v = (a.flags & COAST_F_MAJORITY_VOTER) ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
                         bad += (c01 && c02) ? 0u : 1u;
                     }
                 }
@@ -129,9 +129,9 @@ __device__ __forceinline__ void qsort_nested_body(const xmr_args& a) {
             if (r == 0) {
                 const unsigned long long gunit = a.unit_base + local;
                 if (NC == 3) {
-                    if (a.flags & COAST_F_COUNT_ERRORS_D) {
+                    if (a.flags & COAST_F_COUNT_ERRORS) {
                         tally.errors += bad + vote.ndis;
-                        if (a.flags & COAST_F_COUNT_SYNCS_D) tally.syncs += vote.syncs + L;
+                        if (a.flags & COAST_F_COUNT_SYNCS) tally.syncs += vote.syncs + L;
                     }
                 } else if (NC == 2) {
                     tally.dwc += (bad || vote.ndis) ? 1u : 0u;
@@ -169,7 +169,7 @@ __device__ __forceinline__ void qsort_body(const xmr_args& a) {
     const unsigned long long nwarps = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
     const unsigned long long n_wtiles = (a.n_units + UPW - 1) / UPW;
     const uint32_t L = a.unit_bytes >> 2;
-    const bool majority = (a.flags & COAST_F_MAJORITY_D) != 0;
+    const bool majority = (a.flags & COAST_F_MAJORITY_VOTER) != 0;
     Tally tally(a);
     int32_t* const Au = static_cast<int32_t*>(const_cast<void*>(a.aux)) + (gwarp * 32ull + (unsigned)base) * L;   // this unit's NC x L slot
     auto at = [&](uint32_t e) -> int32_t& { return Au[e * NC + (uint32_t)r]; };                  // element e of this replica
@@ -275,9 +275,9 @@ __device__ __forceinline__ void qsort_body(const xmr_args& a) {
             if (r == 0) {
                 const unsigned long long gunit = a.unit_base + local;
                 if (NC == 3) {
-                    if (a.flags & COAST_F_COUNT_ERRORS_D) {
+                    if (a.flags & COAST_F_COUNT_ERRORS) {
                         tally.errors += bad + ndis;
-                        if (a.flags & COAST_F_COUNT_SYNCS_D) tally.syncs += syncs + L;
+                        if (a.flags & COAST_F_COUNT_SYNCS) tally.syncs += syncs + L;
                     }
                 } else if (NC == 2) {
                     tally.dwc += (bad || ndis) ? 1u : 0u;
@@ -295,10 +295,10 @@ __device__ __forceinline__ void qsort_body(const xmr_args& a) {
 }  // namespace xmr
 
 #define XMR_QSORT_KERNEL(NC, INJ)                                                                        \
-    extern "C" __global__ void __launch_bounds__(128)                                                    \
+    extern "C" __global__ void __launch_bounds__(XMR_QSORT_THREADS)                                              \
     xmr_qsort_nc##NC##_inj##INJ(const __grid_constant__ xmr_args a) { xmr::qsort_body<NC, INJ != 0>(a); }
 #define XMR_QSORT_NESTED_KERNEL(NC, INJ)                                                                 \
-    extern "C" __global__ void __launch_bounds__(128)                                                    \
+    extern "C" __global__ void __launch_bounds__(XMR_QSORT_THREADS)                                              \
     xmr_qsortn_nc##NC##_inj##INJ(const __grid_constant__ xmr_args a) { xmr::qsort_nested_body<NC, INJ != 0>(a); }
 XMR_QSORT_NESTED_KERNEL(1, 0) XMR_QSORT_NESTED_KERNEL(2, 0) XMR_QSORT_NESTED_KERNEL(3, 0)
 XMR_QSORT_NESTED_KERNEL(1, 1) XMR_QSORT_NESTED_KERNEL(2, 1) XMR_QSORT_NESTED_KERNEL(3, 1)

@@ -139,7 +139,7 @@ __device__ __forceinline__ void sha_init(uint32_t (&st)[8]) {   // :108-115
 template <int NC>
 __device__ __forceinline__ void sha_vote_store(const uint32_t (&st)[8], uint8_t* out, unsigned long long local,
                                                unsigned long long gunit, bool valid, int lane, uint32_t flags, Tally& tally) {
-    const bool majority = flags & COAST_F_MAJORITY_D;
+    const bool majority = flags & COAST_F_MAJORITY_VOTER;
     uint32_t o[8], bad = 0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -163,6 +163,7 @@ template <int NC, bool INJECT>
 __device__ __forceinline__ void sha256_b64_body(const xmr_args& a, const CUtensorMap* tmap) {
     constexpr int UPW = Lanes<NC>::kUnitsPerWarp;
     constexpr int TU = XMR_WARPS * UPW;                       // units per tile
+    static_assert(TU == xmr_sha_tile_rows(NC) && TileRing<TU, 64>::SMEM_BYTES <= xmr_sha_smem(NC), "ring fits the launch's shared memory");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     TileRing<TU, 64> ring;
     ring.init(smem_raw, tmap);
@@ -255,7 +256,7 @@ __device__ __forceinline__ void sha256_gen_body(const xmr_args& a) {
             }
         }
         const bool sv = (a.flags & XMR_F_STORE_VOTES) != 0;
-        const bool majority = a.flags & COAST_F_MAJORITY_D;
+        const bool majority = a.flags & COAST_F_MAJORITY_VOTER;
         uint32_t sv_bad = 0;
         uint32_t st[8];
         sha_init(st);
@@ -323,21 +324,25 @@ __device__ __forceinline__ void sha256_gen_body(const xmr_args& a) {
 // state through shared memory, a 96-thread named barrier per group orders it, warp 0 of the group votes
 // (same select voter / counters) and stores 32 lanes x 32 B = 1 KiB contiguous.
 // ---------------------------------------------------------------------------------------------
-constexpr int SEG_THREADS = 384, SEG_GROUPS = 4, SEG_TU = SEG_GROUPS * 32;
+constexpr int SEG_THREADS = XMR_SHA_SEG_THREADS, SEG_GROUPS = SEG_THREADS / 96, SEG_TU = SEG_GROUPS * 32;
+constexpr uint32_t SEG_EXCH_WORDS = 2 * 8 * 32;              // per tile parity and group: [replica 1..2][word][lane]
 
 template <bool INJECT>
 __device__ __forceinline__ void sha256_b64_seg_body(const xmr_args& a, const CUtensorMap* tmap) {
     using Ring = TileRing<SEG_TU, 64>;
+    static_assert(SEG_TU == XMR_SHA_SEG_TILE_ROWS && Ring::SMEM_BYTES <= xmr_sha_seg_exch_offset() &&
+                  xmr_sha_seg_exch_offset() + 2u * SEG_GROUPS * SEG_EXCH_WORDS * 4u <= xmr_sha_seg_smem(),
+                  "ring and exchange buffer fit the launch's shared memory");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     Ring ring;
     ring.init(smem_raw, tmap);
     // exchange buffer [parity][group][replica 1..2][word][lane]
-    uint32_t* exch = reinterpret_cast<uint32_t*>(smem_raw + ((Ring::SMEM_BYTES + 127u) & ~127u));
+    uint32_t* exch = reinterpret_cast<uint32_t*>(smem_raw + xmr_sha_seg_exch_offset());
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = warp / 3, r = warp - 3 * g;
     const int ul = g * 32 + lane;
     const uint32_t n_tiles = a.n_tiles;
-    const bool majority = a.flags & COAST_F_MAJORITY_D;
+    const bool majority = a.flags & COAST_F_MAJORITY_VOTER;
     uint32_t tile = blockIdx.x;
     if (tile < n_tiles) ring.issue(0, tile);
     Tally tally(a);
@@ -376,7 +381,7 @@ __device__ __forceinline__ void sha256_b64_seg_body(const xmr_args& a, const CUt
         m[0] = 0x80000000u; m[15] = 512u;
         sha_compress<INJECT>(st, m, fs1, fmask);
 
-        uint32_t* ex = exch + ((it & 1u) * SEG_GROUPS + g) * (2 * 8 * 32);
+        uint32_t* ex = exch + ((it & 1u) * SEG_GROUPS + g) * SEG_EXCH_WORDS;
         if (r > 0) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) ex[((r - 1) * 8 + i) * 32 + lane] = st[i];

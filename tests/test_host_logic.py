@@ -6,6 +6,7 @@ staging memory released, loud failures for bad arguments and for a non-sm_90 dev
 import ctypes as C
 import json
 import os
+import re
 import subprocess
 import sys
 
@@ -215,6 +216,51 @@ def test_tf32_gemm_kernel_selection_pairs_and_single(mock_dir, tmp_path, nc, M, 
         assert la["grid"] % 2 == 0
     tm = [e for e in ev if e["op"] == "tmap"]
     assert tm[1]["box_bytes"] == 32 * 32 * 4 * (2 if "tf32p" in want_name else 4), tm[1]
+
+
+def _declared_bounds():
+    """{kernel: (EIATTR_MAX_THREADS, EIATTR_CTA_PER_CLUSTER)} of the built cubin: its __launch_bounds__ and __cluster_dims__"""
+    elf = subprocess.run(["cuobjdump", "-elf", os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")],
+                         capture_output=True, text=True, check=True).stdout
+    bounds = {}
+    for sec in re.split(r"^(?=\.)", elf, flags=re.M):
+        m = re.match(r"\.nv\.info\.(xmr_\w+)", sec)
+        if m:
+            attr = lambda name: re.search(name + r"\s+Format:\s+\w+\s+Value:\s+0x([0-9a-f]+)", sec)
+            threads, cluster = attr("EIATTR_MAX_THREADS"), attr("EIATTR_CTA_PER_CLUSTER")
+            bounds[m.group(1)] = (int(threads.group(1), 16) if threads else None, int(cluster.group(1), 16) if cluster else 1)
+    return bounds
+
+
+def test_launches_use_the_kernels_declared_cta_size_and_whole_clusters(mock_dir, tmp_path):
+    """every protected launch's block size is the kernel's own __launch_bounds__, and a cluster kernel gets a grid of whole
+    clusters: the host's launch geometry and the kernels' layouts come from one header, this checks the compiled result"""
+    bounds = _declared_bounds()
+    ops = []
+    for nc in (1, 2, 3):
+        ops += [dict(op="launch", kernel=K_SHA256, nc=nc, n=5000, unit_bytes=64, in_bytes=320000, out_bytes=160000, flags=fl)
+                for fl in (0x8, 0x10)]
+        ops += [dict(op="launch", kernel=K_SHA256, nc=nc, n=500, unit_bytes=64, in_bytes=32016, out_bytes=16000, misalign=4)]
+        ops += [dict(op="launch", kernel=K_CRC16, nc=nc, n=5000, unit_bytes=ub, in_bytes=5000 * ub, out_bytes=10000) for ub in (64, 13)]
+        ops += [dict(op="launch", kernel=K_AES128, nc=nc, n=4096, mode=mode, in_bytes=65536, out_bytes=65536, aux_bytes=65536 if mode & 2 else 0)
+                for mode in range(4)]
+        ops += [dict(op="launch", kernel=K_MM_U32, nc=nc, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4, aux_bytes=K * N * 4, out_bytes=M * N * 4)
+                for M, N, K in ((256, 128, 256), (64, 128, 48), (9, 9, 9))]
+        ops += [dict(op="launch", kernel=K_GEMM_TF32, nc=nc, n=M * N, M=M, N=N, K=64, in_bytes=M * 256, aux_bytes=N * 256, out_bytes=M * N * 4)
+                for M, N in ((512, 512), (512, 384), (384, 512), (1280, 1024))]
+        ops += [dict(op="launch", kernel=K_QSORT, nc=nc, n=700, unit_bytes=400, in_bytes=280000, out_bytes=280000),
+                dict(op="launch", kernel=K_CHSTONE_SHA, nc=nc, n=30, unit_bytes=16384, in_bytes=30 * 16384, out_bytes=600)]
+        ops += [dict(op="launch", kernel=7, nc=nc, n=333, mode=mode, in_bytes=333 * 64, out_bytes=333 * 64) for mode in (0, 1)]
+    seen = set()
+    for env in ({}, {"COAST_GEMM_PAIR": "1", "COAST_QSORT_PATH": "nested"}, {"COAST_GEMM_PAIR": "0"}):
+        res, ev = run_child(mock_dir, tmp_path, ops, env_extra=env)
+        assert all(r["rc"] == 0 for r in res["ops"]), res
+        for la in (e for e in ev if e["op"] == "launch" and "_nc" in e["name"]):
+            threads, cluster = bounds[la["name"]]
+            assert la["block"] == threads and la["grid"] % cluster == 0, (la["name"], la["block"], la["grid"], threads, cluster)
+            seen.add(la["name"])
+    assert seen == {n for n in bounds if "_nc" in n and n.endswith("_inj0")}          # every protected kernel (inj1: same geometry)
+    assert sum(bounds[n][1] == 2 for n in seen) == 3
 
 
 def test_gemm_tuning_switches_reach_the_kernel_as_mode_bits(mock_dir, tmp_path):
