@@ -30,8 +30,14 @@ def host(t):
 
 
 def both(rt, oracle, kernel, nc, inp, n, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0, aux=None, key=None,
-         plan_kw=None, table=None, unit_base=0):
+         plan_kw=None, table=None, unit_base=0, status=False):
+    """One launch on the GPU and one oracle run on the same input: every output byte and all five counters must agree.
+    The GPU output starts as POISON_OUT bytes, so a unit the kernel skips fails.  status=True also passes a d_status buffer
+    poisoned with POISON_STATUS and checks it (check_status)."""
+    import os
+    import torch
     import coast_b200 as cb
+    from coast_b200.runtime import out_bytes
     oplan = gplan = None
     if table is not None:
         oplan = oracle.make_plan(oracle.PLAN_TABLE, table=table)
@@ -39,16 +45,48 @@ def both(rt, oracle, kernel, nc, inp, n, *, flags=0, mode=0, unit_bytes=0, M=0, 
     elif plan_kw:
         oplan = oracle.make_plan(oracle.PLAN_BERNOULLI, **plan_kw)
         gplan = cb.FaultPlan(mode=cb.PLAN_BERNOULLI, **plan_kw)     # seed + (p | threshold)
+    threads = (os.cpu_count() or 1) if n >= 1 << 14 else 1
     o_out, o_st = oracle.run(kernel, nc, inp, n, flags=flags, mode=mode, unit_bytes=unit_bytes, M=M, N=N, K=K, aux=aux,
-                             key=key, plan=oplan, unit_base=unit_base)
+                             key=key, plan=oplan, unit_base=unit_base, threads=threads)
+    out = torch.full((n * out_bytes(kernel, unit_bytes),), POISON_OUT, dtype=torch.uint8, device="cuda")
+    d_status = torch.full((n,), POISON_STATUS, dtype=torch.uint8, device="cuda") if status else None
     g_out, g_st = rt.run(kernel, nc, dev(rt, inp), n, flags=flags, mode=mode, unit_bytes=unit_bytes, M=M, N=N, K=K,
-                         aux=dev(rt, aux) if aux is not None else None, key=key, plan=gplan, unit_base=unit_base)
+                         aux=dev(rt, aux) if aux is not None else None, key=key, plan=gplan, unit_base=unit_base,
+                         out=out, status=d_status)
     g = host(g_out)
     assert g.tobytes() == o_out.tobytes(), f"output mismatch kernel={kernel} nc={nc} n={n}"
     gd = g_st.as_dict()
     for k in STAT_KEYS:
         assert gd[k] == o_st[k], (k, gd, o_st)
+    if status:
+        if table is not None:
+            hit = (table.astype(np.uint32) & np.uint32(0x80000000)) != 0
+        elif plan_kw:
+            from test_gpu_stream_exact import plan_hits
+            thr = plan_kw.get("threshold")
+            thr = thr if thr is not None else min(int(plan_kw["p"] * 2 ** 32), 0xFFFFFFFF)
+            hit = plan_hits(plan_kw["seed"], thr, unit_base, n).numpy()
+        else:
+            hit = np.zeros(n, dtype=bool)
+        check_status(d_status.cpu().numpy(), hit, nc, flags, gd)
     return g, gd
+
+
+POISON_OUT, POISON_STATUS = 0xA5, 0xEE
+
+
+def check_status(status, hit, nc, flags, st):
+    """d_status after a launch: one byte per unit, the count of disagreeing votes (saturating at 255).  Every byte was
+    written; it is zero without replicas and on units the plan does not hit; under DWC its nonzero bytes are the detected
+    units, under TMR with -countErrors its sum is the corrected-error count."""
+    assert (status != POISON_STATUS).all(), f"{int((status == POISON_STATUS).sum())} status bytes never written"
+    assert not status[~hit].any(), f"nonzero status on {int((status[~hit] != 0).sum())} units the plan does not hit"
+    if nc == 1:
+        assert not status.any()
+    elif nc == 2:
+        assert int((status != 0).sum()) == st["dwc_detected"]
+    elif flags & 1 and int(status.max(initial=0)) < 255:
+        assert int(status.astype(np.int64).sum()) == st["errors_corrected"]
 
 
 def msgs(oracle, n, nbytes, seed):
@@ -135,9 +173,9 @@ def test_sha256_unaligned_input_takes_general_path(rt, oracle):
 
 
 def test_sha256_full_size_properties(rt, oracle):
-    """BASELINE config 2: 2^20 x 64-byte messages.  Size-independent properties: digests equal hashlib on a
-    sample; TMR under a p=2^-6 fault plan gives bit-identical output to the fault-free run; counters equal the
-    oracle's on the first 2^15 units' worth of the same plan (prefix run with the same unit_base)."""
+    """BASELINE config 2: 2^20 x 64-byte messages, TMR under a p=2^-6 fault plan: every digest and all five counters equal
+    the oracle's run over the whole batch; the voted output equals the fault-free and the unprotected output."""
+    import os
     import torch
     import coast_b200 as cb
     n = 1 << 20
@@ -151,15 +189,9 @@ def test_sha256_full_size_properties(rt, oracle):
     assert abs(st1.injected - n / 64) < 6 * (n / 64) ** 0.5
     unp, _ = rt.run(cb.K_SHA256, 1, d_in, n, unit_bytes=64)
     assert torch.equal(clean, unp)
-    h_in = d_in.cpu().numpy()
-    h_out = clean.cpu().numpy()
-    for u in list(range(0, n, 65537)) + [n - 1]:
-        assert h_out[32 * u: 32 * u + 32].tobytes() == hashlib.sha256(h_in[64 * u: 64 * u + 64].tobytes()).digest()
-    k = 1 << 15
-    _, so = oracle.run(oracle.K_SHA256, 3, h_in[: 64 * k], k, unit_bytes=64, flags=3,
-                       plan=oracle.make_plan(oracle.PLAN_BERNOULLI, seed=22, p=2 ** -6), threads=8)
-    _, sg = rt.run(cb.K_SHA256, 3, d_in[: 64 * k], k, unit_bytes=64, flags=3, plan=plan)
-    assert sg.as_dict() == so
+    o_out, so = oracle.run(oracle.K_SHA256, 3, d_in.cpu().numpy(), n, unit_bytes=64, flags=3,
+                           plan=oracle.make_plan(oracle.PLAN_BERNOULLI, seed=22, p=2 ** -6), threads=os.cpu_count() or 1)
+    assert host(faulty).tobytes() == o_out.tobytes() and st1.as_dict() == so
 
 
 # ------------------------------------------------------------------------------------------ aes
@@ -218,8 +250,10 @@ def test_aes_decrypt_and_per_unit_keys_with_faults(rt, oracle):
 
 
 def test_aes_full_size_roundtrip_and_detect_rate(rt, oracle):
-    """BASELINE config 3: 2^24 blocks, DWC, Bernoulli(2^-10) flips.  Properties: decrypt(encrypt(x)) == x over the
-    full buffer; dwc_detected == injected (detect-rate parity: 100% of state flips); prefix counters == oracle."""
+    """BASELINE config 3: 2^24 blocks, DWC, Bernoulli(2^-10) flips.  decrypt(encrypt(x)) == x over the full buffer;
+    dwc_detected == injected (detect-rate parity: 100% of state flips); every block and all five counters of the faulty
+    run equal the oracle's run over the whole batch."""
+    import os
     import torch
     import coast_b200 as cb
     n = 1 << 24
@@ -234,11 +268,9 @@ def test_aes_full_size_roundtrip_and_detect_rate(rt, oracle):
     enc_f, st_f = rt.run(cb.K_AES128, 2, d_in, n, key=key, plan=plan)
     assert st_f.dwc_detected == st_f.injected
     assert abs(st_f.injected - n / 1024) < 6 * (n / 1024) ** 0.5
-    k = 1 << 16
-    o_out, so = oracle.run(oracle.K_AES128, 2, d_in[: 16 * k].cpu().numpy(), k, key=key,
-                           plan=oracle.make_plan(oracle.PLAN_BERNOULLI, seed=33, p=2 ** -10), threads=8)
-    g_out, sg = rt.run(cb.K_AES128, 2, d_in[: 16 * k], k, key=key, plan=plan)
-    assert sg.as_dict() == so and host(g_out).tobytes() == o_out.tobytes()
+    o_out, so = oracle.run(oracle.K_AES128, 2, d_in.cpu().numpy(), n, key=key,
+                           plan=oracle.make_plan(oracle.PLAN_BERNOULLI, seed=33, p=2 ** -10), threads=os.cpu_count() or 1)
+    assert st_f.as_dict() == so and host(enc_f).tobytes() == o_out.tobytes()
 
 
 # ------------------------------------------------------------------------------------------ crc16
@@ -262,6 +294,8 @@ def test_crc16_faults(rt, oracle, nc, length, n):
 
 
 def test_crc16_full_size(rt, oracle):
+    """2^20 x 64-byte messages: the unprotected run and TMR under a p=0.01 plan equal the oracle on every CRC and counter"""
+    import os
     import torch
     import coast_b200 as cb
     n = 1 << 20
@@ -270,9 +304,12 @@ def test_crc16_full_size(rt, oracle):
     a, _ = rt.run(cb.K_CRC16, 1, d_in, n, unit_bytes=64)
     b, st = rt.run(cb.K_CRC16, 3, d_in, n, unit_bytes=64, flags=3, plan=cb.FaultPlan(mode=cb.PLAN_BERNOULLI, seed=4, p=0.01))
     assert torch.equal(a, b) and st.errors_corrected == st.injected      # one u16 vote per unit; every crc/data flip shows
-    k = 1 << 14
-    o, _ = oracle.run(oracle.K_CRC16, 1, d_in[: 64 * k].cpu().numpy(), k, unit_bytes=64)
-    assert host(a[: 2 * k]).tobytes() == o.tobytes()
+    h_in, threads = d_in.cpu().numpy(), os.cpu_count() or 1
+    o, _ = oracle.run(oracle.K_CRC16, 1, h_in, n, unit_bytes=64, threads=threads)
+    assert host(a).tobytes() == o.tobytes()
+    o3, so = oracle.run(oracle.K_CRC16, 3, h_in, n, unit_bytes=64, flags=3,
+                        plan=oracle.make_plan(oracle.PLAN_BERNOULLI, seed=4, p=0.01), threads=threads)
+    assert host(b).tobytes() == o3.tobytes() and st.as_dict() == so
 
 
 # ------------------------------------------------------------------------------------------ matmul (exact)
