@@ -13,3 +13,4 @@
 #include "xmr_mm_tc.cuh"
 #include "xmr_qsort.cuh"
 #include "xmr_chstone_sha.cuh"
+#include "xmr_ragged.cuh"

@@ -505,6 +505,7 @@ typedef struct {
     map_desc map[2];
     size_t scratch;               /* stream-ordered scratch for the pre-pass and the maps */
     size_t scratch_per_cta;       /* plus this much per CTA of the grid, handed to the kernel as xmr_args.aux */
+    int scratch_as_aux;           /* hand the scratch to the kernel as xmr_args.aux even without per-CTA scratch */
     int (*prepass)(const coast_launch_desc* d, CUdeviceptr scratch, CUstream s);
 } launch_plan;
 
@@ -551,6 +552,36 @@ static int prepass_split_limbs(const coast_launch_desc* d, CUdeviceptr pa, CUstr
     return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
 }
 
+/* Ragged batches (COAST_UNIT_OFFSETS): the bound on every length, and the checks shared by coast_launch and coast_run_host. */
+static uint32_t ragged_bound_max(uint32_t kernel) { return kernel == COAST_K_CRC16 ? 255u : (1u << 28); }
+static int ragged_check(const coast_launch_desc* d) {
+    if (d->kernel != COAST_K_SHA256 && d->kernel != COAST_K_CRC16)
+        return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: ragged batches exist for CRC16 and SHA256 only (kernel %u)", d->kernel);
+    if (d->unit_bytes > ragged_bound_max(d->kernel))
+        return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: unit_bytes bounds every length and is at most %u for %s (got %u)",
+                    ragged_bound_max(d->kernel), KINFO[d->kernel].name, d->unit_bytes);
+    if (d->n_units >= (1ull << 32)) return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: n_units must be below 2^32");
+    if (!d->d_aux || (((uintptr_t)d->d_aux) & 7u))
+        return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: d_aux must point to n_units + 1 8-byte aligned uint64_t offsets");
+    return COAST_OK;
+}
+
+/* Cost-ordering pre-pass of the ragged kernels (xmr_ragged.cuh): zero the header and the bucket counts, histogram, one-CTA scan
+ * (which also stores the offset table's address in the header), scatter into the permutation.  All on the launch's stream. */
+static int prepass_ragged(const coast_launch_desc* d, CUdeviceptr scratch, CUstream s) {
+    DRV(p_cuMemsetD8Async(scratch, 0, XMR_RAGGED_PERM, s));
+    const void* off = d->d_aux;
+    unsigned long long n = d->n_units;
+    unsigned int bound = d->unit_bytes, sha = d->kernel == COAST_K_SHA256;
+    const uint64_t ctas = (n + XMR_CTA_THREADS - 1) / XMR_CTA_THREADS, cap = (uint64_t)G.sm_count * 8u;
+    const unsigned grid = (unsigned)(ctas < cap ? ctas : cap);
+    void* params[] = { &off, &n, &bound, &sha, &scratch };
+    int rc = launch_small("xmr_ragged_hist", grid, XMR_CTA_THREADS, params, s); if (rc) return rc;
+    void* params_scan[] = { &off, &scratch };
+    rc = launch_small("xmr_ragged_scan", 1, XMR_RAGGED_SCAN_THREADS, params_scan, s); if (rc) return rc;
+    return launch_small("xmr_ragged_scatter", grid, XMR_CTA_THREADS, params, s);
+}
+
 /* Scratch comes from the stream-ordered pool: allocated on the launch's stream and released on it after the kernel, so launches
  * on different streams never share it, and the pool keeps released memory cached (no driver allocation in steady state). */
 static int run_plan(const launch_plan* L, const coast_launch_desc* d, xmr_args* a, CUstream stream) {
@@ -562,7 +593,7 @@ static int run_plan(const launch_plan* L, const coast_launch_desc* d, xmr_args* 
     const size_t bytes = L->scratch + (size_t)grid * L->scratch_per_cta;
     CUdeviceptr scratch = 0;
     if (bytes) DRV(p_cuMemAllocFromPoolAsync(&scratch, bytes, G.pool, stream));
-    if (L->scratch_per_cta) a->aux = (const void*)scratch;
+    if (L->scratch_per_cta || L->scratch_as_aux) a->aux = (const void*)scratch;
     CUtensorMap maps[2];
     rc = L->prepass ? L->prepass(d, scratch, stream) : COAST_OK;
     for (int i = 0; i < L->n_maps && !rc; ++i) rc = encode_map(&L->map[i], scratch, L->cache_maps, &maps[i]);
@@ -583,6 +614,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     if (!d) return fail(COAST_ERR_BAD_ARG, "null descriptor");
     if (d->kernel >= COAST_K_COUNT_) return fail(COAST_ERR_BAD_ARG, "unknown kernel id %u", d->kernel);
     if (d->num_clones < 1 || d->num_clones > 3) return fail(COAST_ERR_BAD_ARG, "num_clones must be 1, 2 (DWC) or 3 (TMR)");
+    const int ragged = (d->mode & COAST_UNIT_OFFSETS) != 0;
+    if (ragged && (rc = ragged_check(d))) return rc;
     if (d->n_units == 0) return COAST_OK;
     if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null device buffer");
     const uint32_t nc = d->num_clones;
@@ -628,7 +661,9 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     switch (d->kernel) {
     case COAST_K_SHA256:
         if (((uintptr_t)d->d_out) & 15u) return fail(COAST_ERR_BAD_ARG, "SHA output must be 16-byte aligned");
-        if (!ring_ok) {
+        if (ragged) {
+            snprintf(L.name, sizeof L.name, "xmr_sha256_var_inj%d_nc%u", inj, nc);
+        } else if (!ring_ok) {
             snprintf(L.name, sizeof L.name, "xmr_sha256_gen_nc%u_inj%d", nc, inj);
         } else if (nc == 3 && !(d->flags & COAST_F_INTERLEAVE)) {
             /* TMR replica scheduling: -s (segmented, the reference default, interface.cpp:245-247) = replicas on
@@ -643,8 +678,12 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         }
         break;
     case COAST_K_CRC16:
+        if (ragged) {
+            snprintf(L.name, sizeof L.name, "xmr_crc16_var_inj%d_nc%u", inj, nc);
+            break;
+        }
         if (d->unit_bytes < 1 || d->unit_bytes > 255) return fail(COAST_ERR_BAD_ARG, "crc16 length is an unsigned char (1..255)");
-        if (ring_ok) {                                       /* table kernel: byte-step table and tile ring in shared memory */
+        if (ring_ok) {                                      /* table kernel: byte-step table and tile ring in shared memory */
             snprintf(L.name, sizeof L.name, "xmr_crc16_b64_nc%u_inj%d", nc, inj);
             L.block = xmr_crc_threads(nc); L.smem = xmr_crc_smem(nc);
             plan_ring(&L, &a, xmr_crc_tile_rows(nc), 64, 0, CU_TENSOR_MAP_SWIZZLE_64B);
@@ -759,7 +798,13 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     default:
         return fail(COAST_ERR_UNSUPPORTED, "kernel %u is not built into this library yet", d->kernel);
     }
-    if (!L.ctas) {                                           /* lane-interleaved kernels: each warp takes 32/nc units */
+    if (ragged) {                                            /* one resident wave pulling cost-ordered warp-tiles (xmr_ragged.cuh) */
+        L.waves = 1;
+        L.scratch = (size_t)xmr_ragged_scratch(d->n_units);
+        L.scratch_as_aux = 1;
+        L.prepass = prepass_ragged;
+    }
+    if (!L.ctas) {                                          /* lane-interleaved kernels: each warp takes 32/nc units */
         const uint64_t warps = (d->n_units + upw - 1) / upw, wpc = L.block / 32u;
         L.ctas = (warps + wpc - 1) / wpc;
     }
@@ -985,6 +1030,71 @@ fail:
     return drain_host_streams(rc);
 }
 
+/* Ragged host call (COAST_UNIT_OFFSETS, d_aux = the caller's host offsets): staged only.  A chunk is a contiguous unit range
+ * whose input, offset slice and outputs fit the chunk bytes (ramping 1, 2, 4, .. MiB up to COAST_HOST_CHUNK_BYTES, 16 MiB by
+ * default); a longer unit is a chunk of its own.  Each chunk uploads its bytes [off[first], off[end]) and its offset slice
+ * off[first .. end] unchanged, and launches with the staging slot's address minus off[first] as d_in (exact under u64
+ * wraparound), so the caller's offsets are never rewritten. */
+static uint64_t ragged_chunk_end(const uint64_t* off, uint64_t first, uint64_t n, uint64_t budget, uint64_t per_unit) {
+    uint64_t e = first + 1;
+    while (e < n && (off[e + 1] - off[first]) + (e + 1 - first) * per_unit <= budget) ++e;
+    return e;
+}
+static int run_host_ragged(const coast_launch_desc* d, coast_stats* out, int* dwc_fired) {
+    int rc = ragged_check(d); if (rc) return rc;
+    const char* hp = getenv("COAST_HOST_PATH");
+    if (hp && (!strcmp(hp, "zerocopy") || !strcmp(hp, "hybrid")))
+        return fail(COAST_ERR_UNSUPPORTED, "COAST_HOST_PATH=%s: ragged host calls (COAST_UNIT_OFFSETS) are staged only", hp);
+    if (d->n_units == 0) return sync_impl(G.hs[2], out, dwc_fired);
+    if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null host buffer");
+    const uint64_t* off = (const uint64_t*)d->d_aux, n = d->n_units;
+    for (uint64_t u = 0; u < n; ++u)
+        if (off[u + 1] < off[u] || off[u + 1] - off[u] > d->unit_bytes)
+            return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: unit %llu runs from offset %llu to %llu; offsets must not decrease and no "
+                                           "length may exceed unit_bytes (%u)", (unsigned long long)u, (unsigned long long)off[u],
+                        (unsigned long long)off[u + 1], d->unit_bytes);
+    const uint64_t ob = KINFO[d->kernel].out_bytes, per_unit = ob + 8u;
+    uint64_t max_chunk_bytes = 16ull << 20;
+    { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) max_chunk_bytes = (uint64_t)atoll(e); }
+    const uint64_t ramp0 = (1ull << 20) < max_chunk_bytes ? (1ull << 20) : max_chunk_bytes;
+    /* the schedule is walked twice: once to size the three slots (never regrown while a chunk may use them), once to run */
+    uint64_t max_span = 16, max_cnt = 1, n_chunks = 0;
+    for (uint64_t first = 0, budget = ramp0; first < n; ++n_chunks) {
+        const uint64_t e = ragged_chunk_end(off, first, n, budget, per_unit);
+        if (off[e] - off[first] > max_span) max_span = off[e] - off[first];
+        if (e - first > max_cnt) max_cnt = e - first;
+        first = e; budget = budget * 2 < max_chunk_bytes ? budget * 2 : max_chunk_bytes;
+    }
+    for (int s = 0; s < 3 && (uint64_t)s < n_chunks; ++s) {
+        if ((rc = slot_reserve(&G.h_in[s], &G.h_in_cap[s], (size_t)max_span))) return rc;
+        if ((rc = slot_reserve(&G.h_aux[s], &G.h_aux_cap[s], (size_t)(max_cnt + 1) * 8u))) return rc;
+        if ((rc = slot_reserve(&G.h_out[s], &G.h_out_cap[s], (size_t)(max_cnt * ob)))) return rc;
+        if (d->d_status && (rc = slot_reserve(&G.h_stat[s], &G.h_stat_cap[s], (size_t)max_cnt))) return rc;
+    }
+    int slot = 0;
+#define STEP(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) { rc = drv_fail(r_, #call); goto fail; } } while (0)
+    for (uint64_t first = 0, budget = ramp0; first < n; slot = (slot + 1) % 3) {
+        const uint64_t e = ragged_chunk_end(off, first, n, budget, per_unit), cnt = e - first, span = off[e] - off[first];
+        if (span) STEP(p_cuMemcpyHtoDAsync_v2(G.h_in[slot], (const uint8_t*)d->d_in + off[first], (size_t)span, G.hs[slot]));
+        STEP(p_cuMemcpyHtoDAsync_v2(G.h_aux[slot], off + first, (size_t)(cnt + 1) * 8u, G.hs[slot]));
+        coast_launch_desc c = *d;
+        c.d_in = (const void*)(uintptr_t)(G.h_in[slot] - off[first]);
+        c.d_aux = (const void*)G.h_aux[slot]; c.d_out = (void*)G.h_out[slot];
+        c.n_units = cnt; c.unit_base = d->unit_base + first;
+        if (d->d_status) c.d_status = (void*)G.h_stat[slot];
+        rc = launch_impl(&c, G.hs[slot]); if (rc) goto fail;
+        STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + first * ob, G.h_out[slot], (size_t)(cnt * ob), G.hs[slot]));
+        if (d->d_status) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_status + first, G.h_stat[slot], (size_t)cnt, G.hs[slot]));
+        first = e; budget = budget * 2 < max_chunk_bytes ? budget * 2 : max_chunk_bytes;
+    }
+#undef STEP
+    G.last_host_path = "staged";
+    DRV(p_cuStreamSynchronize(G.hs[0])); DRV(p_cuStreamSynchronize(G.hs[1]));
+    return sync_impl(G.hs[2], out, dwc_fired);
+fail:
+    return drain_host_streams(rc);
+}
+
 /* Matmul host call.  B (replicated operand) goes up once; C is produced in row blocks: block i's rows of A upload, its
  * launch and the download of its rows of C run on stream i % 3, so uploads, tensor-core work and downloads of
  * neighbouring blocks overlap (PCIe is full duplex).  The fault plan is keyed by the global element index
@@ -1036,6 +1146,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
     if (!d) return fail(COAST_ERR_BAD_ARG, "null descriptor");
     if (d->plan && d->plan->mode == COAST_PLAN_TABLE) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: TABLE plans need device pointers; use coast_launch");
     for (int i = 0; i < 3; ++i) if (!G.hs[i]) DRV(p_cuStreamCreate(&G.hs[i], CU_STREAM_NON_BLOCKING));
+    if (d->mode & COAST_UNIT_OFFSETS) return run_host_ragged(d, out, dwc_fired);
     const uint64_t ob = coast_out_bytes(d->kernel, d->unit_bytes);
     if (d->kernel == COAST_K_MM_U32 || d->kernel == COAST_K_GEMM_TF32) {
         if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");

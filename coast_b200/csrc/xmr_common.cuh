@@ -62,6 +62,31 @@ __device__ __forceinline__ Fault fault_for_unit(const xmr_args& a, uint32_t nc, 
     return f;
 }
 
+// The same decision with a per-unit site count (ragged batches: each unit has its own length).  A unit without sites is never
+// injected, and the Bernoulli draw is not taken modulo zero.
+template <class WidthFn>
+__device__ __forceinline__ Fault fault_for_unit(const xmr_args& a, uint32_t nc, uint64_t local, uint32_t n_sites, WidthFn width) {
+    Fault f{false, 0, 0, 0};
+    if (n_sites == 0u) return f;
+    if (a.plan_mode == 1u) {
+        uint64_t g = a.unit_base + local;
+        u4 x = philox4x32_10((uint32_t)g, (uint32_t)(g >> 32), 0u, 0u, a.seed_lo, a.seed_hi);
+        if (x.x < a.threshold) {
+            f.replica = x.y % nc;
+            f.site = x.z % n_sites;
+            f.bit = x.w % width(f.site);
+            f.active = true;
+        }
+    } else if (a.plan_mode == 2u) {
+        uint32_t e = __ldg(a.plan_table + local);
+        uint32_t rep = (e >> 29) & 3u, site = (e >> 5) & 0xFFFFFFu, bit = e & 31u;
+        if ((e & 0x80000000u) && rep < nc && site < n_sites && bit < width(site)) {
+            f.replica = rep; f.site = site; f.bit = bit; f.active = true;
+        }
+    }
+    return f;
+}
+
 // ---------------------------------------------------------------- lane geometry
 template <int NC> struct Lanes {
     static constexpr int kUnitsPerWarp = 32 / NC;           // 32, 16, 10 (lanes 30,31 idle under TMR)

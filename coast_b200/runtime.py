@@ -18,6 +18,7 @@ F_INTERLEAVE, F_SEGMENT, F_VERBOSE, F_MAJORITY_VOTER = 0x8, 0x10, 0x20, 0x100
 F_STORE_DATA_SYNC, F_NO_STORE_DATA_SYNC, F_NO_LOAD_SYNC, F_NO_STORE_ADDR_SYNC = 0x200, 0x400, 0x800, 0x1000
 PLAN_NONE, PLAN_BERNOULLI, PLAN_TABLE = 0, 1, 2
 AES_DECRYPT, AES_KEY_PER_UNIT, AES_KEY_WRITEBACK = 1, 2, 4
+UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 batches: aux = n_units + 1 u64 byte offsets into inp
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 
@@ -268,12 +269,30 @@ class Runtime:
     def run(self, kernel, num_clones, inp, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0, aux=None,
             key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, out=None, stream=None, status=None):
         torch = self.torch
+        if mode & UNIT_OFFSETS:
+            self._check_offsets(inp, aux, n_units, unit_bytes)
         if out is None:
             out = torch.empty(n_units * out_bytes(kernel, unit_bytes), dtype=torch.uint8, device=f"cuda:{self.device}")
         d = self.make_desc(kernel, num_clones, inp, out, n_units, flags=flags, mode=mode, unit_bytes=unit_bytes,
                            M=M, N=N, K=K, d_aux=aux, key=key, plan=plan, unit_base=unit_base, d_status=status)
         self.launch(d, stream)
         return out, self.sync(stream)
+
+    def _check_offsets(self, inp, aux, n_units, unit_bytes):
+        """A ragged batch's device offsets (int64 or uint64 tensor, n_units + 1 entries): they never decrease, no length
+        exceeds unit_bytes and the last one lies within inp.  The kernels only clamp; this catches a bad table before it runs."""
+        torch = self.torch
+        if aux is None or not hasattr(aux, "data_ptr") or aux.dtype not in (torch.int64, torch.uint64) or not aux.is_cuda:
+            raise CoastError(ERR_BAD_ARG, "UNIT_OFFSETS: aux must be a CUDA int64/uint64 tensor of n_units + 1 byte offsets")
+        if aux.numel() < n_units + 1 or not aux.is_contiguous():
+            raise CoastError(ERR_BAD_ARG, f"UNIT_OFFSETS: aux holds {aux.numel()} offsets, a contiguous n_units + 1 = {n_units + 1} are needed")
+        off = aux[: n_units + 1].view(torch.int64)
+        lens = off[1:] - off[:-1]
+        nbytes = inp.numel() * inp.element_size()
+        bad = torch.stack([(off < 0).any(), (lens < 0).any(), (lens > unit_bytes).any(), off[-1] > nbytes]).tolist()
+        if any(bad):
+            raise CoastError(ERR_BAD_ARG, "UNIT_OFFSETS: offsets must not decrease, no length may exceed unit_bytes "
+                                          f"({unit_bytes}) and the last offset must lie within inp ({nbytes} bytes)")
 
     # -- the reference-facing host call: HOST buffers, H2D + kernel + D2H inside ---------------
     def run_host(self, kernel, num_clones, h_in, h_out, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0,
