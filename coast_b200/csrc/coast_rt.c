@@ -553,13 +553,22 @@ static int prepass_split_limbs(const coast_launch_desc* d, CUdeviceptr pa, CUstr
 }
 
 /* Ragged batches (COAST_UNIT_OFFSETS): the bound on every length, and the checks shared by coast_launch and coast_run_host. */
-static uint32_t ragged_bound_max(uint32_t kernel) { return kernel == COAST_K_CRC16 ? 255u : (1u << 28); }
+static uint32_t ragged_bound_max(uint32_t kernel) {
+    return kernel == COAST_K_CRC16 ? 255u : kernel == COAST_K_QSORT ? 4096u : (1u << 28);
+}
 static int ragged_check(const coast_launch_desc* d) {
-    if (d->kernel != COAST_K_SHA256 && d->kernel != COAST_K_CRC16)
-        return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: ragged batches exist for CRC16 and SHA256 only (kernel %u)", d->kernel);
+    if (d->kernel != COAST_K_SHA256 && d->kernel != COAST_K_CRC16 && d->kernel != COAST_K_QSORT)
+        return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: ragged batches exist for CRC16, SHA256 and QSORT only (kernel %u)", d->kernel);
     if (d->unit_bytes > ragged_bound_max(d->kernel))
         return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: unit_bytes bounds every length and is at most %u for %s (got %u)",
                     ragged_bound_max(d->kernel), KINFO[d->kernel].name, d->unit_bytes);
+    if (d->kernel == COAST_K_QSORT) {                        /* int32 arrays: whole elements, aligned buffers */
+        if (d->unit_bytes == 0 || (d->unit_bytes & 3u))
+            return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: quicksort's unit_bytes bounds every array and is a multiple of 4 in "
+                                           "4..4096 (got %u)", d->unit_bytes);
+        if ((((uintptr_t)d->d_in) & 3u) || (((uintptr_t)d->d_out) & 3u))
+            return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: quicksort's d_in and d_out must be 4-byte aligned");
+    }
     if (d->n_units >= (1ull << 32)) return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: n_units must be below 2^32");
     if (!d->d_aux || (((uintptr_t)d->d_aux) & 7u))
         return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: d_aux must point to n_units + 1 8-byte aligned uint64_t offsets");
@@ -572,10 +581,12 @@ static int prepass_ragged(const coast_launch_desc* d, CUdeviceptr scratch, CUstr
     DRV(p_cuMemsetD8Async(scratch, 0, XMR_RAGGED_PERM, s));
     const void* off = d->d_aux;
     unsigned long long n = d->n_units;
-    unsigned int bound = d->unit_bytes, sha = d->kernel == COAST_K_SHA256;
+    unsigned int bound = d->unit_bytes;
+    unsigned int kind = d->kernel == COAST_K_SHA256 ? XMR_RAGGED_COST_SHA : d->kernel == COAST_K_QSORT ? XMR_RAGGED_COST_QSORT
+                                                                                                       : XMR_RAGGED_COST_CRC;
     const uint64_t ctas = (n + XMR_CTA_THREADS - 1) / XMR_CTA_THREADS, cap = (uint64_t)G.sm_count * 8u;
     const unsigned grid = (unsigned)(ctas < cap ? ctas : cap);
-    void* params[] = { &off, &n, &bound, &sha, &scratch };
+    void* params[] = { &off, &n, &bound, &kind, &scratch };
     int rc = launch_small("xmr_ragged_hist", grid, XMR_CTA_THREADS, params, s); if (rc) return rc;
     void* params_scan[] = { &off, &scratch };
     rc = launch_small("xmr_ragged_scan", 1, XMR_RAGGED_SCAN_THREADS, params_scan, s); if (rc) return rc;
@@ -738,9 +749,15 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     case COAST_K_QSORT:
         if (d->unit_bytes < 4 || (d->unit_bytes & 3u) || d->unit_bytes > 4096u)
             return fail(COAST_ERR_BAD_ARG, "quicksort arrays are 1..1024 int32 (unit_bytes = 4*L, got %u)", d->unit_bytes);
-        {   /* two schedulings of the same algorithm (xmr_qsort.cuh): per-unit state machine (default) or nested loops */
+        {   /* two schedulings of the same algorithm (xmr_qsort.cuh): per-unit state machine (default) or nested loops; a ragged
+             * batch has the state machine over cost-ordered warp-tiles only (xmr_ragged.cuh) */
             const char* path = getenv("COAST_QSORT_PATH");
-            snprintf(L.name, sizeof L.name, "%s_nc%u_inj%d", path && !strcmp(path, "nested") ? "xmr_qsortn" : "xmr_qsort", nc, inj);
+            const int nested = path && !strcmp(path, "nested");
+            if (ragged && nested)
+                return fail(COAST_ERR_UNSUPPORTED, "COAST_QSORT_PATH=nested: ragged quicksort batches (COAST_UNIT_OFFSETS) run the "
+                                                   "state-machine scheduling only");
+            if (ragged) snprintf(L.name, sizeof L.name, "xmr_qsort_var_inj%d_nc%u", inj, nc);
+            else snprintf(L.name, sizeof L.name, "%s_nc%u_inj%d", nested ? "xmr_qsortn" : "xmr_qsort", nc, inj);
         }
         /* one resident wave of persistent warps, each with a private copy of every replica's array, lane-major and CONTIGUOUS
          * per lane (a scan walks one cache line per 32 elements; thread-local memory would put a lane's elements 128 bytes apart) */
@@ -800,7 +817,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     }
     if (ragged) {                                            /* one resident wave pulling cost-ordered warp-tiles (xmr_ragged.cuh) */
         L.waves = 1;
-        L.scratch = (size_t)xmr_ragged_scratch(d->n_units);
+        /* quicksort: the per-warp slots (scratch_per_cta) follow the ragged part in the same allocation */
+        L.scratch = (size_t)(d->kernel == COAST_K_QSORT ? xmr_ragged_slots(d->n_units) : xmr_ragged_scratch(d->n_units));
         L.scratch_as_aux = 1;
         L.prepass = prepass_ragged;
     }
@@ -1034,10 +1052,13 @@ fail:
  * whose input, offset slice and outputs fit the chunk bytes (ramping 1, 2, 4, .. MiB up to COAST_HOST_CHUNK_BYTES, 16 MiB by
  * default); a longer unit is a chunk of its own.  Each chunk uploads its bytes [off[first], off[end]) and its offset slice
  * off[first .. end] unchanged, and launches with the staging slot's address minus off[first] as d_in (exact under u64
- * wraparound), so the caller's offsets are never rewritten. */
-static uint64_t ragged_chunk_end(const uint64_t* off, uint64_t first, uint64_t n, uint64_t budget, uint64_t per_unit) {
+ * wraparound), so the caller's offsets are never rewritten.  Quicksort writes its arrays in place of the input bytes: a chunk's
+ * output is the same span, downloaded to d_out + off[first] from an output slot biased the same way.  `span_copies` counts
+ * the span once (SHA-256, CRC16) or twice (quicksort: in and out) in the chunk budget. */
+static uint64_t ragged_chunk_end(const uint64_t* off, uint64_t first, uint64_t n, uint64_t budget, uint64_t per_unit,
+                                 uint64_t span_copies) {
     uint64_t e = first + 1;
-    while (e < n && (off[e + 1] - off[first]) + (e + 1 - first) * per_unit <= budget) ++e;
+    while (e < n && (off[e + 1] - off[first]) * span_copies + (e + 1 - first) * per_unit <= budget) ++e;
     return e;
 }
 static int run_host_ragged(const coast_launch_desc* d, coast_stats* out, int* dwc_fired) {
@@ -1048,19 +1069,25 @@ static int run_host_ragged(const coast_launch_desc* d, coast_stats* out, int* dw
     if (d->n_units == 0) return sync_impl(G.hs[2], out, dwc_fired);
     if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null host buffer");
     const uint64_t* off = (const uint64_t*)d->d_aux, n = d->n_units;
+    const int qs = d->kernel == COAST_K_QSORT;
     for (uint64_t u = 0; u < n; ++u)
         if (off[u + 1] < off[u] || off[u + 1] - off[u] > d->unit_bytes)
             return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: unit %llu runs from offset %llu to %llu; offsets must not decrease and no "
                                            "length may exceed unit_bytes (%u)", (unsigned long long)u, (unsigned long long)off[u],
                         (unsigned long long)off[u + 1], d->unit_bytes);
-    const uint64_t ob = KINFO[d->kernel].out_bytes, per_unit = ob + 8u;
+    if (qs)
+        for (uint64_t u = 0; u <= n; ++u)
+            if (off[u] & 3u)
+                return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: offset %llu is %llu; quicksort offsets must be multiples of 4",
+                            (unsigned long long)u, (unsigned long long)off[u]);
+    const uint64_t ob = KINFO[d->kernel].out_bytes, per_unit = ob + 8u, span_copies = qs ? 2u : 1u;
     uint64_t max_chunk_bytes = 16ull << 20;
     { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) max_chunk_bytes = (uint64_t)atoll(e); }
     const uint64_t ramp0 = (1ull << 20) < max_chunk_bytes ? (1ull << 20) : max_chunk_bytes;
     /* the schedule is walked twice: once to size the three slots (never regrown while a chunk may use them), once to run */
     uint64_t max_span = 16, max_cnt = 1, n_chunks = 0;
     for (uint64_t first = 0, budget = ramp0; first < n; ++n_chunks) {
-        const uint64_t e = ragged_chunk_end(off, first, n, budget, per_unit);
+        const uint64_t e = ragged_chunk_end(off, first, n, budget, per_unit, span_copies);
         if (off[e] - off[first] > max_span) max_span = off[e] - off[first];
         if (e - first > max_cnt) max_cnt = e - first;
         first = e; budget = budget * 2 < max_chunk_bytes ? budget * 2 : max_chunk_bytes;
@@ -1068,22 +1095,24 @@ static int run_host_ragged(const coast_launch_desc* d, coast_stats* out, int* dw
     for (int s = 0; s < 3 && (uint64_t)s < n_chunks; ++s) {
         if ((rc = slot_reserve(&G.h_in[s], &G.h_in_cap[s], (size_t)max_span))) return rc;
         if ((rc = slot_reserve(&G.h_aux[s], &G.h_aux_cap[s], (size_t)(max_cnt + 1) * 8u))) return rc;
-        if ((rc = slot_reserve(&G.h_out[s], &G.h_out_cap[s], (size_t)(max_cnt * ob)))) return rc;
+        if ((rc = slot_reserve(&G.h_out[s], &G.h_out_cap[s], (size_t)(qs ? max_span : max_cnt * ob)))) return rc;
         if (d->d_status && (rc = slot_reserve(&G.h_stat[s], &G.h_stat_cap[s], (size_t)max_cnt))) return rc;
     }
     int slot = 0;
 #define STEP(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) { rc = drv_fail(r_, #call); goto fail; } } while (0)
     for (uint64_t first = 0, budget = ramp0; first < n; slot = (slot + 1) % 3) {
-        const uint64_t e = ragged_chunk_end(off, first, n, budget, per_unit), cnt = e - first, span = off[e] - off[first];
+        const uint64_t e = ragged_chunk_end(off, first, n, budget, per_unit, span_copies), cnt = e - first, span = off[e] - off[first];
         if (span) STEP(p_cuMemcpyHtoDAsync_v2(G.h_in[slot], (const uint8_t*)d->d_in + off[first], (size_t)span, G.hs[slot]));
         STEP(p_cuMemcpyHtoDAsync_v2(G.h_aux[slot], off + first, (size_t)(cnt + 1) * 8u, G.hs[slot]));
         coast_launch_desc c = *d;
         c.d_in = (const void*)(uintptr_t)(G.h_in[slot] - off[first]);
-        c.d_aux = (const void*)G.h_aux[slot]; c.d_out = (void*)G.h_out[slot];
+        c.d_aux = (const void*)G.h_aux[slot];
+        c.d_out = qs ? (void*)(uintptr_t)(G.h_out[slot] - off[first]) : (void*)G.h_out[slot];
         c.n_units = cnt; c.unit_base = d->unit_base + first;
         if (d->d_status) c.d_status = (void*)G.h_stat[slot];
         rc = launch_impl(&c, G.hs[slot]); if (rc) goto fail;
-        STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + first * ob, G.h_out[slot], (size_t)(cnt * ob), G.hs[slot]));
+        if (qs) { if (span) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + off[first], G.h_out[slot], (size_t)span, G.hs[slot])); }
+        else STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + first * ob, G.h_out[slot], (size_t)(cnt * ob), G.hs[slot]));
         if (d->d_status) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_status + first, G.h_stat[slot], (size_t)cnt, G.hs[slot]));
         first = e; budget = budget * 2 < max_chunk_bytes ? budget * 2 : max_chunk_bytes;
     }

@@ -98,16 +98,24 @@ XMR_GEOM_FN unsigned xmr_mmtc_smem(unsigned nc) {
 /* ---- quicksort: persistent warps, each with a private scratch slot ---- */
 #define XMR_QSORT_THREADS 128
 
-/* ---- ragged SHA-256 / CRC16 (COAST_UNIT_OFFSETS): a counting-sort pre-pass orders the units by cost, longest first, then a
- * persistent grid of XMR_CTA_THREADS CTAs pulls warp-tiles of consecutive permuted units from a counter.  Scratch layout:
+/* ---- ragged SHA-256 / CRC16 / quicksort (COAST_UNIT_OFFSETS): a counting-sort pre-pass orders the units by cost, longest
+ * first, then a persistent grid pulls warp-tiles of consecutive permuted units from a counter (CTAs of XMR_CTA_THREADS for
+ * SHA-256 and CRC16, XMR_QSORT_THREADS for quicksort).  Scratch layout:
  *   [0, 64)                 header: the offset table's address (u64) and the warp-tile counter (u32)
  *   [64, 64 + 4 * BUCKETS)  per-cost-bucket counts, then (after the scan) each bucket's next free slot
  *   [XMR_RAGGED_PERM, ..)   the permutation, one u32 unit index per unit
- * Costs: SHA-256 compressions (nblk, the top bucket takes every nblk >= BUCKETS - 1), CRC16 bytes (0..255). */
+ *   quicksort only: from xmr_ragged_slots(n), 128-byte aligned, one slot of 32 x unit_bytes per warp of the grid (each lane
+ *   group's NC x L copies sized by the bound, as in the uniform kernel)
+ * Costs (XMR_RAGGED_COST_*): CRC16 bytes (0..255), SHA-256 compressions (nblk, the top bucket takes every nblk >= BUCKETS - 1),
+ * quicksort elements (0..1024, the top bucket takes 1023 and 1024). */
 #define XMR_RAGGED_BUCKETS      1024u
 #define XMR_RAGGED_HDR          64u
 #define XMR_RAGGED_PERM         (XMR_RAGGED_HDR + 4u * XMR_RAGGED_BUCKETS)
 #define XMR_RAGGED_SCAN_THREADS 1024         /* the one-CTA scan: one thread per bucket */
+#define XMR_RAGGED_COST_CRC     0u
+#define XMR_RAGGED_COST_SHA     1u
+#define XMR_RAGGED_COST_QSORT   2u
 XMR_GEOM_FN unsigned long long xmr_ragged_scratch(unsigned long long n_units) { return XMR_RAGGED_PERM + 4ull * n_units; }
+XMR_GEOM_FN unsigned long long xmr_ragged_slots(unsigned long long n_units) { return (xmr_ragged_scratch(n_units) + 127ull) & ~127ull; }
 
 #endif

@@ -12,6 +12,7 @@
 // lane-major slot per replica tripled the lines a TMR warp touches (L1 thrash at 44 warps per SM: 16-21 ms).
 // SoR exit: one vote per stored element.
 // Unit = one array of L = unit_bytes/4 ints (L <= 1024; the reference sorts 580).  Recursion = explicit stack, left first.
+// Ragged batches (xmr_ragged.cuh) run the same qsort_step / qsort_exit over arrays of per-unit length.
 // Fault sites: s < 32L: the value loaded for the s-th executed data comparison; 32L <= s < 33L: element s-32L of the
 // replica's private copy before sorting.  The CPU checker under oracle/ uses the identical enumeration, guards and order.
 #pragma once
@@ -158,6 +159,114 @@ __device__ __forceinline__ void qsort_nested_body(const xmr_args& a) {
 // numbering of the fault sites and every counter are unchanged (same oracle, same tests).
 enum : uint32_t { QS_POP = 0u, QS_SCAN_I = 1u, QS_SCAN_J = 2u, QS_DONE = 3u };
 
+// The control state of one unit in the state machine (the NC replica lanes of a unit hold equal copies of it).
+struct QsState {
+    uint32_t ndis = 0, syncs = 0, ev = 0;                       // disagreeing branch votes, executed sync points, compare events
+    uint32_t phase = QS_DONE;
+    uint32_t off = 0, len = 0;
+    int32_t pivot = 0, i = 0, j = 0;
+    int sp = 0;
+};
+
+// One iteration of the warp loop: the data-dependent condition of this lane's unit, the warp ballot (ALL 32 lanes call this),
+// the unit's vote over its NC bits and one step of its control flow.  `at(e)` is element e of this lane's replica, `stack`
+// its explicit recursion stack, (fsite, fmask) its injected compare event.  Shared by the uniform and the ragged kernels.
+template <int NC, bool INJECT, class At>
+__device__ __forceinline__ void qsort_step(QsState& s, const At& at, uint32_t* stack, int base, bool majority, uint32_t fsite,
+                                           uint32_t fmask) {
+    // ---- the data-dependent condition of this step (false for units that are between partitions)
+    const bool scan_i = s.phase == QS_SCAN_I, scan_j = s.phase == QS_SCAN_J;
+    bool c = false;
+    if (scan_i || scan_j) {
+        int32_t v = at(s.off + (uint32_t)(scan_i ? s.i : s.j));
+        if (INJECT && fsite == s.ev) v ^= (int32_t)fmask;
+        ++s.ev;
+        c = scan_i ? (v < s.pivot) : (v > s.pivot);
+        if (scan_i ? (s.i >= (int32_t)s.len - 1) : (s.j <= 0)) c = false;   // trap guard: a mis-steered scan stops at the partition edge
+    }
+    const uint32_t bal = __ballot_sync(0xFFFFFFFFu, c);
+    bool voted = c;
+    if (NC >= 2) {
+        const uint32_t c0 = (bal >> base) & 1u, c1 = (bal >> (base + 1)) & 1u;
+        if (NC == 2) { if (c0 != c1) s.ndis++; voted = c0 != 0u; }
+        else {
+            const uint32_t c2 = (bal >> (base + 2)) & 1u;
+            const bool c01 = c0 == c1, c02 = c0 == c2;
+            if (!(c01 && c02)) s.ndis++;
+            voted = (majority ? ((c0 & c1) | (c0 & c2) | (c1 & c2)) : (c01 ? c0 : c2)) != 0u;
+        }
+    }
+    // ---- advance this unit by one step
+    if (scan_i) {
+        s.syncs++;
+        if (voted) s.i++; else s.phase = QS_SCAN_J;             // while (at(i) < pivot) i++;   :126
+    } else if (scan_j) {
+        s.syncs++;
+        if (voted) s.j--;                                       // while (at(j) > pivot) j--;   :127
+        else {
+            s.syncs++;                                          // if (i >= j) break;   :128 -- indices always agree
+            if (s.i < s.j) {
+                const int32_t t = at(s.off + (uint32_t)s.i); at(s.off + (uint32_t)s.i) = at(s.off + (uint32_t)s.j); at(s.off + (uint32_t)s.j) = t;   // :129-131, own copy
+                s.i++; s.j--; s.phase = QS_SCAN_I;              // for (;; i++, j--)   :125
+            } else {
+                if (s.i < 1) s.i = 1;
+                if (s.i > (int32_t)s.len - 1) s.i = (int32_t)s.len - 1;
+                stack[s.sp++] = ((s.off + (uint32_t)s.i) << 16) | (s.len - (uint32_t)s.i);   // quick_sort(A + i, len - i)  :135 (later)
+                s.len = (uint32_t)s.i;                                                        // quick_sort(A, i)            :134 (now)
+                s.syncs++;                                      // its `if (len < 2) return;`   :122
+                if (s.len < 2) s.phase = QS_POP;
+                else { s.pivot = at(s.off + s.len / 2); s.i = 0; s.j = (int32_t)s.len - 1; s.phase = QS_SCAN_I; }   // :123-125
+            }
+        }
+    } else if (s.phase == QS_POP) {
+        if (s.sp == 0) s.phase = QS_DONE;
+        else {
+            const uint32_t top = stack[--s.sp];
+            s.off = top >> 16; s.len = top & 0xFFFFu;
+            s.syncs++;                                          // `if (len < 2) return;`   :122
+            if (s.len >= 2) { s.pivot = at(s.off + s.len / 2); s.i = 0; s.j = (int32_t)s.len - 1; s.phase = QS_SCAN_I; }
+        }
+    }
+}
+
+// SoR exit of a sorted unit of L elements: one vote per stored element into dst[0 .. L), then the unit's counters and its
+// d_status byte.  The NC lanes of the unit (gmask) call this together.
+template <int NC, class At>
+__device__ __forceinline__ void qsort_exit(const xmr_args& a, Tally& tally, const QsState& s, const At& at, uint32_t L, int32_t* dst,
+                                           unsigned long long local, uint32_t gmask, int base, int r, bool majority) {
+    uint32_t bad = 0;
+    for (uint32_t e = 0; e < L; ++e) {
+        const int32_t x = at(e);
+        int32_t v = x;
+        if (NC >= 2) {
+            const int32_t r1 = __shfl_sync(gmask, x, base + 1);
+            const int32_t r0 = __shfl_sync(gmask, x, base);
+            if (NC == 2) { bad += r0 != r1; v = r0; }
+            else {
+                const int32_t r2 = __shfl_sync(gmask, x, base + 2);
+                const bool c01 = r0 == r1, c02 = r0 == r2;
+                v = majority ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
+                bad += (c01 && c02) ? 0u : 1u;
+            }
+        }
+        if (r == 0) dst[e] = v;
+    }
+    if (r == 0) {
+        const unsigned long long gunit = a.unit_base + local;
+        if (NC == 3) {
+            if (a.flags & COAST_F_COUNT_ERRORS) {
+                tally.errors += bad + s.ndis;
+                if (a.flags & COAST_F_COUNT_SYNCS) tally.syncs += s.syncs + L;
+            }
+        } else if (NC == 2) {
+            tally.dwc += (bad || s.ndis) ? 1u : 0u;
+        }
+        const uint32_t dis = bad + s.ndis;
+        if (NC > 1 && dis && gunit < tally.first) tally.first = gunit;
+        if (tally.status) tally.status[local] = (unsigned char)(NC > 1 ? (dis > 255u ? 255u : dis) : 0u);
+    }
+}
+
 template <int NC, bool INJECT>
 __device__ __forceinline__ void qsort_body(const xmr_args& a) {
     constexpr int UPW = Lanes<NC>::kUnitsPerWarp;
@@ -190,103 +299,12 @@ __device__ __forceinline__ void qsort_body(const xmr_args& a) {
                 if (fsite >= 32u * L && fsite != 0xFFFFFFFFu) at(fsite - 32u * L) ^= (int32_t)fmask;
             }
         }
-        uint32_t ndis = 0, syncs = 0, ev = 0;                   // disagreeing branch votes, executed sync points, compare events
-        uint32_t phase = valid ? QS_POP : QS_DONE;
-        uint32_t off = 0, len = 0;
-        int32_t pivot = 0, i = 0, j = 0;
-        int sp = 0;
-        if (valid) stack[sp++] = L;                             // quick_sort(A, n): off = 0
+        QsState s;
+        s.phase = valid ? QS_POP : QS_DONE;
+        if (valid) stack[s.sp++] = L;                           // quick_sort(A, n): off = 0
         __syncwarp();
-        while (__any_sync(0xFFFFFFFFu, phase != QS_DONE)) {
-            // ---- the data-dependent condition of this step (false for units that are between partitions)
-            const bool scan_i = phase == QS_SCAN_I, scan_j = phase == QS_SCAN_J;
-            bool c = false;
-            if (scan_i || scan_j) {
-                int32_t v = at(off + (uint32_t)(scan_i ? i : j));
-                if (INJECT && fsite == ev) v ^= (int32_t)fmask;
-                ++ev;
-                c = scan_i ? (v < pivot) : (v > pivot);
-                if (scan_i ? (i >= (int32_t)len - 1) : (j <= 0)) c = false;   // trap guard: a mis-steered scan stops at the partition edge
-            }
-            const uint32_t bal = __ballot_sync(0xFFFFFFFFu, c);
-            bool voted = c;
-            if (NC >= 2) {
-                const uint32_t c0 = (bal >> base) & 1u, c1 = (bal >> (base + 1)) & 1u;
-                if (NC == 2) { if (c0 != c1) ndis++; voted = c0 != 0u; }
-                else {
-                    const uint32_t c2 = (bal >> (base + 2)) & 1u;
-                    const bool c01 = c0 == c1, c02 = c0 == c2;
-                    if (!(c01 && c02)) ndis++;
-                    voted = (majority ? ((c0 & c1) | (c0 & c2) | (c1 & c2)) : (c01 ? c0 : c2)) != 0u;
-                }
-            }
-            // ---- advance this unit by one step
-            if (scan_i) {
-                syncs++;
-                if (voted) i++; else phase = QS_SCAN_J;         // while (at(i) < pivot) i++;   :126
-            } else if (scan_j) {
-                syncs++;
-                if (voted) j--;                                 // while (at(j) > pivot) j--;   :127
-                else {
-                    syncs++;                                    // if (i >= j) break;   :128 -- indices always agree
-                    if (i < j) {
-                        const int32_t t = at(off + (uint32_t)i); at(off + (uint32_t)i) = at(off + (uint32_t)j); at(off + (uint32_t)j) = t;   // :129-131, own copy
-                        i++; j--; phase = QS_SCAN_I;            // for (;; i++, j--)   :125
-                    } else {
-                        if (i < 1) i = 1;
-                        if (i > (int32_t)len - 1) i = (int32_t)len - 1;
-                        stack[sp++] = ((off + (uint32_t)i) << 16) | (len - (uint32_t)i);   // quick_sort(A + i, len - i)  :135 (later)
-                        len = (uint32_t)i;                                                  // quick_sort(A, i)            :134 (now)
-                        syncs++;                                // its `if (len < 2) return;`   :122
-                        if (len < 2) phase = QS_POP;
-                        else { pivot = at(off + len / 2); i = 0; j = (int32_t)len - 1; phase = QS_SCAN_I; }   // :123-125
-                    }
-                }
-            } else if (phase == QS_POP) {
-                if (sp == 0) phase = QS_DONE;
-                else {
-                    const uint32_t top = stack[--sp];
-                    off = top >> 16; len = top & 0xFFFFu;
-                    syncs++;                                    // `if (len < 2) return;`   :122
-                    if (len >= 2) { pivot = at(off + len / 2); i = 0; j = (int32_t)len - 1; phase = QS_SCAN_I; }
-                }
-            }
-        }
-        if (valid) {
-            // SoR exit: one vote per stored element
-            int32_t* dst = static_cast<int32_t*>(a.out) + local * L;
-            uint32_t bad = 0;
-            for (uint32_t e = 0; e < L; ++e) {
-                const int32_t x = at(e);
-                int32_t v = x;
-                if (NC >= 2) {
-                    const int32_t r1 = __shfl_sync(gmask, x, base + 1);
-                    const int32_t r0 = __shfl_sync(gmask, x, base);
-                    if (NC == 2) { bad += r0 != r1; v = r0; }
-                    else {
-                        const int32_t r2 = __shfl_sync(gmask, x, base + 2);
-                        const bool c01 = r0 == r1, c02 = r0 == r2;
-                        v = majority ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
-                        bad += (c01 && c02) ? 0u : 1u;
-                    }
-                }
-                if (r == 0) dst[e] = v;
-            }
-            if (r == 0) {
-                const unsigned long long gunit = a.unit_base + local;
-                if (NC == 3) {
-                    if (a.flags & COAST_F_COUNT_ERRORS) {
-                        tally.errors += bad + ndis;
-                        if (a.flags & COAST_F_COUNT_SYNCS) tally.syncs += syncs + L;
-                    }
-                } else if (NC == 2) {
-                    tally.dwc += (bad || ndis) ? 1u : 0u;
-                }
-                const uint32_t dis = bad + ndis;
-                if (NC > 1 && dis && gunit < tally.first) tally.first = gunit;
-                if (tally.status) tally.status[local] = (unsigned char)(NC > 1 ? (dis > 255u ? 255u : dis) : 0u);
-            }
-        }
+        while (__any_sync(0xFFFFFFFFu, s.phase != QS_DONE)) qsort_step<NC, INJECT>(s, at, stack, base, majority, fsite, fmask);
+        if (valid) qsort_exit<NC>(a, tally, s, at, L, static_cast<int32_t*>(a.out) + local * L, local, gmask, base, r, majority);
         __syncwarp();
     }
     tally.flush(a.counters);

@@ -1,12 +1,13 @@
-// xmr_ragged.cuh -- ragged batches of SHA-256 and CRC16 (COAST_UNIT_OFFSETS in coast_rt.h).
+// xmr_ragged.cuh -- ragged batches of SHA-256, CRC16 and quicksort (COAST_UNIT_OFFSETS in coast_rt.h).
 //
 // n messages lie end to end in one buffer; n + 1 u64 byte offsets say where each starts.  Unit u hashes d_in[off[u] ..
 // off[u+1]) with exactly what a single-unit launch of that length does (same compressions / byte steps, same fault sites,
 // same votes and counters), so the per-message bodies reuse the building blocks of xmr_sha256.cuh and xmr_crc16.cuh.
+// Quicksort units are int32 arrays, sorted into the same byte range of d_out by the state machine of xmr_qsort.cuh.
 //
 // Schedule.  A warp runs as long as its longest unit, so with mixed lengths the lanes of short units idle.  A stream-ordered
 // counting sort orders the units by cost first (xmr_ragged_hist -> xmr_ragged_scan -> xmr_ragged_scatter: a histogram with
-// shared-memory atomics, a one-CTA exclusive scan in DESCENDING cost order, a scatter into a u32 permutation).  The hash
+// shared-memory atomics, a one-CTA exclusive scan in DESCENDING cost order, a scatter into a u32 permutation).  The unit
 // kernels then run a persistent grid whose warps pull warp-tiles of consecutive permuted units from a counter: neighbours
 // in a tile cost about the same, the longest units go first and the short ones fill the tail.  The order inside a bucket may
 // differ between runs; nothing observable depends on it (every unit is independent, first_fault_unit is a minimum).
@@ -16,6 +17,7 @@
 #pragma once
 #include "xmr_sha256.cuh"
 #include "xmr_crc16.cuh"
+#include "xmr_qsort.cuh"
 
 namespace xmr {
 
@@ -26,17 +28,28 @@ struct RaggedHdr {
 static_assert(sizeof(RaggedHdr) <= XMR_RAGGED_HDR && XMR_RAGGED_SCAN_THREADS == XMR_RAGGED_BUCKETS,
               "the header fits its slot; the scan has one thread per cost bucket");
 
-// length of unit u, clamped to [0, bound]; a decreasing pair counts as 0, so a malformed table never makes a unit read
-// past off[u] + bound
+// Offset u as a unit boundary.  Units of ELEM-byte elements (quicksort: 4) start on element boundaries: the low bits of an
+// offset are ignored, so a malformed table never makes a unit load or store a misaligned element.
+template <uint32_t ELEM = 1u>
+__device__ __forceinline__ unsigned long long ragged_at(const unsigned long long* off, unsigned long long u) {
+    return __ldg(off + u) & ~(unsigned long long)(ELEM - 1u);
+}
+// length of unit u in bytes, clamped to [0, bound]; a decreasing pair counts as 0, so a malformed table never makes a unit read
+// past off[u] + bound.  The pre-pass and the kernels both take it from here, so the sort key and a unit's length agree.
+template <uint32_t ELEM = 1u>
 __device__ __forceinline__ uint32_t ragged_len(const unsigned long long* off, unsigned long long u, uint32_t bound) {
-    const unsigned long long o0 = __ldg(off + u), o1 = __ldg(off + u + 1);
+    const unsigned long long o0 = ragged_at<ELEM>(off, u), o1 = ragged_at<ELEM>(off, u + 1);
     return o1 > o0 ? (o1 - o0 < bound ? (uint32_t)(o1 - o0) : bound) : 0u;
 }
-// sort key: compressions for SHA-256 (the top bucket takes everything longer), bytes for CRC16
-__device__ __forceinline__ uint32_t ragged_cost(uint32_t len, bool sha) {
-    if (!sha) return len;
-    const uint32_t nblk = (len + 8u) / 64u + 1u;
-    return nblk < XMR_RAGGED_BUCKETS - 1u ? nblk : XMR_RAGGED_BUCKETS - 1u;
+// sort key of a unit of len bytes (XMR_RAGGED_COST_*): bytes for CRC16, compressions for SHA-256 and elements for quicksort
+// (the top bucket takes everything longer)
+__device__ __forceinline__ uint32_t ragged_cost(uint32_t len, uint32_t kind) {
+    if (kind == XMR_RAGGED_COST_CRC) return len;
+    const uint32_t c = kind == XMR_RAGGED_COST_SHA ? (len + 8u) / 64u + 1u : len / 4u;
+    return c < XMR_RAGGED_BUCKETS - 1u ? c : XMR_RAGGED_BUCKETS - 1u;
+}
+__device__ __forceinline__ uint32_t ragged_unit_cost(const unsigned long long* off, unsigned long long u, uint32_t bound, uint32_t kind) {
+    return ragged_cost(kind == XMR_RAGGED_COST_QSORT ? ragged_len<4>(off, u, bound) : ragged_len(off, u, bound), kind);
 }
 
 // The next warp-tile of this warp (uniform), from the counter in the scratch header.
@@ -244,17 +257,71 @@ __device__ __forceinline__ void crc16_var_body(const xmr_args& a) {
     tally.flush(a.counters);
 }
 
+// Quicksort of a ragged batch: the state machine of xmr_qsort.cuh (qsort_step, qsort_exit) over cost-ordered warp-tiles.
+// Unit u sorts the int32 elements d_in[off[u] .. off[u+1]) (offsets rounded down to a multiple of 4) into the same bytes of
+// d_out.  Each lane group keeps its NC x L copies in a slot of NC x bound elements (scratch from xmr_ragged_slots); a zero-length
+// unit executes its one `if (len < 2) return;` and stores nothing.
+template <int NC, bool INJECT>
+__device__ __forceinline__ void qsort_var_body(const xmr_args& a) {
+    constexpr int UPW = Lanes<NC>::kUnitsPerWarp;
+    const int lane = threadIdx.x & 31;
+    const bool spare = NC == 3 && lane >= 30;                   // the two idle TMR lanes only take part in the ballots
+    const int u = spare ? 0 : lane / NC, r = spare ? 0 : lane % NC, base = u * NC;
+    const uint32_t gmask = spare ? 0u : (((1u << NC) - 1u) << base);
+    const unsigned long long gwarp = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    RaggedHdr* hdr = reinterpret_cast<RaggedHdr*>(const_cast<void*>(a.aux));
+    const unsigned long long* off = hdr->off;
+    const uint32_t* perm = reinterpret_cast<const uint32_t*>(static_cast<const uint8_t*>(a.aux) + XMR_RAGGED_PERM);
+    const unsigned long long n_wtiles = (a.n_units + UPW - 1) / UPW;
+    const uint32_t Lb = a.unit_bytes >> 2;                      // the bound in elements
+    const bool majority = (a.flags & COAST_F_MAJORITY_VOTER) != 0;
+    Tally tally(a);
+    int32_t* const Au = reinterpret_cast<int32_t*>(static_cast<uint8_t*>(const_cast<void*>(a.aux)) + xmr_ragged_slots(a.n_units)) +
+                        (gwarp * 32ull + (unsigned)base) * Lb;  // this lane group's NC x Lb slot
+    auto at = [&](uint32_t e) -> int32_t& { return Au[e * NC + (uint32_t)r]; };                  // element e of this replica
+    uint32_t stack[QS_MAX];                                     // (off << 16) | len, len <= 1024 needs 11 bits
+    for (uint32_t wt = ragged_pull(hdr, lane); wt < n_wtiles; wt = ragged_pull(hdr, lane)) {
+        const unsigned long long pos = (unsigned long long)wt * UPW + u;
+        const bool valid = !spare && pos < a.n_units;
+        const unsigned long long local = valid ? __ldg(perm + pos) : 0ull;
+        const uint32_t L = valid ? ragged_len<4>(off, local, a.unit_bytes) / 4u : 0u;
+        const unsigned long long o = valid ? ragged_at<4>(off, local) : 0ull;
+        uint32_t fsite = 0xFFFFFFFFu, fmask = 0u;
+        if (valid) {
+            const int32_t* src = reinterpret_cast<const int32_t*>(static_cast<const uint8_t*>(a.in) + o);
+            for (uint32_t e = 0; e < L; ++e) at(e) = __ldg(src + e);
+            if (INJECT) {
+                Fault f = fault_for_unit(a, NC, local, 33u * L, [](uint32_t) { return 32u; });
+                if (f.active) {
+                    if (r == 0) tally.injected++;
+                    if ((int)f.replica == r) { fsite = f.site; fmask = 1u << f.bit; }
+                }
+                if (fsite >= 32u * L && fsite != 0xFFFFFFFFu) at(fsite - 32u * L) ^= (int32_t)fmask;
+            }
+        }
+        QsState s;
+        s.phase = valid ? QS_POP : QS_DONE;
+        if (valid) stack[s.sp++] = L;                           // quick_sort(A, n): off = 0
+        __syncwarp();
+        while (__any_sync(0xFFFFFFFFu, s.phase != QS_DONE)) qsort_step<NC, INJECT>(s, at, stack, base, majority, fsite, fmask);
+        if (valid)
+            qsort_exit<NC>(a, tally, s, at, L, reinterpret_cast<int32_t*>(static_cast<uint8_t*>(a.out) + o), local, gmask, base, r, majority);
+        __syncwarp();
+    }
+    tally.flush(a.counters);
+}
+
 }  // namespace xmr
 
-// ---- the cost-ordering pre-pass (scratch layout in xmr_geom.h) ----
+// ---- the cost-ordering pre-pass (scratch layout in xmr_geom.h); `kind` is an XMR_RAGGED_COST_* ----
 extern "C" __global__ void __launch_bounds__(XMR_CTA_THREADS)
-xmr_ragged_hist(const unsigned long long* off, unsigned long long n, unsigned int bound, unsigned int sha, unsigned char* scratch) {
+xmr_ragged_hist(const unsigned long long* off, unsigned long long n, unsigned int bound, unsigned int kind, unsigned char* scratch) {
     __shared__ unsigned int h[XMR_RAGGED_BUCKETS];
     for (unsigned i = threadIdx.x; i < XMR_RAGGED_BUCKETS; i += blockDim.x) h[i] = 0u;
     __syncthreads();
     const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
     for (unsigned long long u = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; u < n; u += stride)
-        atomicAdd(&h[xmr::ragged_cost(xmr::ragged_len(off, u, bound), sha != 0u)], 1u);
+        atomicAdd(&h[xmr::ragged_unit_cost(off, u, bound, kind)], 1u);
     __syncthreads();
     unsigned int* cnt = reinterpret_cast<unsigned int*>(scratch + XMR_RAGGED_HDR);
     for (unsigned i = threadIdx.x; i < XMR_RAGGED_BUCKETS; i += blockDim.x)
@@ -291,7 +358,7 @@ xmr_ragged_scan(const unsigned long long* off, unsigned char* scratch) {
 
 // units -> permutation slots; one atomic per bucket present in a warp (lanes with equal cost share it)
 extern "C" __global__ void __launch_bounds__(XMR_CTA_THREADS)
-xmr_ragged_scatter(const unsigned long long* off, unsigned long long n, unsigned int bound, unsigned int sha, unsigned char* scratch) {
+xmr_ragged_scatter(const unsigned long long* off, unsigned long long n, unsigned int bound, unsigned int kind, unsigned char* scratch) {
     unsigned int* next = reinterpret_cast<unsigned int*>(scratch + XMR_RAGGED_HDR);
     unsigned int* perm = reinterpret_cast<unsigned int*>(scratch + XMR_RAGGED_PERM);
     const int lane = threadIdx.x & 31;
@@ -301,7 +368,7 @@ xmr_ragged_scatter(const unsigned long long* off, unsigned long long n, unsigned
         const bool act = u < n;
         const unsigned int live = __ballot_sync(0xFFFFFFFFu, act);
         if (act) {
-            const unsigned int b = xmr::ragged_cost(xmr::ragged_len(off, u, bound), sha != 0u);
+            const unsigned int b = xmr::ragged_unit_cost(off, u, bound, kind);
             const unsigned int peers = __match_any_sync(live, b);
             const int leader = __ffs(peers) - 1;
             unsigned int slot = 0u;
@@ -322,7 +389,14 @@ xmr_ragged_scatter(const unsigned long long* off, unsigned long long n, unsigned
     xmr_crc16_var_inj##INJ##_nc##NC(const __grid_constant__ xmr_args a) {                                \
         xmr::crc16_var_body<NC, INJ != 0>(a);                                                            \
     }
+#define XMR_QSORT_VAR_KERNEL(NC, INJ)                                                                    \
+    extern "C" __global__ void __launch_bounds__(XMR_QSORT_THREADS)                                      \
+    xmr_qsort_var_inj##INJ##_nc##NC(const __grid_constant__ xmr_args a) {                                \
+        xmr::qsort_var_body<NC, INJ != 0>(a);                                                            \
+    }
 XMR_SHA_VAR_KERNEL(1, 0) XMR_SHA_VAR_KERNEL(2, 0) XMR_SHA_VAR_KERNEL(3, 0)
 XMR_SHA_VAR_KERNEL(1, 1) XMR_SHA_VAR_KERNEL(2, 1) XMR_SHA_VAR_KERNEL(3, 1)
 XMR_CRC_VAR_KERNEL(1, 0) XMR_CRC_VAR_KERNEL(2, 0) XMR_CRC_VAR_KERNEL(3, 0)
 XMR_CRC_VAR_KERNEL(1, 1) XMR_CRC_VAR_KERNEL(2, 1) XMR_CRC_VAR_KERNEL(3, 1)
+XMR_QSORT_VAR_KERNEL(1, 0) XMR_QSORT_VAR_KERNEL(2, 0) XMR_QSORT_VAR_KERNEL(3, 0)
+XMR_QSORT_VAR_KERNEL(1, 1) XMR_QSORT_VAR_KERNEL(2, 1) XMR_QSORT_VAR_KERNEL(3, 1)

@@ -18,7 +18,7 @@ F_INTERLEAVE, F_SEGMENT, F_VERBOSE, F_MAJORITY_VOTER = 0x8, 0x10, 0x20, 0x100
 F_STORE_DATA_SYNC, F_NO_STORE_DATA_SYNC, F_NO_LOAD_SYNC, F_NO_STORE_ADDR_SYNC = 0x200, 0x400, 0x800, 0x1000
 PLAN_NONE, PLAN_BERNOULLI, PLAN_TABLE = 0, 1, 2
 AES_DECRYPT, AES_KEY_PER_UNIT, AES_KEY_WRITEBACK = 1, 2, 4
-UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 batches: aux = n_units + 1 u64 byte offsets into inp
+UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 / QSORT batches: aux = n_units + 1 u64 byte offsets into inp
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 
@@ -269,8 +269,11 @@ class Runtime:
     def run(self, kernel, num_clones, inp, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0, aux=None,
             key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, out=None, stream=None, status=None):
         torch = self.torch
+        ragged_qsort = bool(mode & UNIT_OFFSETS) and kernel == K_QSORT
+        if out is None and ragged_qsort:       # the arrays are sorted into the bytes they came from: out mirrors inp
+            out = torch.zeros(inp.numel() * inp.element_size(), dtype=torch.uint8, device=f"cuda:{self.device}")
         if mode & UNIT_OFFSETS:
-            self._check_offsets(inp, aux, n_units, unit_bytes)
+            self._check_offsets(inp, aux, n_units, unit_bytes, kernel=kernel, out=out)
         if out is None:
             out = torch.empty(n_units * out_bytes(kernel, unit_bytes), dtype=torch.uint8, device=f"cuda:{self.device}")
         d = self.make_desc(kernel, num_clones, inp, out, n_units, flags=flags, mode=mode, unit_bytes=unit_bytes,
@@ -278,9 +281,11 @@ class Runtime:
         self.launch(d, stream)
         return out, self.sync(stream)
 
-    def _check_offsets(self, inp, aux, n_units, unit_bytes):
+    def _check_offsets(self, inp, aux, n_units, unit_bytes, *, kernel=None, out=None):
         """A ragged batch's device offsets (int64 or uint64 tensor, n_units + 1 entries): they never decrease, no length
-        exceeds unit_bytes and the last one lies within inp.  The kernels only clamp; this catches a bad table before it runs."""
+        exceeds unit_bytes and the last one lies within inp.  The kernels only clamp; this catches a bad table before it runs.
+        QSORT (int32 arrays sorted into the same bytes of out): every offset is a multiple of 4, inp and out are 4-byte
+        aligned and the last offset lies within out too."""
         torch = self.torch
         if aux is None or not hasattr(aux, "data_ptr") or aux.dtype not in (torch.int64, torch.uint64) or not aux.is_cuda:
             raise CoastError(ERR_BAD_ARG, "UNIT_OFFSETS: aux must be a CUDA int64/uint64 tensor of n_units + 1 byte offsets")
@@ -293,6 +298,13 @@ class Runtime:
         if any(bad):
             raise CoastError(ERR_BAD_ARG, "UNIT_OFFSETS: offsets must not decrease, no length may exceed unit_bytes "
                                           f"({unit_bytes}) and the last offset must lie within inp ({nbytes} bytes)")
+        if kernel == K_QSORT:
+            if inp.data_ptr() % 4 or (out is not None and out.data_ptr() % 4):
+                raise CoastError(ERR_BAD_ARG, "UNIT_OFFSETS: QSORT's inp and out must be 4-byte aligned")
+            obytes = out.numel() * out.element_size() if out is not None else nbytes
+            if bool(((off & 3) != 0).any()) or int(off[-1]) > obytes:
+                raise CoastError(ERR_BAD_ARG, "UNIT_OFFSETS: QSORT offsets must be multiples of 4 (whole int32 elements) and the "
+                                              f"last one must lie within out ({obytes} bytes)")
 
     # -- the reference-facing host call: HOST buffers, H2D + kernel + D2H inside ---------------
     def run_host(self, kernel, num_clones, h_in, h_out, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0,

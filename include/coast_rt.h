@@ -166,16 +166,26 @@ typedef struct coast_fault_plan {
  *            out: n_units x 16 int32;  aux: n_units x 16 int32 keys with COAST_AES_KEY_PER_UNIT, else `key` below;
  *            mode bit0 = decrypt.  The key is never modified (KeySchedule expands into word[][], aes_key.c:129-163).
  *   CRC16 / SHA256 with COAST_UNIT_OFFSETS: in = the messages end to end, aux = n_units + 1 u64 byte offsets (see below).
+ *   QSORT with COAST_UNIT_OFFSETS: in = int32 arrays end to end, aux = n_units + 1 u64 byte offsets (multiples of 4);
+ *            out: each array sorted into the same byte range of d_out, d_out[off[u] .. off[u+1]); nothing else is written.
  */
-/* Ragged batches (CRC16 and SHA256 only): with COAST_UNIT_OFFSETS in `mode`, the n_units messages lie end to end in d_in
+/* Ragged batches (CRC16, SHA256 and QSORT only): with COAST_UNIT_OFFSETS in `mode`, the n_units units lie end to end in d_in
  * and d_aux points to n_units + 1 uint64_t byte offsets (8-byte aligned); unit u is d_in[off[u] .. off[u+1]).  unit_bytes is
  * then the caller's bound on every length: at most 255 for CRC16 (crc16.c:21 takes an unsigned char), at most 2^28 for
- * SHA256; n_units must be below 2^32.  The launch equals n_units single-unit launches, unit u with unit_bytes = its length,
- * d_in + off[u] and unit_base + u: the same outputs, d_status bytes, summed counters and minimum first_fault_unit.  Fault
- * sites count per unit (a zero-length CRC16 unit has none: never injected, output 0xFFFF, one exit vote).  The kernel clamps
- * each length to [0, unit_bytes] (a decreasing pair counts as 0); coast_run_host rejects such tables.  A shard passes
- * off + lo with the same d_in and unit_base = lo.  The units are ordered by cost in a pre-pass so that long messages do not
- * leave the replica lanes of short ones idle.  Any other kernel fails with COAST_ERR_BAD_ARG. */
+ * SHA256, a multiple of 4 in 4..4096 for QSORT; n_units must be below 2^32.  The launch equals n_units single-unit launches,
+ * unit u with unit_bytes = its length, d_in + off[u] and unit_base + u: the same outputs, d_status bytes, summed counters
+ * and minimum first_fault_unit.  Fault sites count per unit (a zero-length CRC16 unit has none: never injected, output
+ * 0xFFFF, one exit vote).  The kernel clamps each length to [0, unit_bytes] (a decreasing pair counts as 0); coast_run_host
+ * rejects such tables.  A shard passes off + lo with the same d_in and unit_base = lo.  The units are ordered by cost in a
+ * pre-pass so that long units do not leave the replica lanes of short ones idle.  Any other kernel fails with
+ * COAST_ERR_BAD_ARG.
+ * QSORT: the units are int32 arrays; d_in and d_out are 4-byte aligned and every offset is a multiple of 4 (the kernel rounds
+ * an offset down to one; coast_run_host rejects it).  Array u is sorted into d_out + off[u], the bytes it came from; bytes of
+ * d_out outside [off[0], off[n_units]) are never written.  Fault sites are 33 L_u per array (width 32).  A zero-length array
+ * (which the uniform launch refuses) has no sites, writes nothing, has d_status 0 and executes one sync point, the
+ * `if (len < 2) return;` of quicksort.c:122.  A shard passes off + lo with the same d_in, the SAME d_out (unlike CRC16 and
+ * SHA256, whose d_out is indexed by the shard's own units) and unit_base = lo.  COAST_QSORT_PATH=nested gives
+ * COAST_ERR_UNSUPPORTED: a ragged batch runs the state-machine scheduling only. */
 #define COAST_UNIT_OFFSETS      0x10000u
 #define COAST_AES_DECRYPT       0x1u
 #define COAST_AES_KEY_PER_UNIT  0x2u
@@ -312,8 +322,9 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  *     chunk, chunks of 1..16 MiB round-robin over three internal streams and staging slots
  *     (a unit larger than 16 MiB is a chunk of its own).  d_status is staged per chunk too.
  * COAST_HOST_PATH=staged|zerocopy forces a path.  Ragged calls (COAST_UNIT_OFFSETS, d_aux = host offsets, which must never
- * decrease nor give a length above unit_bytes) are always staged: chunks are contiguous unit ranges, each uploads its bytes and
- * its slice of the offsets unchanged; a forced zerocopy or hybrid path gives COAST_ERR_UNSUPPORTED.  On any failure every copy already queued on
+ * decrease nor give a length above unit_bytes, and for QSORT must be multiples of 4) are always staged: chunks are contiguous
+ * unit ranges, each uploads its bytes and its slice of the offsets unchanged (QSORT also downloads the same byte range to
+ * d_out + off[first]); a forced zerocopy or hybrid path gives COAST_ERR_UNSUPPORTED.  On any failure every copy already queued on
  * the caller's buffers is drained before the call returns. */
 int  coast_run_host(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
 const char* coast_last_host_path(void);   /* "zerocopy", "staged" or "one-shot" (matmuls): what the last host call did */
