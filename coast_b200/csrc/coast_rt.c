@@ -537,18 +537,41 @@ static void plan_wg_map(map_desc* m, CUtensorMapDataType dtype, unsigned esize, 
 
 /* Pre-passes of the wgmma kernels: TF32 wgmma reads both operands K-major, so B (K x N, row-major) is transposed into scratch;
  * the limb kernel splits A and B into u8 limb planes ([plane][M][K] and, transposed, [plane][N][K]). */
+/* Batched matmuls (COAST_MM_BATCHED): the products in the launch (1 without the bit), and the checks shared by coast_launch
+ * and coast_run_host.  The stacked A and C are one (batch*M)-row matrix; only B changes from one product to the next. */
+static uint64_t mm_batch(const coast_launch_desc* d) {
+    return (d->mode & COAST_MM_BATCHED) ? d->n_units / ((uint64_t)d->M * d->N) : 1u;
+}
+static int batched_check(const coast_launch_desc* d) {
+    if (d->kernel != COAST_K_MM_U32 && d->kernel != COAST_K_GEMM_TF32)
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batched products exist for MM_U32 and GEMM_TF32 only (kernel %u)", d->kernel);
+    if (!d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: M, N and K are the shape of one product and must be nonzero");
+    const uint64_t mn = (uint64_t)d->M * d->N;
+    if (!d->n_units || d->n_units % mn)
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: n_units must be a nonzero multiple of M*N = %llu (got %llu)",
+                    (unsigned long long)mn, (unsigned long long)d->n_units);
+    const uint64_t batch = d->n_units / mn;
+    if (batch * d->M >= (1ull << 31) || batch * d->N >= (1ull << 31))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batch*M and batch*N must be below 2^31 (batch %llu, M %u, N %u)",
+                    (unsigned long long)batch, d->M, d->N);
+    return COAST_OK;
+}
+
+/* Pre-passes of the wgmma kernels: TF32 wgmma reads both operands K-major, so B (K x N, row-major) is transposed into scratch;
+ * the limb kernel splits A and B into u8 limb planes ([plane][M][K] and, transposed, [plane][N][K]).  A batch's B matrices
+ * become one stacked (batch*N) x K operand, its A matrices are already one (batch*M) x K matrix. */
 static int prepass_transpose_b(const coast_launch_desc* d, CUdeviceptr bt, CUstream s) {
-    const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N;
-    void* params[] = { &B, &bt, &k32, &n32 };
+    const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N, nb = (unsigned)mm_batch(d);
+    void* params[] = { &B, &bt, &k32, &n32, &nb };
     return launch_small("xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
 }
 static int prepass_split_limbs(const coast_launch_desc* d, CUdeviceptr pa, CUstream s) {
-    unsigned long long rows = d->M, K = d->K; const void* A = d->d_in;
+    unsigned long long rows = mm_batch(d) * d->M, K = d->K; const void* A = d->d_in;
     void* params_a[] = { &A, &pa, &rows, &K };
     int rc = launch_small("xmr_mm_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_a, s); if (rc) return rc;
-    CUdeviceptr pb = pa + (size_t)d->M * d->K * 4u;
-    unsigned int k32 = d->K, n32 = d->N; const void* B = d->d_aux;
-    void* params_b[] = { &B, &pb, &k32, &n32 };
+    CUdeviceptr pb = pa + (size_t)rows * d->K * 4u;
+    unsigned int k32 = d->K, n32 = d->N, nb = (unsigned)mm_batch(d); const void* B = d->d_aux;
+    void* params_b[] = { &B, &pb, &k32, &n32, &nb };
     return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
 }
 
@@ -627,6 +650,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     if (d->num_clones < 1 || d->num_clones > 3) return fail(COAST_ERR_BAD_ARG, "num_clones must be 1, 2 (DWC) or 3 (TMR)");
     const int ragged = (d->mode & COAST_UNIT_OFFSETS) != 0;
     if (ragged && (rc = ragged_check(d))) return rc;
+    const int batched = (d->mode & COAST_MM_BATCHED) != 0;
+    if (batched && (rc = batched_check(d))) return rc;
     if (d->n_units == 0) return COAST_OK;
     if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null device buffer");
     const uint32_t nc = d->num_clones;
@@ -638,7 +663,9 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     a.n_units = d->n_units; a.unit_base = d->unit_base;
     a.counters = (unsigned long long*)(G.peer_counters ? G.peer_counters : G.counters);
     a.status = (unsigned char*)d->d_status;
-    a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode;
+    /* the kernels find a batch from n_units / N (rows of the stacked problem) and a.M (rows per product): a batch of one is
+     * an unbatched launch, argument block included */
+    a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~COAST_MM_BATCHED;
     a.M = d->M; a.N = d->N; a.K = d->K;
     memcpy(a.key, d->key, 16);
     if (inj) {
@@ -722,27 +749,29 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     }
     case COAST_K_MM_U32: {
         if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "MM needs A (d_in), B (d_aux) and M,N,K");
-        if (d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "MM: n_units must be M*N");
+        if (!batched && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "MM: n_units must be M*N");
         /* the plain kernel (one lane per replica per element) takes any shape and the per-k votes on `sum`; tile-aligned problems
-         * go to the tensor cores (exact, u8 limbs on wgmma) or the register-tiled kernel; COAST_MM_PATH=tc|tiled|naive overrides */
+         * go to the tensor cores (exact, u8 limbs on wgmma) or the register-tiled kernel; COAST_MM_PATH=tc|tiled|naive overrides.
+         * The shape rules are those of one product; a batch stacks the products' rows (no tile straddles two of them). */
         snprintf(L.name, sizeof L.name, "xmr_mm_u32_nc%u_inj%d", nc, inj);
         const char* path = getenv("COAST_MM_PATH");
         const int aligned = aligned16 && !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u);
+        const uint64_t batch = mm_batch(d), rows = batch * d->M;
         if (store_votes || !aligned) break;
         if ((!path || !strcmp(path, "tc")) && d->M % XMR_WG_BM == 0 && d->N % xmr_mmtc_bn(1) == 0 && d->K % XMR_MMTC_BK == 0) {
             const unsigned bn = xmr_mmtc_bn(nc);
             snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_nc%u_inj%d", nc, inj);
             L.block = XMR_WG_THREADS; L.smem = xmr_mmtc_smem(nc);
-            L.ctas = (d->M / XMR_WG_BM) * (d->N / bn); L.waves = 1;
-            L.scratch = ((size_t)d->M * d->K + (size_t)d->K * d->N) * 4u;          /* 4 planes of 1 byte per element */
+            L.ctas = (rows / XMR_WG_BM) * (d->N / bn); L.waves = 1;
+            L.scratch = ((size_t)rows * d->K + (size_t)batch * d->K * d->N) * 4u;     /* 4 planes of 1 byte per element */
             L.prepass = prepass_split_limbs;
             L.n_maps = 2;
-            plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, d->M, 4, XMR_WG_BM);
-            plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)d->M * d->K * 4u, 1, d->K, d->N, 4, bn);
+            plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, (uint32_t)rows, 4, XMR_WG_BM);
+            plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)rows * d->K * 4u, 1, d->K, (uint32_t)(batch * d->N), 4, bn);
         } else if (!(path && !strcmp(path, "naive")) && d->M % XMR_MMT_BM == 0 && d->N % XMR_MMT_BN == 0 && d->K % XMR_MMT_BK == 0) {
             snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_nc%u_inj%d", nc, inj);
             L.block = xmr_mmt_threads(nc); L.smem = XMR_MMT_SMEM;
-            L.ctas = (d->M / XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;
+            L.ctas = (rows / XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;
         }
         break;
     }
@@ -782,13 +811,14 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     }
     case COAST_K_GEMM_TF32: {
         if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "GEMM needs A (d_in), B (d_aux) and M,N,K");
-        if (d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "GEMM: n_units must be M*N");
+        if (!batched && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "GEMM: n_units must be M*N");
         if (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % XMR_GEMM_BK)
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_TF32 tiles are 128x128x32: M,N must be multiples of 128 and K of 32 (got %u,%u,%u)", d->M, d->N, d->K);
         if (!aligned16 || (((uintptr_t)d->d_aux) & 15u) || (((uintptr_t)d->d_out) & 15u)) return fail(COAST_ERR_BAD_ARG, "GEMM buffers must be 16-byte aligned");
         /* xmr_gemm_tf32.cuh: unprotected 128 x 256 tiles when N allows (wide), else 128 x 128.  CTA-pair kernels (cluster 2 x 1 x 1,
          * 256-row pair tiles, B multicast) are bit-identical to the single-CTA kernels.  Default: pairs for the unprotected and
-         * DWC kernels when the shape allows, the single-CTA kernel for TMR; COAST_GEMM_PAIR=0 / 1 forces one or the other. */
+         * DWC kernels when the shape allows, the single-CTA kernel for TMR; COAST_GEMM_PAIR=0 / 1 forces one or the other.
+         * A batch stacks its products' rows: a pair tile needs the rows of ONE product, so M (per product) % 256 == 0. */
         const int wide = nc == 1 && d->N % xmr_gemm_bn(1) == 0;
         const char* e = getenv("COAST_GEMM_PAIR");
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
@@ -804,12 +834,13 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         { const char* h = getenv("COAST_GEMM_TAIL_SPLIT"); if (h && !strcmp(h, "0")) a.mode |= XMR_MODE_NO_TAIL_SPLIT; }
         /* persistent CTAs, one per SM (their shared memory allows no second); pairs: an even grid */
         L.block = XMR_WG_THREADS; L.smem = xmr_gemm_smem(wide);
-        L.ctas = (d->M / XMR_WG_BM) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = pair ? 2 : 1;
-        L.scratch = (size_t)d->K * d->N * 4u;                                   /* B^T */
+        const uint64_t batch = mm_batch(d), rows = batch * d->M;
+        L.ctas = (rows / XMR_WG_BM) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = pair ? 2 : 1;
+        L.scratch = (size_t)batch * d->K * d->N * 4u;                          /* B^T of every product */
         L.prepass = prepass_transpose_b;
         L.n_maps = 2;
-        plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uintptr_t)d->d_in, 0, d->K, d->M, 1, XMR_WG_BM);
-        plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, d->N, 1, xmr_gemm_b_box(pair));
+        plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uintptr_t)d->d_in, 0, d->K, (uint32_t)rows, 1, XMR_WG_BM);
+        plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, (uint32_t)(batch * d->N), 1, xmr_gemm_b_box(pair));
         break;
     }
     default:
@@ -1169,6 +1200,45 @@ fail:
     return drain_host_streams(rc);
 }
 
+/* Batched matmul host call (COAST_MM_BATCHED): chunks of whole products, as many as fit the chunk bytes (COAST_HOST_CHUNK_BYTES,
+ * 16 MiB by default, counting A, B and C; a product larger than that is a chunk of its own), round-robin over the three host
+ * streams and staging slots.  A chunk uploads its A and B matrices, launches with unit_base + first * M * N and downloads its
+ * C matrices, so uploads, kernels and downloads of neighbouring chunks overlap. */
+static int run_host_mm_batched(const coast_launch_desc* d, coast_stats* out, int* dwc_fired) {
+    int rc;
+    if (!d->d_in || !d->d_out || !d->d_aux) return fail(COAST_ERR_BAD_ARG, "null host buffer");
+    const uint64_t mn = (uint64_t)d->M * d->N, batch = d->n_units / mn;
+    const uint64_t ab = (uint64_t)d->M * d->K * 4u, bb = (uint64_t)d->K * d->N * 4u, cb = mn * 4u;
+    uint64_t max_chunk_bytes = 16ull << 20;
+    { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) max_chunk_bytes = (uint64_t)atoll(e); }
+    uint64_t per = max_chunk_bytes / (ab + bb + cb);
+    if (per < 1) per = 1;
+    if (per > batch) per = batch;
+    for (int s = 0; s < 3 && (uint64_t)s * per < batch; ++s) {
+        if ((rc = slot_reserve(&G.h_in[s], &G.h_in_cap[s], (size_t)(per * ab)))) return rc;
+        if ((rc = slot_reserve(&G.h_aux[s], &G.h_aux_cap[s], (size_t)(per * bb)))) return rc;
+        if ((rc = slot_reserve(&G.h_out[s], &G.h_out_cap[s], (size_t)(per * cb)))) return rc;
+    }
+    int slot = 0;
+#define STEP(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) { rc = drv_fail(r_, #call); goto fail; } } while (0)
+    for (uint64_t first = 0; first < batch; first += per, slot = (slot + 1) % 3) {
+        const uint64_t cnt = batch - first < per ? batch - first : per;
+        STEP(p_cuMemcpyHtoDAsync_v2(G.h_in[slot], (const uint8_t*)d->d_in + first * ab, (size_t)(cnt * ab), G.hs[slot]));
+        STEP(p_cuMemcpyHtoDAsync_v2(G.h_aux[slot], (const uint8_t*)d->d_aux + first * bb, (size_t)(cnt * bb), G.hs[slot]));
+        coast_launch_desc c = *d;
+        c.d_in = (void*)G.h_in[slot]; c.d_aux = (void*)G.h_aux[slot]; c.d_out = (void*)G.h_out[slot];
+        c.n_units = cnt * mn; c.unit_base = d->unit_base + first * mn;
+        rc = launch_impl(&c, G.hs[slot]); if (rc) goto fail;
+        STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + first * cb, G.h_out[slot], (size_t)(cnt * cb), G.hs[slot]));
+    }
+#undef STEP
+    G.last_host_path = "staged";
+    DRV(p_cuStreamSynchronize(G.hs[0])); DRV(p_cuStreamSynchronize(G.hs[1]));
+    return sync_impl(G.hs[2], out, dwc_fired);
+fail:
+    return drain_host_streams(rc);
+}
+
 /* `d_in` / `d_out` / `d_aux` / `d_status` of the descriptor are HOST pointers here. */
 static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_fired) {
     int rc = ensure_ctx(); if (rc) return rc;
@@ -1176,10 +1246,11 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
     if (d->plan && d->plan->mode == COAST_PLAN_TABLE) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: TABLE plans need device pointers; use coast_launch");
     for (int i = 0; i < 3; ++i) if (!G.hs[i]) DRV(p_cuStreamCreate(&G.hs[i], CU_STREAM_NON_BLOCKING));
     if (d->mode & COAST_UNIT_OFFSETS) return run_host_ragged(d, out, dwc_fired);
+    if ((d->mode & COAST_MM_BATCHED) && (rc = batched_check(d))) return rc;
     const uint64_t ob = coast_out_bytes(d->kernel, d->unit_bytes);
     if (d->kernel == COAST_K_MM_U32 || d->kernel == COAST_K_GEMM_TF32) {
         if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");
-        return run_host_matmul(d, out, dwc_fired);
+        return (d->mode & COAST_MM_BATCHED) ? run_host_mm_batched(d, out, dwc_fired) : run_host_matmul(d, out, dwc_fired);
     }
     const uint64_t ib = in_bytes_per_unit(d);
     /* a zero-length SHA-256 message (sha256_hash(len = 0) hashes one padded block) has nothing to stage */

@@ -218,7 +218,8 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
     const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
     const uint32_t worker = blockIdx.x / CTAS, n_workers = gridDim.x / CTAS;
     const uint32_t TM = BM * CTAS;                              // rows of a (pair) tile
-    const uint32_t tiles_n = a.N / BN, tiles_m = a.M / TM, n_tiles = tiles_m * tiles_n, kblocks = a.K / BK;
+    // a batch stacks its products' rows (n_units / N of them, a.M per product); the host keeps every tile inside one product
+    const uint32_t tiles_n = a.N / BN, tiles_m = (uint32_t)(a.n_units / a.N) / TM, n_tiles = tiles_m * tiles_n, kblocks = a.K / BK;
     const uint32_t gm1 = (a.mode & XMR_MODE_GROUP_M_MASK) ? (a.mode & XMR_MODE_GROUP_M_MASK) : GROUP_M_DEFAULT;
     const uint32_t group_m = PAIR ? (gm1 > 1u ? gm1 / 2u : 1u) : gm1;   // pair tiles are 256 rows: half as many tile-rows per group
     const bool hints = (a.mode & XMR_MODE_L2_HINTS) != 0;
@@ -257,6 +258,7 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
                 uint32_t tm, n_off, bn_t;
                 decode(tile, tm, n_off, bn_t);
                 const int m0 = (int)(tm * TM + rank * BM);
+                const uint32_t nb = (tm * TM) / a.M * a.N;          // first B^T row of the tile's product (stacked B^T)
                 const uint32_t rows_b = bn_t / CTAS;                // B^T rows this CTA loads (for both CTAs of a pair)
                 for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
                     const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
@@ -265,8 +267,8 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
                     tma_load_2d_hint(sA + s * A_STAGE, map_a, &full[s], (int)(kb * BK), m0, pol_a);          // box {32 k, 128 m}
                     for (uint32_t c = 0; c < rows_b / B_BOX; ++c) {
                         const uint32_t r = rank * rows_b + c * B_BOX;                                        // row of the tile's B^T
-                        if (PAIR) tma_load_2d_mcast(sB + s * B_STAGE + r * 128u, map_b, &full[s], (int)(kb * BK), (int)(n_off + r), (uint16_t)3, pol_b);
-                        else tma_load_2d_hint(sB + s * B_STAGE + r * 128u, map_b, &full[s], (int)(kb * BK), (int)(n_off + r), pol_b);
+                        if (PAIR) tma_load_2d_mcast(sB + s * B_STAGE + r * 128u, map_b, &full[s], (int)(kb * BK), (int)(nb + n_off + r), (uint16_t)3, pol_b);
+                        else tma_load_2d_hint(sB + s * B_STAGE + r * 128u, map_b, &full[s], (int)(kb * BK), (int)(nb + n_off + r), pol_b);
                     }
                 }
             }
@@ -335,16 +337,21 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
 }  // namespace gemm
 }  // namespace xmr
 
-// B (K x N, row-major) -> B^T (N x K): the K-major operand TF32 wgmma reads.  32 x 32 tiles through shared memory.
+// B (batch x K x N, row-major) -> B^T (batch x N x K, one stacked (batch N) x K operand): the K-major operand TF32 wgmma reads.
+// 32 x 32 tiles through shared memory.
 extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
-xmr_gemm_bt(const float* __restrict__ B, float* __restrict__ Bt, unsigned int K, unsigned int N) {
+xmr_gemm_bt(const float* __restrict__ B, float* __restrict__ Bt, unsigned int K, unsigned int N, unsigned int batch) {
     __shared__ float tile[32][33];
     const unsigned int tiles_n = N / 32u, tiles_k = K / 32u;
-    for (unsigned int t = blockIdx.x; t < tiles_n * tiles_k; t += gridDim.x) {
-        const unsigned int k0 = (t / tiles_n) * 32u, n0 = (t % tiles_n) * 32u;
-        for (int i = threadIdx.x; i < 1024; i += 256) tile[i >> 5][i & 31] = __ldg(B + (size_t)(k0 + (i >> 5)) * N + n0 + (i & 31));
+    const unsigned long long per = (unsigned long long)tiles_n * tiles_k, n_tiles = per * batch;
+    for (unsigned long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const unsigned long long b = t / per;
+        const unsigned int w = (unsigned int)(t - b * per), k0 = (w / tiles_n) * 32u, n0 = (w % tiles_n) * 32u;
+        const float* Bb = B + b * K * N;
+        float* Btb = Bt + b * N * K;
+        for (int i = threadIdx.x; i < 1024; i += 256) tile[i >> 5][i & 31] = __ldg(Bb + (size_t)(k0 + (i >> 5)) * N + n0 + (i & 31));
         __syncthreads();
-        for (int i = threadIdx.x; i < 1024; i += 256) Bt[(size_t)(n0 + (i >> 5)) * K + k0 + (i & 31)] = tile[i & 31][i >> 5];
+        for (int i = threadIdx.x; i < 1024; i += 256) Btb[(size_t)(n0 + (i >> 5)) * K + k0 + (i & 31)] = tile[i & 31][i >> 5];
         __syncthreads();
     }
 }

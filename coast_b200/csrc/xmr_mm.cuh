@@ -40,8 +40,8 @@ __device__ __forceinline__ void mm_u32_body(const xmr_args& a) {
                 if ((int)f.replica == r) { fsite = f.site; fmask = 1u << f.bit; }
             }
         }
-        const uint32_t* ap = A + (size_t)i * K;
-        const uint32_t* bp = B + j;
+        const uint32_t* ap = A + (size_t)i * K;                 // i: row of the stacked problem; a batch's product i / M
+        const uint32_t* bp = B + (size_t)(i / a.M) * K * N + j;
         uint32_t sum = 0;
         if (!(a.flags & XMR_F_STORE_VOTES)) {
             for (uint32_t k = 0; k < K; ++k) {                  // :12-14

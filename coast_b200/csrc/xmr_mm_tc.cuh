@@ -49,7 +49,8 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
     uint64_t* full = bars;
     uint64_t* empty = bars + STAGES_;
 
-    const uint32_t tiles_n = a.N / BN, tiles_m = a.M / TBM, n_tiles = tiles_m * tiles_n, kblocks = a.K / TBK;
+    // a batch stacks its products' rows (n_units / N of them, a.M per product; no tile straddles two products)
+    const uint32_t tiles_n = a.N / BN, tiles_m = (uint32_t)(a.n_units / a.N) / TBM, n_tiles = tiles_m * tiles_n, kblocks = a.K / TBK;
     // tile order: GROUP_M tile-rows per group, column-major inside (same L2 argument as the TF32 kernel)
     auto coords = [&](uint32_t tile, uint32_t& tm, uint32_t& tn) { tile_coords(tile, tiles_m, tiles_n, GROUP_M, tm, tn); };
 
@@ -67,12 +68,13 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
             uint32_t it = 0;
             for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
                 uint32_t tm, tn; coords(tile, tm, tn);
+                const uint32_t nb = (tm * TBM) / a.M * a.N;     // first B^T row of the tile's product (stacked B^T planes)
                 for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
                     const uint32_t s = it % STAGES_, ph = (it / STAGES_) & 1u;
                     mbar_wait_or_trap(&empty[s], ph ^ 1u);
                     mbar_arrive_expect_tx(&full[s], G::A_STAGE_B + G::B_STAGE_B);
-                    tma_load_3d(sA + s * G::A_STAGE_B, map_a, &full[s], (int)(kb * TBK), (int)(tm * TBM), 0);   // box {128 k, 128 m, 4 planes}
-                    tma_load_3d(sB + s * G::B_STAGE_B, map_b, &full[s], (int)(kb * TBK), (int)(tn * BN), 0);    // box {128 k, BN n, 4 planes}
+                    tma_load_3d(sA + s * G::A_STAGE_B, map_a, &full[s], (int)(kb * TBK), (int)(tm * TBM), 0);       // box {128 k, 128 m, 4 planes}
+                    tma_load_3d(sB + s * G::B_STAGE_B, map_b, &full[s], (int)(kb * TBK), (int)(nb + tn * BN), 0);  // box {128 k, BN n, 4 planes}
                 }
             }
         }
@@ -148,7 +150,8 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
                             if (f.active) {
                                 tally.injected++;
                                 uint32_t part = 0;          // S_s = partial sum over k <= site, from the original u32 operands
-                                for (uint32_t k = 0; k <= f.site; ++k) part += __ldg(A32 + (size_t)row * a.K + k) * __ldg(B32 + (size_t)k * a.N + col + e);
+                                const uint32_t* Bp = B32 + (size_t)(row / a.M) * a.K * a.N;    // the element's own product's B
+                                for (uint32_t k = 0; k <= f.site; ++k) part += __ldg(A32 + (size_t)row * a.K + k) * __ldg(Bp + (size_t)k * a.N + col + e);
                                 const uint32_t mk = 1u << f.bit, delta = (part & mk) ? (0u - mk) : mk;
                                 if (f.replica == 0) r0 += delta; else if (f.replica == 1) r1 += delta; else r2 += delta;
                             }
@@ -192,20 +195,24 @@ xmr_mm_split_a(const uint32_t* __restrict__ A, uint8_t* __restrict__ planes, uns
         p[3ull * plane + q] = __byte_perm(hi, hi2, 0x7632u);       // plane 3
     }
 }
-// B (u32, K x N, row-major) -> planes[l][n][k] (u8, TRANSPOSED so the MMA's B operand is K-major).  32 x 32 tiles via smem.
+// B (u32, batch x K x N, row-major) -> planes[l][b N + n][k] (u8, TRANSPOSED so the MMA's B operand is K-major; a batch's
+// products stacked along n).  32 x 32 tiles via smem.
 extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
-xmr_mm_split_bt(const uint32_t* __restrict__ B, uint8_t* __restrict__ planes, unsigned int K, unsigned int N) {
+xmr_mm_split_bt(const uint32_t* __restrict__ B, uint8_t* __restrict__ planes, unsigned int K, unsigned int N, unsigned int batch) {
     __shared__ uint32_t tile[32][33];
     const unsigned int tiles_n = N / 32u, tiles_k = K / 32u;
-    for (unsigned int t = blockIdx.x; t < tiles_n * tiles_k; t += gridDim.x) {
-        const unsigned int k0 = (t / tiles_n) * 32u, n0 = (t % tiles_n) * 32u;
-        for (int i = threadIdx.x; i < 1024; i += 256) tile[i >> 5][i & 31] = __ldg(B + (size_t)(k0 + (i >> 5)) * N + n0 + (i & 31));
+    const unsigned long long per = (unsigned long long)tiles_n * tiles_k, n_tiles = per * batch;
+    for (unsigned long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const unsigned long long b = t / per;
+        const unsigned int w = (unsigned int)(t - b * per), k0 = (w / tiles_n) * 32u, n0 = (w % tiles_n) * 32u;
+        const uint32_t* Bb = B + b * K * N;
+        for (int i = threadIdx.x; i < 1024; i += 256) tile[i >> 5][i & 31] = __ldg(Bb + (size_t)(k0 + (i >> 5)) * N + n0 + (i & 31));
         __syncthreads();
         const int n = threadIdx.x >> 3, kq = threadIdx.x & 7;      // 32 n x 8 k-quads
         const uint32_t w0 = tile[kq * 4][n], w1 = tile[kq * 4 + 1][n], w2 = tile[kq * 4 + 2][n], w3 = tile[kq * 4 + 3][n];
         const uint32_t lo = __byte_perm(w0, w1, 0x5140u), hi = __byte_perm(w0, w1, 0x7362u);
         const uint32_t lo2 = __byte_perm(w2, w3, 0x5140u), hi2 = __byte_perm(w2, w3, 0x7362u);
-        const size_t plane = (size_t)N * K, off = (size_t)(n0 + n) * K + k0 + kq * 4;
+        const size_t plane = (size_t)batch * N * K, off = (size_t)(b * N + n0 + n) * K + k0 + kq * 4;
         *reinterpret_cast<uint32_t*>(planes + off) = __byte_perm(lo, lo2, 0x5410u);
         *reinterpret_cast<uint32_t*>(planes + plane + off) = __byte_perm(lo, lo2, 0x7632u);
         *reinterpret_cast<uint32_t*>(planes + 2 * plane + off) = __byte_perm(hi, hi2, 0x5410u);

@@ -39,9 +39,9 @@ __device__ __forceinline__ void body(const xmr_args& a) {
     const int tx = vt & 15, ty = vt >> 4;        // micro-tile: rows {ty*4+i, 32+ty*4+i}, cols {tx*4+j, 64+tx*4+j}
     const uint32_t M = a.M, N = a.N, K = a.K;
     const uint32_t tiles_n = N / BN;
-    const uint32_t m0 = (blockIdx.x / tiles_n) * BM, n0 = (blockIdx.x % tiles_n) * BN;
+    const uint32_t m0 = (blockIdx.x / tiles_n) * BM, n0 = (blockIdx.x % tiles_n) * BN;   // m0: row of the stacked problem (batch)
     const uint32_t* __restrict__ A = static_cast<const uint32_t*>(a.in);
-    const uint32_t* __restrict__ B = static_cast<const uint32_t*>(a.aux);
+    const uint32_t* __restrict__ B = static_cast<const uint32_t*>(a.aux) + (size_t)(m0 / M) * K * N;   // the tile's product's B
     constexpr int NT = NC * VT;
     constexpr int A_V4 = BM * BK / 4, B_V4 = BK * BN / 4;          // 256 + 512 uint4 per k-tile
     constexpr int PER = (A_V4 + B_V4 + NT - 1) / NT;

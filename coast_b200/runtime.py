@@ -19,6 +19,7 @@ F_STORE_DATA_SYNC, F_NO_STORE_DATA_SYNC, F_NO_LOAD_SYNC, F_NO_STORE_ADDR_SYNC = 
 PLAN_NONE, PLAN_BERNOULLI, PLAN_TABLE = 0, 1, 2
 AES_DECRYPT, AES_KEY_PER_UNIT, AES_KEY_WRITEBACK = 1, 2, 4
 UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 / QSORT batches: aux = n_units + 1 u64 byte offsets into inp
+MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32: n_units = batch*M*N, inp / aux / out hold batch A / B / C
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 

@@ -158,6 +158,7 @@ typedef struct coast_fault_plan {
  *            path: wgmma u8 x u8 on u8 limbs when M%128 == N%64 == K%128 == 0 (limb planes are per-launch scratch
  *            from a stream-ordered pool: any number of streams), register-tiled CUDA cores when M%64 == N%128 ==
  *            K%16 == 0, a plain kernel otherwise (e.g. the 9 x 9 tests).  COAST_MM_PATH=tc|tiled|naive overrides.
+ *            With COAST_MM_BATCHED: `batch` products of one shape in one launch (see below).
  *   GEMM_TF32 same with float.
  *   QSORT    in : n_units x unit_bytes, arrays of L = unit_bytes/4 int32 (L <= 1024)   out: the sorted arrays
  *   CHSTONE_SHA in : n_units x unit_bytes stream bytes (unit_bytes a multiple of 64, 64 <= unit_bytes < 2^29)
@@ -187,6 +188,17 @@ typedef struct coast_fault_plan {
  * SHA256, whose d_out is indexed by the shard's own units) and unit_base = lo.  COAST_QSORT_PATH=nested gives
  * COAST_ERR_UNSUPPORTED: a ragged batch runs the state-machine scheduling only. */
 #define COAST_UNIT_OFFSETS      0x10000u
+/* Batched matmuls (MM_U32 and GEMM_TF32 only): with COAST_MM_BATCHED in `mode`, M, N and K are the shape of ONE product and
+ * n_units = batch x M x N.  d_in holds `batch` A matrices (M x K) end to end, d_aux `batch` B matrices (K x N) and d_out
+ * receives `batch` C matrices (M x N), all dense and row-major.  The launch equals `batch` single launches, matrix b with
+ * d_in + b*M*K, d_aux + b*K*N, d_out + b*M*N (elements) and unit_base + b*M*N: the same output bytes, summed counters and
+ * minimum first_fault_unit.  Fault plans stay keyed by the global unit index (a TABLE plan has n_units entries), and the
+ * in-loop store votes keep their meaning (K + 1 votes per unit on the plain kernel).  Each path's shape rules apply to the
+ * per-matrix M, N and K; a TF32 CTA pair needs the per-matrix M to be a multiple of 256.  COAST_ERR_BAD_ARG for the bit on
+ * any other kernel, for n_units zero or not a multiple of M*N, and for batch*M or batch*N at or above 2^31.  Without the
+ * bit n_units must be M*N; with batch = 1 the launch is identical to an unbatched one.  A shard takes whole matrices
+ * [b_lo, b_hi): the three pointers and unit_base offset as above, n_units = (b_hi - b_lo) x M x N. */
+#define COAST_MM_BATCHED        0x20000u
 #define COAST_AES_DECRYPT       0x1u
 #define COAST_AES_KEY_PER_UNIT  0x2u
 #define COAST_AES_KEY_WRITEBACK 0x4u   /* with KEY_PER_UNIT: store what aes_enc_dec() leaves in key[] (TI_aes_128.c:214-221 mutates
@@ -324,7 +336,9 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  * COAST_HOST_PATH=staged|zerocopy forces a path.  Ragged calls (COAST_UNIT_OFFSETS, d_aux = host offsets, which must never
  * decrease nor give a length above unit_bytes, and for QSORT must be multiples of 4) are always staged: chunks are contiguous
  * unit ranges, each uploads its bytes and its slice of the offsets unchanged (QSORT also downloads the same byte range to
- * d_out + off[first]); a forced zerocopy or hybrid path gives COAST_ERR_UNSUPPORTED.  On any failure every copy already queued on
+ * d_out + off[first]); a forced zerocopy or hybrid path gives COAST_ERR_UNSUPPORTED.  Batched matmuls (COAST_MM_BATCHED) are
+ * staged in chunks of whole matrices sized by COAST_HOST_CHUNK_BYTES (a matrix larger than that is a chunk of its own): each
+ * chunk uploads its A and B matrices, launches with its unit_base and downloads its C matrices.  On any failure every copy already queued on
  * the caller's buffers is drained before the call returns. */
 int  coast_run_host(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
 const char* coast_last_host_path(void);   /* "zerocopy", "staged" or "one-shot" (matmuls): what the last host call did */
