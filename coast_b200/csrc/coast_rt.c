@@ -104,6 +104,10 @@ typedef struct {
 } map_desc;
 _Static_assert(sizeof(map_desc) == 80, "map_desc has no padding");
 
+/* coast_run_host staging: a device buffer and its capacity; a slot is one host-call stream and the buffers its chunks use */
+typedef struct { CUdeviceptr p; size_t cap; } dev_buf;
+typedef struct { CUstream s; dev_buf in, out, aux, stat; } host_slot;
+
 #define MAX_FN 128
 static struct {
     int inited;
@@ -121,12 +125,10 @@ static struct {
     char err[512];
     /* protection mode of the four reference entry points (coast_set_opt_passes / COAST_OPT_PASSES) */
     uint32_t def_nc, def_flags; int def_set;
-    /* coast_run_host scratch: 3 slots */
-    CUstream hs[3]; CUdeviceptr h_in[3], h_out[3], h_aux[3]; size_t h_in_cap[3], h_out_cap[3], h_aux_cap[3];
+    host_slot slot[3];               /* coast_run_host: chunk i runs on slot i % 3 */
+    dev_buf h_b; CUevent ev_b;       /* matmul host call: the replicated operand B and "B has landed" */
     /* stream-ordered scratch (the replicas' private arrays of xmr_qsort.cuh): any number of streams may launch at once */
     CUmemoryPool pool;
-    CUdeviceptr h_stat[3]; size_t h_stat_cap[3];     /* per-slot d_status staging of coast_run_host */
-    CUdeviceptr h_b; size_t h_b_cap; CUevent ev_b;   /* matmul host call: the replicated operand B and "B has landed" */
     int numa_node;                   /* NUMA node the process was bound to by coast_init (-1: not bound) */
     int busy;                        /* one host thread at a time (the reference is single-threaded); others fail loudly */
     /* tensor maps of the row-tiled kernels: coast_run_host re-encodes the same few maps every call */
@@ -329,16 +331,12 @@ int coast_init(int device) { ENTER(); LEAVE(init_impl(device)); }
 static int shutdown_impl(void) {
     if (!G.inited) return COAST_OK;
     ensure_ctx();
-    for (int i = 0; i < 3; ++i) {
-        if (G.h_in[i]) p_cuMemFree_v2(G.h_in[i]);
-        if (G.h_out[i]) p_cuMemFree_v2(G.h_out[i]);
-        if (G.h_aux[i]) p_cuMemFree_v2(G.h_aux[i]);
-        if (G.h_stat[i]) p_cuMemFree_v2(G.h_stat[i]);
-        if (G.hs[i]) p_cuStreamDestroy_v2(G.hs[i]);
-        if (i == 0) { if (G.h_b) p_cuMemFree_v2(G.h_b); if (G.ev_b) p_cuEventDestroy_v2(G.ev_b); G.h_b = 0; G.h_b_cap = 0; G.ev_b = NULL; }
-        G.h_in[i] = G.h_out[i] = G.h_aux[i] = G.h_stat[i] = 0;
-        G.h_in_cap[i] = G.h_out_cap[i] = G.h_aux_cap[i] = G.h_stat_cap[i] = 0; G.hs[i] = NULL;
-    }
+    dev_buf* bufs[] = { &G.h_b, &G.slot[0].in, &G.slot[0].out, &G.slot[0].aux, &G.slot[0].stat, &G.slot[1].in, &G.slot[1].out,
+                        &G.slot[1].aux, &G.slot[1].stat, &G.slot[2].in, &G.slot[2].out, &G.slot[2].aux, &G.slot[2].stat };
+    for (size_t i = 0; i < sizeof bufs / sizeof bufs[0]; ++i) if (bufs[i]->p) p_cuMemFree_v2(bufs[i]->p);
+    for (int i = 0; i < 3; ++i) if (G.slot[i].s) p_cuStreamDestroy_v2(G.slot[i].s);
+    if (G.ev_b) p_cuEventDestroy_v2(G.ev_b);
+    memset(G.slot, 0, sizeof G.slot); memset(&G.h_b, 0, sizeof G.h_b); G.ev_b = NULL;
     G.n_tmaps = G.tmap_next = 0;
     if (G.peer_counters) { p_cuIpcCloseMemHandle(G.peer_counters); G.peer_counters = 0; }
     p_cuMemFree_v2(G.counters);
@@ -1015,248 +1013,232 @@ static CUdeviceptr host_alias(const void* h, size_t bytes) {
  * host-call streams before returning -- and keep the error text of the failure, not of the wait. */
 static int drain_host_streams(int rc) {
     char keep[sizeof G.err]; memcpy(keep, G.err, sizeof keep);
-    for (int i = 0; i < 3; ++i) p_cuStreamSynchronize(G.hs[i]);
+    for (int i = 0; i < 3; ++i) p_cuStreamSynchronize(G.slot[i].s);
     memcpy(G.err, keep, sizeof keep);
     return rc;
 }
 
-/* Chunked pipeline: H2D -> kernel -> D2H per chunk, chunks round-robin over 3 streams / 3 staging slots. */
-static int run_host_staged(const coast_launch_desc* d, uint64_t ib, uint64_t ob, int per_unit_key, CUdeviceptr zin) {
-    int rc;
-    const uint64_t ab = aux_bytes_per_unit(d);
-    const uint64_t ibs = ib ? ib : 1;                          /* divisor of the chunk schedule */
-    /* each chunk is its own launch (own tensor map); the fault plan is keyed by the global unit index so
-     * chunking never changes results */
-    /* Chunk schedule (tools/e2e_chunk_sweep.py sweeps it): large chunks amortise the driver work of each chunk, but a fixed size leaves the copy engines idle while the first chunk goes up and the last comes
-     * down.  So chunks ramp 1,2,4,8,16,16,... MiB and shrink again towards the end (each at most half of what remains).
-     * Chunks are bounded in BYTES: a unit larger than the bound (a long CHStone stream, a long SHA message) is a chunk
-     * of its own, so the staging slots never exceed max(16 MiB, one unit) each. */
-    uint64_t max_chunk_bytes = 16ull << 20;
-    { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) max_chunk_bytes = (uint64_t)atoll(e); }   /* tuning knob */
-    const uint64_t min_chunk = ((1ull << 20) / ibs) > 1ull ? ((1ull << 20) / ibs) : 1ull;
-    const uint64_t max_chunk = (max_chunk_bytes / ibs) > min_chunk ? (max_chunk_bytes / ibs) : min_chunk;
-    const uint64_t chunk = max_chunk < d->n_units ? max_chunk : d->n_units;   /* slot buffers: the largest chunk this call can make */
-    uint64_t ramp = min_chunk;
-    uint64_t done = 0; int slot = 0;
-#define STEP(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) { rc = drv_fail(r_, #call); goto fail; } } while (0)
-    while (done < d->n_units) {
-        const uint64_t left = d->n_units - done;
-        uint64_t n = ramp < max_chunk ? ramp : max_chunk;          /* ramp up */
-        if (n > left / 2 && left > 2 * min_chunk) n = left / 2;    /* ramp down */
-        if (n < min_chunk) n = min_chunk;
-        if (n > left) n = left;
-        ramp *= 2;
-        rc = slot_reserve(&G.h_out[slot], &G.h_out_cap[slot], (size_t)(chunk * ob)); if (rc) goto fail;
-        coast_launch_desc c = *d;
-        if (zin) {                                                 /* hybrid: the kernel reads this chunk straight from mapped host memory */
-            c.d_in = (void*)(zin + done * ib);
-        } else {
-            rc = slot_reserve(&G.h_in[slot], &G.h_in_cap[slot], (size_t)(chunk * ib) > 16 ? (size_t)(chunk * ib) : 16); if (rc) goto fail;
-            if (ib) STEP(p_cuMemcpyHtoDAsync_v2(G.h_in[slot], (const uint8_t*)d->d_in + done * ib, (size_t)(n * ib), G.hs[slot]));
-            c.d_in = (void*)G.h_in[slot];
-        }
-        c.d_out = (void*)G.h_out[slot];
-        c.n_units = n; c.unit_base = d->unit_base + done;
-        if (per_unit_key) {
-            rc = slot_reserve(&G.h_aux[slot], &G.h_aux_cap[slot], (size_t)(chunk * ab)); if (rc) goto fail;
-            STEP(p_cuMemcpyHtoDAsync_v2(G.h_aux[slot], (const uint8_t*)d->d_aux + done * ab, (size_t)(n * ab), G.hs[slot]));
-            c.d_aux = (void*)G.h_aux[slot];
-        }
-        if (d->d_status) {                                         /* kernels index status[] chunk-locally: stage it per slot */
-            rc = slot_reserve(&G.h_stat[slot], &G.h_stat_cap[slot], (size_t)chunk); if (rc) goto fail;
-            c.d_status = (void*)G.h_stat[slot];
-        }
-        rc = launch_impl(&c, G.hs[slot]); if (rc) goto fail;
-        STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + done * ob, G.h_out[slot], (size_t)(n * ob), G.hs[slot]));
-        if (per_unit_key && d->kernel == COAST_K_AES128 && (d->mode & COAST_AES_KEY_WRITEBACK))
-            STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_aux + done * ab, G.h_aux[slot], (size_t)(n * ab), G.hs[slot]));
-        if (d->d_status) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_status + done, G.h_stat[slot], (size_t)n, G.hs[slot]));
-        done += n; slot = (slot + 1) % 3;
-    }
-#undef STEP
-    return COAST_OK;
-fail:
-    return drain_host_streams(rc);
+/* The chunk pipeline.  A schedule cuts the call into chunks of whole items (units, matmul rows or products); chunk i runs on
+ * slot i % 3: its input and aux bytes go up into the slot, its launch reads and writes the slot, its output and status bytes
+ * come down, so uploads, kernels and downloads of neighbouring chunks overlap (PCIe is full duplex).  Each chunk is its own
+ * launch keyed by the global unit index (unit_base), and the fault plan is keyed by that index, so chunking never changes
+ * results. */
+typedef struct { uint64_t off, len; } byte_range;           /* bytes [off, off + len) of one of the caller's buffers */
+typedef struct {
+    uint64_t items;                                          /* items the chunk takes */
+    byte_range in, aux, out, stat;                           /* of d_in, d_aux, d_out and d_status */
+    uint64_t n_units, unit_base;                             /* of the chunk's launch; unit_base is added to the call's */
+    uint32_t M;                                              /* rows of a matmul row block (0: the call's M) */
+    uint64_t in_bias, out_bias;                              /* the launch's d_in / d_out are the slot's buffers minus these */
+} host_chunk;
+
+typedef struct host_sched host_sched;
+struct host_sched {
+    const coast_launch_desc* d;
+    /* the chunk after `done` items; *budget is the schedule's running bound (units or bytes), advanced for the next chunk */
+    void (*next)(const host_sched* s, uint64_t done, uint64_t* budget, host_chunk* c);
+    uint64_t total, budget;                                  /* items of the call; the first chunk's budget */
+    uint64_t ib, ab, ob, upi;                                /* per item: bytes of input, aux data and output; units */
+    uint64_t min_items, max_items, max_bytes;                /* chunk bounds */
+    uint64_t min_in;                                         /* least input slot: an empty input still launches on an address */
+    uint64_t shared_b;                                       /* bytes of the matmul's B: uploaded once, every chunk waits for it */
+    CUdeviceptr zin;                                         /* hybrid: the input's mapped alias, which the kernels read in place */
+    int qs, aux_back;                                        /* ragged quicksort (output in place of the input); AES key write-back */
+    const char* path;                                        /* what coast_last_host_path() reports */
+};
+
+/* Items [first, first + n) of a schedule with fixed bytes per item. */
+static void item_chunk(const host_sched* s, uint64_t first, uint64_t n, host_chunk* c) {
+    memset(c, 0, sizeof *c);
+    c->items = n; c->n_units = n * s->upi; c->unit_base = first * s->upi;
+    c->in = (byte_range){ first * s->ib, n * s->ib };
+    c->aux = (byte_range){ first * s->ab, n * s->ab };
+    c->out = (byte_range){ first * s->ob, n * s->ob };
+    c->stat = (byte_range){ c->unit_base, c->n_units };     /* one status byte per unit */
 }
 
-/* Ragged host call (COAST_UNIT_OFFSETS, d_aux = the caller's host offsets): staged only.  A chunk is a contiguous unit range
- * whose input, offset slice and outputs fit the chunk bytes (ramping 1, 2, 4, .. MiB up to COAST_HOST_CHUNK_BYTES, 16 MiB by
- * default); a longer unit is a chunk of its own.  Each chunk uploads its bytes [off[first], off[end]) and its offset slice
- * off[first .. end] unchanged, and launches with the staging slot's address minus off[first] as d_in (exact under u64
- * wraparound), so the caller's offsets are never rewritten.  Quicksort writes its arrays in place of the input bytes: a chunk's
- * output is the same span, downloaded to d_out + off[first] from an output slot biased the same way.  `span_copies` counts
- * the span once (SHA-256, CRC16) or twice (quicksort: in and out) in the chunk budget. */
-static uint64_t ragged_chunk_end(const uint64_t* off, uint64_t first, uint64_t n, uint64_t budget, uint64_t per_unit,
-                                 uint64_t span_copies) {
+/* Uniform units.  Large chunks amortise the driver work of each chunk, but a fixed size leaves the copy engines idle while the
+ * first chunk goes up and the last comes down.  So chunks ramp 1, 2, 4, .. MiB of input up to COAST_HOST_CHUNK_BYTES and
+ * shrink again towards the end, each at most half of what remains (tools/e2e_chunk_sweep.py sweeps the bound).  The bounds are
+ * in BYTES: a unit larger than the bound (a long CHStone stream, a long SHA message) is a chunk of its own. */
+static void next_units(const host_sched* s, uint64_t done, uint64_t* ramp, host_chunk* c) {
+    const uint64_t left = s->total - done;
+    uint64_t n = *ramp < s->max_items ? *ramp : s->max_items;          /* ramp up */
+    if (n > left / 2 && left > 2 * s->min_items) n = left / 2;         /* ramp down */
+    if (n < s->min_items) n = s->min_items;
+    if (n > left) n = left;
+    *ramp *= 2;
+    item_chunk(s, done, n, c);
+}
+
+/* Ragged units (COAST_UNIT_OFFSETS, d_aux = the caller's host offsets): a chunk is the longest unit range whose bytes
+ * [off[first], off[end]) -- counted twice for quicksort, in and out -- and per-unit offset and output bytes fit the budget,
+ * which ramps 1, 2, 4, .. MiB up to COAST_HOST_CHUNK_BYTES; a longer unit is a chunk of its own.  The chunk uploads its bytes
+ * and its offset slice off[first .. end] unchanged and launches with the slot's address minus off[first] as d_in (exact under
+ * u64 wraparound), so the caller's offsets are never rewritten.  Quicksort sorts each array in place of its input bytes: the
+ * output is the same span, downloaded from an output slot biased the same way. */
+static void next_ragged(const host_sched* s, uint64_t first, uint64_t* budget, host_chunk* c) {
+    const uint64_t* off = (const uint64_t*)s->d->d_aux;
+    const uint64_t per_unit = s->ob + 8u, span_copies = s->qs ? 2u : 1u;
     uint64_t e = first + 1;
-    while (e < n && (off[e + 1] - off[first]) * span_copies + (e + 1 - first) * per_unit <= budget) ++e;
-    return e;
-}
-static int run_host_ragged(const coast_launch_desc* d, coast_stats* out, int* dwc_fired) {
-    int rc = ragged_check(d); if (rc) return rc;
-    const char* hp = getenv("COAST_HOST_PATH");
-    if (hp && (!strcmp(hp, "zerocopy") || !strcmp(hp, "hybrid")))
-        return fail(COAST_ERR_UNSUPPORTED, "COAST_HOST_PATH=%s: ragged host calls (COAST_UNIT_OFFSETS) are staged only", hp);
-    if (d->n_units == 0) return sync_impl(G.hs[2], out, dwc_fired);
-    if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null host buffer");
-    const uint64_t* off = (const uint64_t*)d->d_aux, n = d->n_units;
-    const int qs = d->kernel == COAST_K_QSORT;
-    for (uint64_t u = 0; u < n; ++u)
-        if (off[u + 1] < off[u] || off[u + 1] - off[u] > d->unit_bytes)
-            return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: unit %llu runs from offset %llu to %llu; offsets must not decrease and no "
-                                           "length may exceed unit_bytes (%u)", (unsigned long long)u, (unsigned long long)off[u],
-                        (unsigned long long)off[u + 1], d->unit_bytes);
-    if (qs)
-        for (uint64_t u = 0; u <= n; ++u)
-            if (off[u] & 3u)
-                return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: offset %llu is %llu; quicksort offsets must be multiples of 4",
-                            (unsigned long long)u, (unsigned long long)off[u]);
-    const uint64_t ob = KINFO[d->kernel].out_bytes, per_unit = ob + 8u, span_copies = qs ? 2u : 1u;
-    uint64_t max_chunk_bytes = 16ull << 20;
-    { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) max_chunk_bytes = (uint64_t)atoll(e); }
-    const uint64_t ramp0 = (1ull << 20) < max_chunk_bytes ? (1ull << 20) : max_chunk_bytes;
-    /* the schedule is walked twice: once to size the three slots (never regrown while a chunk may use them), once to run */
-    uint64_t max_span = 16, max_cnt = 1, n_chunks = 0;
-    for (uint64_t first = 0, budget = ramp0; first < n; ++n_chunks) {
-        const uint64_t e = ragged_chunk_end(off, first, n, budget, per_unit, span_copies);
-        if (off[e] - off[first] > max_span) max_span = off[e] - off[first];
-        if (e - first > max_cnt) max_cnt = e - first;
-        first = e; budget = budget * 2 < max_chunk_bytes ? budget * 2 : max_chunk_bytes;
-    }
-    for (int s = 0; s < 3 && (uint64_t)s < n_chunks; ++s) {
-        if ((rc = slot_reserve(&G.h_in[s], &G.h_in_cap[s], (size_t)max_span))) return rc;
-        if ((rc = slot_reserve(&G.h_aux[s], &G.h_aux_cap[s], (size_t)(max_cnt + 1) * 8u))) return rc;
-        if ((rc = slot_reserve(&G.h_out[s], &G.h_out_cap[s], (size_t)(qs ? max_span : max_cnt * ob)))) return rc;
-        if (d->d_status && (rc = slot_reserve(&G.h_stat[s], &G.h_stat_cap[s], (size_t)max_cnt))) return rc;
-    }
-    int slot = 0;
-#define STEP(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) { rc = drv_fail(r_, #call); goto fail; } } while (0)
-    for (uint64_t first = 0, budget = ramp0; first < n; slot = (slot + 1) % 3) {
-        const uint64_t e = ragged_chunk_end(off, first, n, budget, per_unit, span_copies), cnt = e - first, span = off[e] - off[first];
-        if (span) STEP(p_cuMemcpyHtoDAsync_v2(G.h_in[slot], (const uint8_t*)d->d_in + off[first], (size_t)span, G.hs[slot]));
-        STEP(p_cuMemcpyHtoDAsync_v2(G.h_aux[slot], off + first, (size_t)(cnt + 1) * 8u, G.hs[slot]));
-        coast_launch_desc c = *d;
-        c.d_in = (const void*)(uintptr_t)(G.h_in[slot] - off[first]);
-        c.d_aux = (const void*)G.h_aux[slot];
-        c.d_out = qs ? (void*)(uintptr_t)(G.h_out[slot] - off[first]) : (void*)G.h_out[slot];
-        c.n_units = cnt; c.unit_base = d->unit_base + first;
-        if (d->d_status) c.d_status = (void*)G.h_stat[slot];
-        rc = launch_impl(&c, G.hs[slot]); if (rc) goto fail;
-        if (qs) { if (span) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + off[first], G.h_out[slot], (size_t)span, G.hs[slot])); }
-        else STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + first * ob, G.h_out[slot], (size_t)(cnt * ob), G.hs[slot]));
-        if (d->d_status) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_status + first, G.h_stat[slot], (size_t)cnt, G.hs[slot]));
-        first = e; budget = budget * 2 < max_chunk_bytes ? budget * 2 : max_chunk_bytes;
-    }
-#undef STEP
-    G.last_host_path = "staged";
-    DRV(p_cuStreamSynchronize(G.hs[0])); DRV(p_cuStreamSynchronize(G.hs[1]));
-    return sync_impl(G.hs[2], out, dwc_fired);
-fail:
-    return drain_host_streams(rc);
+    while (e < s->total && (off[e + 1] - off[first]) * span_copies + (e + 1 - first) * per_unit <= *budget) ++e;
+    *budget = *budget * 2 < s->max_bytes ? *budget * 2 : s->max_bytes;
+    memset(c, 0, sizeof *c);
+    c->items = c->n_units = e - first; c->unit_base = first;
+    c->in = (byte_range){ off[first], off[e] - off[first] }; c->in_bias = off[first];
+    c->aux = (byte_range){ first * 8u, (e - first + 1) * 8u };
+    c->out = s->qs ? c->in : (byte_range){ first * s->ob, (e - first) * s->ob };
+    c->out_bias = s->qs ? off[first] : 0;
+    c->stat = (byte_range){ first, e - first };
 }
 
-/* Matmul host call.  B (replicated operand) goes up once; C is produced in row blocks: block i's rows of A upload, its
- * launch and the download of its rows of C run on stream i % 3, so uploads, tensor-core work and downloads of
- * neighbouring blocks overlap (PCIe is full duplex).  The fault plan is keyed by the global element index
- * (unit_base + row * N + col), so blocking never changes results.  Small or oddly-shaped problems go in one block. */
-static int run_host_matmul(const coast_launch_desc* d, coast_stats* out, int* dwc_fired) {
+/* Batched matmuls (COAST_MM_BATCHED): chunks of max_items whole products, each with its own A, B and C. */
+static void next_products(const host_sched* s, uint64_t done, uint64_t* budget, host_chunk* c) {
+    (void)budget;
+    const uint64_t left = s->total - done;
+    item_chunk(s, done, left < s->max_items ? left : s->max_items, c);
+}
+
+/* Matmul row blocks: max_items rows of A up and of C down per chunk; B is the schedule's shared operand. */
+static void next_row_block(const host_sched* s, uint64_t done, uint64_t* budget, host_chunk* c) {
+    next_products(s, done, budget, c);
+    c->M = (uint32_t)c->items;
+}
+
+static void grow(uint64_t* need, uint64_t len) { if (len > *need) *need = len; }
+
+/* Runs a call's chunks.  The schedule is walked twice: once to size each slot for the largest chunk it gets -- every slot is
+ * reserved before the first copy, so a failed allocation never leaves a partly written output -- and once to run. */
+static int run_chunks(const host_sched* s, coast_stats* out, int* dwc_fired) {
+    const coast_launch_desc* d = s->d;
+    struct { uint64_t in, aux, out, stat; } need[3];
+    memset(need, 0, sizeof need);
+    uint64_t n_chunks = 0;
+    for (uint64_t done = 0, budget = s->budget; done < s->total; ++n_chunks) {
+        host_chunk c; s->next(s, done, &budget, &c);
+        const int i = (int)(n_chunks % 3);
+        grow(&need[i].in, c.in.len); grow(&need[i].aux, c.aux.len); grow(&need[i].out, c.out.len); grow(&need[i].stat, c.stat.len);
+        done += c.items;
+    }
     int rc;
-    const size_t bb = (size_t)d->K * d->N * 4;
-    uint32_t blocks = 1, rows = d->M;
-    { const char* hp = getenv("COAST_HOST_PATH");
-      if (d->M % 128u == 0 && d->M >= 512u && !(hp && !strcmp(hp, "one-shot"))) {
-          blocks = d->M / 128u < 8u ? d->M / 128u : 8u;
-          rows = ((d->M / 128u + blocks - 1u) / blocks) * 128u;
-          blocks = (d->M + rows - 1u) / rows;
-      } }
-    rc = slot_reserve(&G.h_b, &G.h_b_cap, bb); if (rc) return rc;
-    if (!G.ev_b) DRV(p_cuEventCreate(&G.ev_b, CU_EVENT_DISABLE_TIMING));
-    for (int i = 0; i < 3 && (uint32_t)i < blocks; ++i) {
-        rc = slot_reserve(&G.h_in[i], &G.h_in_cap[i], (size_t)rows * d->K * 4); if (rc) return rc;
-        rc = slot_reserve(&G.h_out[i], &G.h_out_cap[i], (size_t)rows * d->N * 4); if (rc) return rc;
+    for (int i = 0; i < 3 && (uint64_t)i < n_chunks; ++i) {
+        host_slot* sl = &G.slot[i];
+        const uint64_t in = need[i].in > s->min_in ? need[i].in : s->min_in;
+        if (!s->zin && (rc = slot_reserve(&sl->in.p, &sl->in.cap, in))) return rc;
+        if ((rc = slot_reserve(&sl->out.p, &sl->out.cap, s->qs ? in : need[i].out))) return rc;   /* quicksort: in's twin */
+        if ((rc = slot_reserve(&sl->aux.p, &sl->aux.cap, need[i].aux))) return rc;
+        if (d->d_status && (rc = slot_reserve(&sl->stat.p, &sl->stat.cap, need[i].stat))) return rc;
+    }
+    if (s->shared_b) {
+        if ((rc = slot_reserve(&G.h_b.p, &G.h_b.cap, s->shared_b))) return rc;
+        if (!G.ev_b) DRV(p_cuEventCreate(&G.ev_b, CU_EVENT_DISABLE_TIMING));
     }
 #define STEP(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) { rc = drv_fail(r_, #call); goto fail; } } while (0)
-    /* the first block of A leads on stream 0, B follows on stream 1: the first launch needs both, later blocks only their A */
-    for (uint32_t i = 0; i < blocks; ++i) {
-        const int slot = (int)(i % 3u);
-        const uint32_t r0 = i * rows, nr = d->M - r0 < rows ? d->M - r0 : rows;
-        STEP(p_cuMemcpyHtoDAsync_v2(G.h_in[slot], (const uint8_t*)d->d_in + (size_t)r0 * d->K * 4, (size_t)nr * d->K * 4, G.hs[slot]));
-        if (i == 0) {
-            STEP(p_cuMemcpyHtoDAsync_v2(G.h_b, d->d_aux, bb, G.hs[1]));
-            STEP(p_cuEventRecord(G.ev_b, G.hs[1]));
+    uint64_t done = 0, budget = s->budget;
+    for (uint64_t i = 0; done < s->total; ++i) {
+        host_chunk k; s->next(s, done, &budget, &k);
+        const host_slot* sl = &G.slot[i % 3];
+        coast_launch_desc c = *d;
+        if (s->zin) {
+            c.d_in = (const void*)(uintptr_t)(s->zin + k.in.off);
+        } else {
+            if (k.in.len) STEP(p_cuMemcpyHtoDAsync_v2(sl->in.p, (const uint8_t*)d->d_in + k.in.off, (size_t)k.in.len, sl->s));
+            c.d_in = (const void*)(uintptr_t)(sl->in.p - k.in_bias);
         }
-        STEP(p_cuStreamWaitEvent(G.hs[slot], G.ev_b, 0));
-        coast_launch_desc c = *d;
-        c.d_in = (void*)G.h_in[slot]; c.d_aux = (void*)G.h_b; c.d_out = (void*)G.h_out[slot];
-        c.M = nr; c.n_units = (uint64_t)nr * d->N; c.unit_base = d->unit_base + (uint64_t)r0 * d->N;
-        rc = launch_impl(&c, G.hs[slot]); if (rc) goto fail;
-        STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + (size_t)r0 * d->N * 4, G.h_out[slot], (size_t)nr * d->N * 4, G.hs[slot]));
+        if (k.aux.len) {
+            STEP(p_cuMemcpyHtoDAsync_v2(sl->aux.p, (const uint8_t*)d->d_aux + k.aux.off, (size_t)k.aux.len, sl->s));
+            c.d_aux = (const void*)sl->aux.p;
+        }
+        if (s->shared_b) {                                   /* B follows the first chunk's input, on stream 1 */
+            if (i == 0) {
+                STEP(p_cuMemcpyHtoDAsync_v2(G.h_b.p, d->d_aux, (size_t)s->shared_b, G.slot[1].s));
+                STEP(p_cuEventRecord(G.ev_b, G.slot[1].s));
+            }
+            STEP(p_cuStreamWaitEvent(sl->s, G.ev_b, 0));
+            c.d_aux = (const void*)G.h_b.p;
+        }
+        c.d_out = (void*)(uintptr_t)(sl->out.p - k.out_bias);
+        if (d->d_status) c.d_status = (void*)sl->stat.p;    /* kernels index status[] chunk-locally */
+        c.n_units = k.n_units; c.unit_base = d->unit_base + k.unit_base;
+        if (k.M) c.M = k.M;
+        rc = launch_impl(&c, sl->s); if (rc) goto fail;
+        if (k.out.len) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + k.out.off, sl->out.p, (size_t)k.out.len, sl->s));
+        if (s->aux_back) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_aux + k.aux.off, sl->aux.p, (size_t)k.aux.len, sl->s));
+        if (d->d_status) STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_status + k.stat.off, sl->stat.p, (size_t)k.stat.len, sl->s));
+        done += k.items;
     }
 #undef STEP
-    G.last_host_path = blocks > 1 ? "row-blocks" : "one-shot";
-    DRV(p_cuStreamSynchronize(G.hs[0])); DRV(p_cuStreamSynchronize(G.hs[1]));
-    return sync_impl(G.hs[2], out, dwc_fired);
+    G.last_host_path = s->path;
+    DRV(p_cuStreamSynchronize(G.slot[0].s)); DRV(p_cuStreamSynchronize(G.slot[1].s));
+    return sync_impl(G.slot[2].s, out, dwc_fired);
 fail:
     return drain_host_streams(rc);
 }
 
-/* Batched matmul host call (COAST_MM_BATCHED): chunks of whole products, as many as fit the chunk bytes (COAST_HOST_CHUNK_BYTES,
- * 16 MiB by default, counting A, B and C; a product larger than that is a chunk of its own), round-robin over the three host
- * streams and staging slots.  A chunk uploads its A and B matrices, launches with unit_base + first * M * N and downloads its
- * C matrices, so uploads, kernels and downloads of neighbouring chunks overlap. */
-static int run_host_mm_batched(const coast_launch_desc* d, coast_stats* out, int* dwc_fired) {
-    int rc;
-    if (!d->d_in || !d->d_out || !d->d_aux) return fail(COAST_ERR_BAD_ARG, "null host buffer");
-    const uint64_t mn = (uint64_t)d->M * d->N, batch = d->n_units / mn;
-    const uint64_t ab = (uint64_t)d->M * d->K * 4u, bb = (uint64_t)d->K * d->N * 4u, cb = mn * 4u;
-    uint64_t max_chunk_bytes = 16ull << 20;
-    { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) max_chunk_bytes = (uint64_t)atoll(e); }
-    uint64_t per = max_chunk_bytes / (ab + bb + cb);
-    if (per < 1) per = 1;
-    if (per > batch) per = batch;
-    for (int s = 0; s < 3 && (uint64_t)s * per < batch; ++s) {
-        if ((rc = slot_reserve(&G.h_in[s], &G.h_in_cap[s], (size_t)(per * ab)))) return rc;
-        if ((rc = slot_reserve(&G.h_aux[s], &G.h_aux_cap[s], (size_t)(per * bb)))) return rc;
-        if ((rc = slot_reserve(&G.h_out[s], &G.h_out_cap[s], (size_t)(per * cb)))) return rc;
-    }
-    int slot = 0;
-#define STEP(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) { rc = drv_fail(r_, #call); goto fail; } } while (0)
-    for (uint64_t first = 0; first < batch; first += per, slot = (slot + 1) % 3) {
-        const uint64_t cnt = batch - first < per ? batch - first : per;
-        STEP(p_cuMemcpyHtoDAsync_v2(G.h_in[slot], (const uint8_t*)d->d_in + first * ab, (size_t)(cnt * ab), G.hs[slot]));
-        STEP(p_cuMemcpyHtoDAsync_v2(G.h_aux[slot], (const uint8_t*)d->d_aux + first * bb, (size_t)(cnt * bb), G.hs[slot]));
-        coast_launch_desc c = *d;
-        c.d_in = (void*)G.h_in[slot]; c.d_aux = (void*)G.h_aux[slot]; c.d_out = (void*)G.h_out[slot];
-        c.n_units = cnt * mn; c.unit_base = d->unit_base + first * mn;
-        rc = launch_impl(&c, G.hs[slot]); if (rc) goto fail;
-        STEP(p_cuMemcpyDtoHAsync_v2((uint8_t*)d->d_out + first * cb, G.h_out[slot], (size_t)(cnt * cb), G.hs[slot]));
-    }
-#undef STEP
-    G.last_host_path = "staged";
-    DRV(p_cuStreamSynchronize(G.hs[0])); DRV(p_cuStreamSynchronize(G.hs[1]));
-    return sync_impl(G.hs[2], out, dwc_fired);
-fail:
-    return drain_host_streams(rc);
-}
-
-/* `d_in` / `d_out` / `d_aux` / `d_status` of the descriptor are HOST pointers here. */
+/* `d_in` / `d_out` / `d_aux` / `d_status` of the descriptor are HOST pointers here.  The policy of the host call: the refusals,
+ * which schedule cuts the call into chunks and, for the uniform kernels, whether the bytes move by staged copies, hybrid or one
+ * zero-copy launch. */
 static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_fired) {
     int rc = ensure_ctx(); if (rc) return rc;
     if (!d) return fail(COAST_ERR_BAD_ARG, "null descriptor");
     if (d->plan && d->plan->mode == COAST_PLAN_TABLE) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: TABLE plans need device pointers; use coast_launch");
-    for (int i = 0; i < 3; ++i) if (!G.hs[i]) DRV(p_cuStreamCreate(&G.hs[i], CU_STREAM_NON_BLOCKING));
-    if (d->mode & COAST_UNIT_OFFSETS) return run_host_ragged(d, out, dwc_fired);
+    for (int i = 0; i < 3; ++i) if (!G.slot[i].s) DRV(p_cuStreamCreate(&G.slot[i].s, CU_STREAM_NON_BLOCKING));
+    const char* hp = getenv("COAST_HOST_PATH");
+    uint64_t chunk_bytes = 16ull << 20;                      /* largest chunk (tuning knob; ragged and batched: of all its bytes) */
+    { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) chunk_bytes = (uint64_t)atoll(e); }
+    host_sched s; memset(&s, 0, sizeof s);
+    s.d = d; s.upi = 1; s.path = "staged";
+
+    if (d->mode & COAST_UNIT_OFFSETS) {                      /* ragged: staged only */
+        if ((rc = ragged_check(d))) return rc;
+        if (hp && (!strcmp(hp, "zerocopy") || !strcmp(hp, "hybrid")))
+            return fail(COAST_ERR_UNSUPPORTED, "COAST_HOST_PATH=%s: ragged host calls (COAST_UNIT_OFFSETS) are staged only", hp);
+        if (d->n_units == 0) return sync_impl(G.slot[2].s, out, dwc_fired);
+        if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null host buffer");
+        const uint64_t* off = (const uint64_t*)d->d_aux, n = d->n_units;
+        s.qs = d->kernel == COAST_K_QSORT;
+        for (uint64_t u = 0; u < n; ++u)
+            if (off[u + 1] < off[u] || off[u + 1] - off[u] > d->unit_bytes)
+                return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: unit %llu runs from offset %llu to %llu; offsets must not decrease and no "
+                                               "length may exceed unit_bytes (%u)", (unsigned long long)u, (unsigned long long)off[u],
+                            (unsigned long long)off[u + 1], d->unit_bytes);
+        if (s.qs)
+            for (uint64_t u = 0; u <= n; ++u)
+                if (off[u] & 3u)
+                    return fail(COAST_ERR_BAD_ARG, "COAST_UNIT_OFFSETS: offset %llu is %llu; quicksort offsets must be multiples of 4",
+                                (unsigned long long)u, (unsigned long long)off[u]);
+        s.next = next_ragged; s.total = n; s.ob = KINFO[d->kernel].out_bytes; s.min_in = 16;
+        s.budget = (1ull << 20) < chunk_bytes ? (1ull << 20) : chunk_bytes; s.max_bytes = chunk_bytes;
+        return run_chunks(&s, out, dwc_fired);
+    }
     if ((d->mode & COAST_MM_BATCHED) && (rc = batched_check(d))) return rc;
-    const uint64_t ob = coast_out_bytes(d->kernel, d->unit_bytes);
     if (d->kernel == COAST_K_MM_U32 || d->kernel == COAST_K_GEMM_TF32) {
         if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");
-        return (d->mode & COAST_MM_BATCHED) ? run_host_mm_batched(d, out, dwc_fired) : run_host_matmul(d, out, dwc_fired);
+        const uint64_t ab = (uint64_t)d->M * d->K * 4u, bb = (uint64_t)d->K * d->N * 4u, cb = (uint64_t)d->M * d->N * 4u;
+        if (d->mode & COAST_MM_BATCHED) {                    /* as many whole products as the chunk bytes hold, at least one */
+            if (!d->d_in || !d->d_out || !d->d_aux) return fail(COAST_ERR_BAD_ARG, "null host buffer");
+            s.next = next_products; s.total = d->n_units / ((uint64_t)d->M * d->N); s.upi = (uint64_t)d->M * d->N;
+            s.ib = ab; s.ab = bb; s.ob = cb;
+            s.max_items = chunk_bytes / (ab + bb + cb) ? chunk_bytes / (ab + bb + cb) : 1u;
+        } else {
+            /* B (the replicated operand) goes up once; C comes in at most 8 blocks of whole 128-row groups.  Small or oddly
+             * shaped problems go in one block. */
+            uint64_t rows = d->M;
+            if (d->M % 128u == 0 && d->M >= 512u && !(hp && !strcmp(hp, "one-shot"))) {
+                const uint64_t blocks = d->M / 128u < 8u ? d->M / 128u : 8u;
+                rows = ((d->M / 128u + blocks - 1u) / blocks) * 128u;
+            }
+            s.next = next_row_block; s.total = d->M; s.upi = d->N; s.ib = (uint64_t)d->K * 4u; s.ob = (uint64_t)d->N * 4u;
+            s.max_items = rows; s.shared_b = bb;
+            s.path = rows < d->M ? "row-blocks" : "one-shot";
+        }
+        return run_chunks(&s, out, dwc_fired);
     }
-    const uint64_t ib = in_bytes_per_unit(d);
+    const uint64_t ob = coast_out_bytes(d->kernel, d->unit_bytes), ib = in_bytes_per_unit(d);
     /* a zero-length SHA-256 message (sha256_hash(len = 0) hashes one padded block) has nothing to stage */
     if (!ob || (!ib && d->kernel != COAST_K_SHA256)) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: kernel %u", d->kernel);
     const int per_unit_key = aux_bytes_per_unit(d) != 0;
-    if (d->n_units == 0) return sync_impl(G.hs[2], out, dwc_fired);
+    if (d->n_units == 0) return sync_impl(G.slot[2].s, out, dwc_fired);
 
     /* Three ways to move the bytes (COAST_HOST_PATH=staged|hybrid|zerocopy overrides the default):
      *   staged  : H2D -> kernel -> D2H per chunk over three streams (any host memory);
@@ -1265,7 +1247,6 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
      *             per chunk;
      *   zerocopy: ONE launch reads and WRITES mapped host memory: SM stores of 16-32 bytes per lane to host memory
      *             are small PCIe writes, so it is meant for calls whose output is small. */
-    const char* hp = getenv("COAST_HOST_PATH");
     const int streams_once = KINFO[d->kernel].streams_once;
     /* default: staged -- except when the output is tiny next to the input (crc16: 2 of 64 bytes, CHStone sha: 20 bytes per
      * stream), where one zero-copy launch on pinned buffers reads each input byte once and saves the chunk pipeline's copies */
@@ -1283,18 +1264,23 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
             c.d_in = (void*)zi; c.d_out = (void*)zo;
             if (per_unit_key) c.d_aux = (void*)za;
             if (d->d_status) c.d_status = (void*)zs;
-            rc = launch_impl(&c, G.hs[2]); if (rc) return rc;
+            rc = launch_impl(&c, G.slot[2].s); if (rc) return rc;
             G.last_host_path = "zerocopy";
-            return sync_impl(G.hs[2], out, dwc_fired);
+            return sync_impl(G.slot[2].s, out, dwc_fired);
         }
         if (hp) return fail(COAST_ERR_BAD_ARG, "COAST_HOST_PATH=zerocopy needs pinned (mapped) host buffers");
         zin = 0;                                                   /* the default policy falls back to staged copies for pageable memory */
     }
     if (hp && want == 1 && streams_once && ib && !zin) return fail(COAST_ERR_BAD_ARG, "COAST_HOST_PATH=hybrid needs a pinned (mapped) input buffer");
-    rc = run_host_staged(d, ib, ob, per_unit_key, want ? zin : 0); if (rc) return rc;
-    G.last_host_path = (want && zin) ? "hybrid" : "staged";
-    DRV(p_cuStreamSynchronize(G.hs[0])); DRV(p_cuStreamSynchronize(G.hs[1]));
-    return sync_impl(G.hs[2], out, dwc_fired);
+    const uint64_t ibs = ib ? ib : 1;                              /* divisor of the chunk bounds */
+    s.next = next_units; s.total = d->n_units; s.ib = ib; s.ab = aux_bytes_per_unit(d); s.ob = ob; s.min_in = 16;
+    s.min_items = (1ull << 20) / ibs > 1u ? (1ull << 20) / ibs : 1u;
+    s.max_items = chunk_bytes / ibs > s.min_items ? chunk_bytes / ibs : s.min_items;
+    s.budget = s.min_items;
+    s.aux_back = per_unit_key && d->kernel == COAST_K_AES128 && (d->mode & COAST_AES_KEY_WRITEBACK);
+    s.zin = zin;                                                   /* nonzero only when hybrid was asked for */
+    if (zin) s.path = "hybrid";
+    return run_chunks(&s, out, dwc_fired);
 }
 static int run_host_guarded(const coast_launch_desc* d, coast_stats* out, int call_handler) {
     ENTER();

@@ -326,14 +326,19 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
 /* What the reference's protected function call becomes: host in -> xMR kernel -> host out,
  * counters folded as coast_sync().  d_in / d_out / d_aux / d_status of the descriptor are HOST
  * pointers here.
- *   pinned buffers (cuMemHostAlloc, cudaHostAlloc/Register, coast_host_alloc, torch pin_memory)
- *     and a kernel that reads its input once (CRC16, SHA256, AES128, CHSTONE_SHA): ONE launch
- *     reads the mapped host memory through the TMA ring and writes the voted output straight
- *     back -- upload, compute and download overlap inside the kernel (zero-copy);
- *   anything else (pageable memory, matmuls, quicksort): staged -- H2D -> kernel -> D2H per
- *     chunk, chunks of 1..16 MiB round-robin over three internal streams and staging slots
- *     (a unit larger than 16 MiB is a chunk of its own).  d_status is staged per chunk too.
- * COAST_HOST_PATH=staged|zerocopy forces a path.  Ragged calls (COAST_UNIT_OFFSETS, d_aux = host offsets, which must never
+ *   staged (the default): H2D -> kernel -> D2H per chunk, chunks round-robin over three
+ *     internal streams and staging slots, every slot reserved before the first copy.  Uniform
+ *     units come in chunks of 1..16 MiB of input (COAST_HOST_CHUNK_BYTES; a unit larger than
+ *     that is a chunk of its own); d_status is staged per chunk too;
+ *   zerocopy: pinned buffers (cuMemHostAlloc, cudaHostAlloc/Register, coast_host_alloc, torch
+ *     pin_memory) and a kernel that reads its input once (CRC16, SHA256, AES128, CHSTONE_SHA):
+ *     ONE launch reads the mapped host memory and writes the voted output straight back; the
+ *     default when the output is at most 1/8 of the input (CRC16, CHSTONE_SHA);
+ *   hybrid: the staged chunks' kernels read a pinned input in place, outputs are staged;
+ *   matmuls (MM_U32, GEMM_TF32): B goes up once and C comes down in row blocks (one-shot: one
+ *     block for small or oddly shaped problems).
+ * COAST_HOST_PATH=staged|hybrid|zerocopy forces a path, and for matmuls one-shot forces one block
+ * (INTEGRATION.md §config).  Ragged calls (COAST_UNIT_OFFSETS, d_aux = host offsets, which must never
  * decrease nor give a length above unit_bytes, and for QSORT must be multiples of 4) are always staged: chunks are contiguous
  * unit ranges, each uploads its bytes and its slice of the offsets unchanged (QSORT also downloads the same byte range to
  * d_out + off[first]); a forced zerocopy or hybrid path gives COAST_ERR_UNSUPPORTED.  Batched matmuls (COAST_MM_BATCHED) are
@@ -341,7 +346,8 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  * chunk uploads its A and B matrices, launches with its unit_base and downloads its C matrices.  On any failure every copy already queued on
  * the caller's buffers is drained before the call returns. */
 int  coast_run_host(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
-const char* coast_last_host_path(void);   /* "zerocopy", "staged" or "one-shot" (matmuls): what the last host call did */
+/* What the last host call did: "staged", "hybrid" or "zerocopy"; unbatched matmuls: "row-blocks" or "one-shot". */
+const char* coast_last_host_path(void);
 /* Same, but never calls FAULT_DETECTED_DWC (fault campaigns want the count, not SIGABRT). */
 int  coast_run_host_noabort(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
 
