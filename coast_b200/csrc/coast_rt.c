@@ -106,7 +106,7 @@ _Static_assert(sizeof(map_desc) == 80, "map_desc has no padding");
 
 /* coast_run_host staging: a device buffer and its capacity; a slot is one host-call stream and the buffers its chunks use */
 typedef struct { CUdeviceptr p; size_t cap; } dev_buf;
-typedef struct { CUstream s; dev_buf in, out, aux, stat; } host_slot;
+typedef struct { CUstream s; dev_buf in, out, aux, stat, rows; } host_slot;
 
 #define MAX_FN 128
 static struct {
@@ -136,7 +136,7 @@ static struct {
     int n_tmaps, tmap_next;
     unsigned warned_store_votes;     /* one warning per kernel and process */
     int host_path_default;           /* host-call path for pinned buffers: 0 = staged, 1 = hybrid, 2 = zero-copy */
-    const char* last_host_path;      /* "staged" | "hybrid" | "zerocopy" | "row-blocks" | "one-shot": what the last coast_run_host did */
+    const char* last_host_path;      /* "staged" | "hybrid" | "zerocopy" | "row-blocks" | "one-shot" | "groups": what the last coast_run_host did */
 } G;
 
 /* Single-caller guard.  The reference's emitted code is single-threaded (plain load/add/store on its counters,
@@ -331,8 +331,9 @@ int coast_init(int device) { ENTER(); LEAVE(init_impl(device)); }
 static int shutdown_impl(void) {
     if (!G.inited) return COAST_OK;
     ensure_ctx();
-    dev_buf* bufs[] = { &G.h_b, &G.slot[0].in, &G.slot[0].out, &G.slot[0].aux, &G.slot[0].stat, &G.slot[1].in, &G.slot[1].out,
-                        &G.slot[1].aux, &G.slot[1].stat, &G.slot[2].in, &G.slot[2].out, &G.slot[2].aux, &G.slot[2].stat };
+    dev_buf* bufs[] = { &G.h_b, &G.slot[0].in, &G.slot[0].out, &G.slot[0].aux, &G.slot[0].stat, &G.slot[0].rows, &G.slot[1].in,
+                        &G.slot[1].out, &G.slot[1].aux, &G.slot[1].stat, &G.slot[1].rows, &G.slot[2].in, &G.slot[2].out,
+                        &G.slot[2].aux, &G.slot[2].stat, &G.slot[2].rows };
     for (size_t i = 0; i < sizeof bufs / sizeof bufs[0]; ++i) if (bufs[i]->p) p_cuMemFree_v2(bufs[i]->p);
     for (int i = 0; i < 3; ++i) if (G.slot[i].s) p_cuStreamDestroy_v2(G.slot[i].s);
     if (G.ev_b) p_cuEventDestroy_v2(G.ev_b);
@@ -505,6 +506,11 @@ typedef struct {
     size_t scratch_per_cta;       /* plus this much per CTA of the grid, handed to the kernel as xmr_args.aux */
     int scratch_as_aux;           /* hand the scratch to the kernel as xmr_args.aux even without per-CTA scratch */
     int (*prepass)(const coast_launch_desc* d, CUdeviceptr scratch, CUstream s);
+    /* grouped matmuls: the kernel takes the row offsets and the group block (at grp_off in scratch) after its maps; the scan
+     * pre-pass cuts the products into tiles of grp_tm rows, grp_tiles_n per tile row (grp_tm 0: no scan, the plain kernel) */
+    int grouped;
+    size_t grp_off;
+    unsigned grp_tm, grp_tiles_n;
 } launch_plan;
 
 /* The TMA-ring kernels: tiles of tile_rows units of row_bytes each, loaded as equal boxes of at most 256 rows.  With a row
@@ -573,6 +579,52 @@ static int prepass_split_limbs(const coast_launch_desc* d, CUdeviceptr pa, CUstr
     return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
 }
 
+/* Grouped matmuls (COAST_MM_GROUPED): the checks shared by coast_launch and coast_run_host.  M is the product count G, the
+ * stacked A and C are one R-row matrix from row ro[0] (R = n_units / N), B is G matrices end to end. */
+static int grouped_check(const coast_launch_desc* d) {
+    if (d->kernel != COAST_K_MM_U32 && d->kernel != COAST_K_GEMM_TF32)
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: grouped products exist for MM_U32 and GEMM_TF32 only (kernel %u)", d->kernel);
+    if (d->mode & (COAST_MM_BATCHED | COAST_UNIT_OFFSETS))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: cannot be combined with COAST_MM_BATCHED or COAST_UNIT_OFFSETS");
+    if (!d->M || d->M > XMR_MM_GRP_MAX)
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: M is the product count G, 1..%u (got %u)", XMR_MM_GRP_MAX, d->M);
+    if (!d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: N and K are shared by every product and must be nonzero");
+    if (d->n_units % d->N)
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: n_units must be a multiple of N = %u (R rows x N; got %llu)", d->N,
+                    (unsigned long long)d->n_units);
+    if (d->n_units / d->N >= (1ull << 31) || (uint64_t)d->M * d->N >= (1ull << 31))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the rows R and G*N must be below 2^31 (R %llu, G %u, N %u)",
+                    (unsigned long long)(d->n_units / d->N), d->M, d->N);
+    if (!d->d_rows || (((uintptr_t)d->d_rows) & 7u))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: d_rows must point to G + 1 8-byte aligned uint64_t row offsets");
+    return COAST_OK;
+}
+/* The limb kernel's pre-pass for groups: the R rows of A from row ro[0], then every product's B (as a batch). */
+static int prepass_split_limbs_grouped(const coast_launch_desc* d, CUdeviceptr pa, CUstream s) {
+    unsigned long long rows = d->n_units / d->N, K = d->K; const void* A = d->d_in; const void* ro = d->d_rows;
+    void* params_a[] = { &ro, &A, &pa, &rows, &K };
+    int rc = launch_small("xmr_mm_grp_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_a, s); if (rc) return rc;
+    CUdeviceptr pb = pa + (size_t)rows * d->K * 4u;
+    unsigned int k32 = d->K, n32 = d->N, nb = d->M; const void* B = d->d_aux;
+    void* params_b[] = { &B, &pb, &k32, &n32, &nb };
+    return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
+}
+static int prepass_transpose_b_grouped(const coast_launch_desc* d, CUdeviceptr bt, CUstream s) {
+    const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N, nb = d->M;
+    void* params[] = { &B, &bt, &k32, &n32, &nb };
+    return launch_small("xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
+}
+/* tile_start of the products (xmr_mm_group_scan, one CTA) into the group block; for TF32 (a_map) it also rebases the host's A map
+ * onto row ro[0] of d_in with R rows, so no host-side read of the device table is needed */
+static int prepass_group_scan(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr grp, const CUtensorMap* a_map, CUstream s) {
+    const void* ro = d->d_rows; const void* base = d->d_in;
+    unsigned int n_grp = d->M, R = (unsigned)(d->n_units / d->N), tm = L->grp_tm, tn = L->grp_tiles_n;
+    unsigned int row_bytes = a_map ? d->K * 4u : 0u;
+    CUtensorMap none; memset(&none, 0, sizeof none);
+    void* params[] = { &ro, &n_grp, &R, &tm, &tn, &grp, &base, &row_bytes, (void*)(a_map ? a_map : &none) };
+    return launch_small("xmr_mm_group_scan", 1, XMR_MM_GRP_SCAN_THREADS, params, s);
+}
+
 /* Ragged batches (COAST_UNIT_OFFSETS): the bound on every length, and the checks shared by coast_launch and coast_run_host. */
 static uint32_t ragged_bound_max(uint32_t kernel) {
     return kernel == COAST_K_CRC16 ? 255u : kernel == COAST_K_QSORT ? 4096u : (1u << 28);
@@ -629,8 +681,14 @@ static int run_plan(const launch_plan* L, const coast_launch_desc* d, xmr_args* 
     CUtensorMap maps[2];
     rc = L->prepass ? L->prepass(d, scratch, stream) : COAST_OK;
     for (int i = 0; i < L->n_maps && !rc; ++i) rc = encode_map(&L->map[i], scratch, L->cache_maps, &maps[i]);
+    /* grouped: the tile table (and TF32's rebased A map) after the other pre-passes; the kernel takes ro and the group block */
+    const void* ro = d->d_rows;
+    CUdeviceptr grp = scratch + L->grp_off;
+    if (!rc && L->grouped && L->grp_tm)
+        rc = prepass_group_scan(L, d, grp, d->kernel == COAST_K_GEMM_TF32 ? &maps[0] : NULL, stream);
     if (!rc) {
-        void* params[3] = { a, &maps[0], &maps[1] };
+        void* params[5] = { a, &maps[0], &maps[1], &ro, &grp };
+        if (L->grouped && !L->n_maps) { params[1] = &ro; params[2] = &grp; }
         if (d->flags & COAST_F_VERBOSE)
             fprintf(stderr, "coast_rt: %s grid=%u block=%u smem=%u units=%llu\n", L->name, grid, L->block, L->smem,
                     (unsigned long long)d->n_units);
@@ -650,6 +708,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     if (ragged && (rc = ragged_check(d))) return rc;
     const int batched = (d->mode & COAST_MM_BATCHED) != 0;
     if (batched && (rc = batched_check(d))) return rc;
+    const int grouped = (d->mode & COAST_MM_GROUPED) != 0;
+    if (grouped && (rc = grouped_check(d))) return rc;
     if (d->n_units == 0) return COAST_OK;
     if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null device buffer");
     const uint32_t nc = d->num_clones;
@@ -663,7 +723,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     a.status = (unsigned char*)d->d_status;
     /* the kernels find a batch from n_units / N (rows of the stacked problem) and a.M (rows per product): a batch of one is
      * an unbatched launch, argument block included */
-    a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~COAST_MM_BATCHED;
+    a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~(COAST_MM_BATCHED | COAST_MM_GROUPED);
     a.M = d->M; a.N = d->N; a.K = d->K;
     memcpy(a.key, d->key, 16);
     if (inj) {
@@ -747,7 +807,34 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     }
     case COAST_K_MM_U32: {
         if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "MM needs A (d_in), B (d_aux) and M,N,K");
-        if (!batched && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "MM: n_units must be M*N");
+        if (!batched && !grouped && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "MM: n_units must be M*N");
+        if (grouped) {                                       /* the shape rules are N's and K's; every product's rows are free */
+            const char* gpath = getenv("COAST_MM_PATH");
+            const int galigned = aligned16 && !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u);
+            const uint64_t R = d->n_units / d->N;
+            L.grouped = 1;
+            snprintf(L.name, sizeof L.name, "xmr_mm_u32_grp_inj%d_nc%u", inj, nc);
+            if (store_votes || !galigned) break;
+            if ((!gpath || !strcmp(gpath, "tc")) && d->N % xmr_mmtc_bn(1) == 0 && d->K % XMR_MMTC_BK == 0) {
+                const unsigned bn = xmr_mmtc_bn(nc);
+                snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_grp_inj%d_nc%u", inj, nc);
+                L.block = XMR_WG_THREADS; L.smem = xmr_mmtc_smem(nc);
+                L.ctas = (R / XMR_WG_BM + d->M) * (d->N / bn); L.waves = 1;       /* a bound on the tiles; persistent CTAs */
+                L.grp_off = ((size_t)R * d->K + (size_t)d->M * d->K * d->N) * 4u;   /* after the limb planes */
+                L.scratch = L.grp_off + (size_t)xmr_mm_grp_bytes(d->M);
+                L.prepass = prepass_split_limbs_grouped; L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / bn;
+                L.n_maps = 2;
+                plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, (uint32_t)R, 4, XMR_WG_BM);
+                plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)R * d->K * 4u, 1, d->K, d->M * d->N, 4, bn);
+            } else if (!(gpath && !strcmp(gpath, "naive")) && d->N % XMR_MMT_BN == 0 && d->K % XMR_MMT_BK == 0) {
+                snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_grp_inj%d_nc%u", inj, nc);
+                L.block = xmr_mmt_threads(nc); L.smem = XMR_MMT_SMEM;
+                L.ctas = (R / XMR_MMT_BM + d->M) * (d->N / XMR_MMT_BN); L.waves = 0;   /* a bound on the tiles: surplus CTAs exit */
+                L.scratch = (size_t)xmr_mm_grp_bytes(d->M);
+                L.grp_tm = XMR_MMT_BM; L.grp_tiles_n = d->N / XMR_MMT_BN;
+            }
+            break;
+        }
         /* the plain kernel (one lane per replica per element) takes any shape and the per-k votes on `sum`; tile-aligned problems
          * go to the tensor cores (exact, u8 limbs on wgmma) or the register-tiled kernel; COAST_MM_PATH=tc|tiled|naive overrides.
          * The shape rules are those of one product; a batch stacks the products' rows (no tile straddles two of them). */
@@ -809,19 +896,24 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     }
     case COAST_K_GEMM_TF32: {
         if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "GEMM needs A (d_in), B (d_aux) and M,N,K");
-        if (!batched && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "GEMM: n_units must be M*N");
-        if (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % XMR_GEMM_BK)
+        if (!batched && !grouped && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "GEMM: n_units must be M*N");
+        if (grouped && (d->N % xmr_gemm_bn(0) || d->K % XMR_GEMM_BK))
+            return fail(COAST_ERR_UNSUPPORTED, "GEMM_TF32 grouped tiles are 128 x 128 x 32: N must be a multiple of 128 and K of 32 "
+                                               "(got %u, %u); the products' rows are free", d->N, d->K);
+        if (!grouped && (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % XMR_GEMM_BK))
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_TF32 tiles are 128x128x32: M,N must be multiples of 128 and K of 32 (got %u,%u,%u)", d->M, d->N, d->K);
         if (!aligned16 || (((uintptr_t)d->d_aux) & 15u) || (((uintptr_t)d->d_out) & 15u)) return fail(COAST_ERR_BAD_ARG, "GEMM buffers must be 16-byte aligned");
         /* xmr_gemm_tf32.cuh: unprotected 128 x 256 tiles when N allows (wide), else 128 x 128.  CTA-pair kernels (cluster 2 x 1 x 1,
          * 256-row pair tiles, B multicast) are bit-identical to the single-CTA kernels.  Default: pairs for the unprotected and
          * DWC kernels when the shape allows, the single-CTA kernel for TMR; COAST_GEMM_PAIR=0 / 1 forces one or the other.
          * A batch stacks its products' rows: a pair tile needs the rows of ONE product, so M (per product) % 256 == 0. */
-        const int wide = nc == 1 && d->N % xmr_gemm_bn(1) == 0;
+        const int wide = !grouped && nc == 1 && d->N % xmr_gemm_bn(1) == 0;          /* grouped: 128 x 128 tiles */
         const char* e = getenv("COAST_GEMM_PAIR");
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
-        const int pair = want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
-        if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32p_nc%u_inj%d", nc, inj);
+        const int pair = !grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
+        if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32n_grp_inj%d_nc1", inj);
+        else if (grouped) snprintf(L.name, sizeof L.name, nc == 2 ? "xmr_gemm_tf32_grp_inj%d_nc2" : "xmr_gemm_tf32_grp_inj%d_nc3", inj);
+        else if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32p_nc%u_inj%d", nc, inj);
         else if (nc == 1 && !wide) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32n_nc1_inj%d", inj);
         else snprintf(L.name, sizeof L.name, "xmr_gemm_tf32_nc%u_inj%d", nc, inj);
         { const char* g = getenv("COAST_GEMM_GROUP_M");
@@ -837,6 +929,19 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         L.scratch = (size_t)batch * d->K * d->N * 4u;                          /* B^T of every product */
         L.prepass = prepass_transpose_b;
         L.n_maps = 2;
+        if (grouped) {
+            /* 128 x 128 tiles of every product on single CTAs (no pairs, no wide tiles); A's map is encoded here over 128 rows of the B^T
+             * scratch and rebased by the scan onto row ro[0] of d_in with R rows (the host does not read the device table) */
+            const uint64_t R = d->n_units / d->N;
+            L.grouped = 1;
+            L.ctas = (R / XMR_WG_BM + d->M) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = 1;
+            L.grp_off = (size_t)d->M * d->K * d->N * 4u;                           /* after B^T of every product */
+            L.scratch = L.grp_off + (size_t)xmr_mm_grp_bytes(d->M);
+            L.prepass = prepass_transpose_b_grouped; L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / xmr_gemm_bn(wide);
+            plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, XMR_WG_BM, 1, XMR_WG_BM);
+            plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, d->M * d->N, 1, xmr_gemm_b_box(0));
+            break;
+        }
         plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uintptr_t)d->d_in, 0, d->K, (uint32_t)rows, 1, XMR_WG_BM);
         plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, (uint32_t)(batch * d->N), 1, xmr_gemm_b_box(pair));
         break;
@@ -1026,7 +1131,7 @@ static int drain_host_streams(int rc) {
 typedef struct { uint64_t off, len; } byte_range;           /* bytes [off, off + len) of one of the caller's buffers */
 typedef struct {
     uint64_t items;                                          /* items the chunk takes */
-    byte_range in, aux, out, stat;                           /* of d_in, d_aux, d_out and d_status */
+    byte_range in, aux, out, stat, rows;                     /* of d_in, d_aux, d_out, d_status and d_rows */
     uint64_t n_units, unit_base;                             /* of the chunk's launch; unit_base is added to the call's */
     uint32_t M;                                              /* rows of a matmul row block (0: the call's M) */
     uint64_t in_bias, out_bias;                              /* the launch's d_in / d_out are the slot's buffers minus these */
@@ -1099,6 +1204,25 @@ static void next_products(const host_sched* s, uint64_t done, uint64_t* budget, 
     item_chunk(s, done, left < s->max_items ? left : s->max_items, c);
 }
 
+/* Grouped matmuls (COAST_MM_GROUPED, d_rows = the caller's host row offsets ro[]): a chunk is the longest run of whole products
+ * whose A rows, B matrices, C rows and offsets fit COAST_HOST_CHUNK_BYTES; a larger product is a chunk of its own.  The chunk
+ * uploads its offset slice ro[first .. end] unchanged and launches with the slots' addresses minus ro[first] rows as d_in and
+ * d_out (exact under u64 wraparound, as next_ragged), so the caller's offsets are never rewritten. */
+static void next_groups(const host_sched* s, uint64_t first, uint64_t* budget, host_chunk* c) {
+    const uint64_t* ro = (const uint64_t*)s->d->d_rows;
+    const uint64_t K = s->d->K, N = s->d->N;
+    uint64_t e = first + 1;
+    while (e < s->total && (ro[e + 1] - ro[first]) * (K + N) * 4u + (e + 1 - first) * (K * N * 4u + 8u) + 8u <= *budget) ++e;
+    memset(c, 0, sizeof *c);
+    const uint64_t rows = ro[e] - ro[first];
+    c->items = e - first; c->M = (uint32_t)(e - first);
+    c->n_units = rows * N; c->unit_base = (ro[first] - ro[0]) * N;
+    c->in = (byte_range){ ro[first] * K * 4u, rows * K * 4u }; c->in_bias = ro[first] * K * 4u;
+    c->aux = (byte_range){ first * K * N * 4u, (e - first) * K * N * 4u };
+    c->out = (byte_range){ ro[first] * N * 4u, rows * N * 4u }; c->out_bias = ro[first] * N * 4u;
+    c->rows = (byte_range){ first * 8u, (e - first + 1) * 8u };
+}
+
 /* Matmul row blocks: max_items rows of A up and of C down per chunk; B is the schedule's shared operand. */
 static void next_row_block(const host_sched* s, uint64_t done, uint64_t* budget, host_chunk* c) {
     next_products(s, done, budget, c);
@@ -1111,13 +1235,14 @@ static void grow(uint64_t* need, uint64_t len) { if (len > *need) *need = len; }
  * reserved before the first copy, so a failed allocation never leaves a partly written output -- and once to run. */
 static int run_chunks(const host_sched* s, coast_stats* out, int* dwc_fired) {
     const coast_launch_desc* d = s->d;
-    struct { uint64_t in, aux, out, stat; } need[3];
+    struct { uint64_t in, aux, out, stat, rows; } need[3];
     memset(need, 0, sizeof need);
     uint64_t n_chunks = 0;
     for (uint64_t done = 0, budget = s->budget; done < s->total; ++n_chunks) {
         host_chunk c; s->next(s, done, &budget, &c);
         const int i = (int)(n_chunks % 3);
         grow(&need[i].in, c.in.len); grow(&need[i].aux, c.aux.len); grow(&need[i].out, c.out.len); grow(&need[i].stat, c.stat.len);
+        grow(&need[i].rows, c.rows.len);
         done += c.items;
     }
     int rc;
@@ -1128,6 +1253,7 @@ static int run_chunks(const host_sched* s, coast_stats* out, int* dwc_fired) {
         if ((rc = slot_reserve(&sl->out.p, &sl->out.cap, s->qs ? in : need[i].out))) return rc;   /* quicksort: in's twin */
         if ((rc = slot_reserve(&sl->aux.p, &sl->aux.cap, need[i].aux))) return rc;
         if (d->d_status && (rc = slot_reserve(&sl->stat.p, &sl->stat.cap, need[i].stat))) return rc;
+        if (need[i].rows && (rc = slot_reserve(&sl->rows.p, &sl->rows.cap, need[i].rows))) return rc;
     }
     if (s->shared_b) {
         if ((rc = slot_reserve(&G.h_b.p, &G.h_b.cap, s->shared_b))) return rc;
@@ -1148,6 +1274,10 @@ static int run_chunks(const host_sched* s, coast_stats* out, int* dwc_fired) {
         if (k.aux.len) {
             STEP(p_cuMemcpyHtoDAsync_v2(sl->aux.p, (const uint8_t*)d->d_aux + k.aux.off, (size_t)k.aux.len, sl->s));
             c.d_aux = (const void*)sl->aux.p;
+        }
+        if (k.rows.len) {
+            STEP(p_cuMemcpyHtoDAsync_v2(sl->rows.p, (const uint8_t*)d->d_rows + k.rows.off, (size_t)k.rows.len, sl->s));
+            c.d_rows = (const void*)sl->rows.p;
         }
         if (s->shared_b) {                                   /* B follows the first chunk's input, on stream 1 */
             if (i == 0) {
@@ -1212,6 +1342,21 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
         return run_chunks(&s, out, dwc_fired);
     }
     if ((d->mode & COAST_MM_BATCHED) && (rc = batched_check(d))) return rc;
+    if (d->mode & COAST_MM_GROUPED) {                        /* whole products per chunk, the offsets checked first */
+        if ((rc = grouped_check(d))) return rc;
+        if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");
+        const uint64_t* ro = (const uint64_t*)d->d_rows, R = d->n_units / d->N;
+        for (uint32_t g = 0; g < d->M; ++g)
+            if (ro[g + 1] < ro[g])
+                return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: product %u runs from row %llu to %llu; row offsets must not decrease",
+                            g, (unsigned long long)ro[g], (unsigned long long)ro[g + 1]);
+        if (ro[d->M] - ro[0] != R)
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the products hold %llu rows but n_units / N is %llu",
+                        (unsigned long long)(ro[d->M] - ro[0]), (unsigned long long)R);
+        if (R && (!d->d_in || !d->d_out || !d->d_aux)) return fail(COAST_ERR_BAD_ARG, "null host buffer");
+        s.next = next_groups; s.total = d->M; s.max_bytes = chunk_bytes; s.budget = chunk_bytes; s.min_in = 16; s.path = "groups";
+        return run_chunks(&s, out, dwc_fired);
+    }
     if (d->kernel == COAST_K_MM_U32 || d->kernel == COAST_K_GEMM_TF32) {
         if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");
         const uint64_t ab = (uint64_t)d->M * d->K * 4u, bb = (uint64_t)d->K * d->N * 4u, cb = (uint64_t)d->M * d->N * 4u;

@@ -24,6 +24,7 @@
 // Every element sees the same wgmma sequence as in the single-CTA kernel, so the outputs are bit-identical.
 #pragma once
 #include "xmr_common.cuh"
+#include "xmr_mm_grp.cuh"
 
 namespace xmr {
 namespace gemm {
@@ -148,12 +149,13 @@ __device__ __forceinline__ void wgmma_u8_m64n64k32(uint32_t (&d)[32], uint64_t d
 
 // Epilogue of one consumer thread: vote the NC accumulators of its fragment element by element with the reference's select
 // voter / `fcmp oeq`, count, ONE store of the voted value.  Columns [n0 + 128 sub, ...) for sub < nsub_t.
-template <int NC, int NSUB, bool INJECT>
+// GROUPED: C starts at row ro[0] (c_grp) and rows from row_end on belong to the next product: no vote, tally, flip or store.
+template <int NC, int NSUB, bool INJECT, bool GROUPED = false>
 __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float (&acc)[NC][NSUB][64], uint32_t row0, uint32_t n0, uint32_t nsub_t,
-                                         bool hints, uint64_t pol_c) {
+                                         bool hints, uint64_t pol_c, float* c_grp = nullptr, uint32_t row_end = 0) {
     const uint32_t flags = a.flags;
     const bool majority = flags & COAST_F_MAJORITY_VOTER;
-    float* C = static_cast<float*>(a.out);
+    float* C = GROUPED ? c_grp : static_cast<float*>(a.out);
     const uint32_t lane = threadIdx.x & 31;
 #pragma unroll
     for (int sub = 0; sub < NSUB; ++sub) {
@@ -163,6 +165,7 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float 
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const uint32_t row = row0 + 8 * h, col = n0 + sub * WG_N + 8 * j + 2 * (lane & 3);
+                if constexpr (GROUPED) { if (row >= row_end) continue; }
                 const unsigned long long local0 = (unsigned long long)row * a.N + col;
                 uint32_t o[2];
 #pragma unroll
@@ -200,8 +203,12 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float 
 
 // PAIR: the CTA pair of a cluster 2 x 1 x 1 computes a 256 x BN tile, rank r the rows [128 r, 128 r + 128); each rank loads half
 // of the tile's B^T rows and multicasts them to both, so a stage is released only when the consumers of BOTH CTAs are done with it.
-template <int NC, bool INJECT, bool WIDE, bool PAIR>
-__device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b) {
+// GROUPED (single CTAs with 128 x 128 tiles, xmr_mm_grp.cuh): a.M products of their own row counts, `ro` their row offsets and
+// `grp` the group block: the tiles come from its tile_start table, A through its rebased map, B^T rows from g N.
+template <int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false>
+__device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b,
+                                          const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr) {
+    static_assert(!(GROUPED && (PAIR || WIDE)), "grouped launches run on single CTAs with 128 x 128 tiles");
     using G = Geom<NC, WIDE>;
     constexpr int BN = G::BN, NSUB = G::NSUB, STAGES = G::STAGES;
     constexpr uint32_t B_STAGE = G::B_STAGE;
@@ -219,7 +226,13 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
     const uint32_t worker = blockIdx.x / CTAS, n_workers = gridDim.x / CTAS;
     const uint32_t TM = BM * CTAS;                              // rows of a (pair) tile
     // a batch stacks its products' rows (n_units / N of them, a.M per product); the host keeps every tile inside one product
-    const uint32_t tiles_n = a.N / BN, tiles_m = (uint32_t)(a.n_units / a.N) / TM, n_tiles = tiles_m * tiles_n, kblocks = a.K / BK;
+    const uint32_t tiles_n = a.N / BN, tiles_m = (uint32_t)(a.n_units / a.N) / TM, kblocks = a.K / BK;
+    // grouped: R = n_units / N rows from row ro[0] of d_in / d_out, a.M products
+    const uint32_t R = GROUPED ? (uint32_t)(a.n_units / a.N) : 0u, n_grp = GROUPED ? a.M : 0u;
+    const uint32_t* ts = GROUPED ? reinterpret_cast<const uint32_t*>(grp + XMR_MM_GRP_TILES) : nullptr;
+    const unsigned long long ro0 = GROUPED ? __ldg(ro) : 0ull;
+    const uint32_t n_tiles = GROUPED ? __ldg(ts + n_grp) * tiles_n : tiles_m * tiles_n;
+    if constexpr (GROUPED) map_a = reinterpret_cast<const CUtensorMap*>(grp);
     const uint32_t gm1 = (a.mode & XMR_MODE_GROUP_M_MASK) ? (a.mode & XMR_MODE_GROUP_M_MASK) : GROUP_M_DEFAULT;
     const uint32_t group_m = PAIR ? (gm1 > 1u ? gm1 / 2u : 1u) : gm1;   // pair tiles are 256 rows: half as many tile-rows per group
     const bool hints = (a.mode & XMR_MODE_L2_HINTS) != 0;
@@ -240,6 +253,8 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
     };
 
     if (threadIdx.x == 0) {
+        // the rebased A map was written by the pre-pass through the generic proxy
+        if constexpr (GROUPED) asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(map_a) : "memory");
         tma_prefetch_desc(map_a); tma_prefetch_desc(map_b);
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2u * CTAS); }   // 2 consumer warpgroups per CTA
         fence_barrier_init();
@@ -256,9 +271,17 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
             const uint64_t pol_a = hints ? l2_policy_evict_last() : l2_policy_normal(), pol_b = hints ? l2_policy_evict_first() : l2_policy_normal();
             for (uint32_t tile = worker; tile < n_virtual; tile += n_workers) {
                 uint32_t tm, n_off, bn_t;
-                decode(tile, tm, n_off, bn_t);
-                const int m0 = (int)(tm * TM + rank * BM);
-                const uint32_t nb = (tm * TM) / a.M * a.N;          // first B^T row of the tile's product (stacked B^T)
+                int m0;
+                uint32_t nb;
+                if constexpr (GROUPED) {
+                    // rows past the product read the next product's rows (masked in the epilogue), or zeros past R
+                    const grp::Tile x = grp::tile_of(ro, ro0, R, ts, n_grp, tiles_n, group_m, tile);
+                    m0 = (int)(x.start + x.tm * TM); nb = x.g * a.N; n_off = x.tn * BN; bn_t = BN;
+                } else {
+                    decode(tile, tm, n_off, bn_t);
+                    m0 = (int)(tm * TM + rank * BM);
+                    nb = (tm * TM) / a.M * a.N;                     // first B^T row of the tile's product (stacked B^T)
+                }
                 const uint32_t rows_b = bn_t / CTAS;                // B^T rows this CTA loads (for both CTAs of a pair)
                 for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
                     const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
@@ -284,7 +307,8 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
         uint32_t it = 0;
         for (uint32_t tile = worker; tile < n_virtual; tile += n_workers) {
             uint32_t tm, n0, bn_t;
-            decode(tile, tm, n0, bn_t);
+            if constexpr (GROUPED) bn_t = BN;                   // grouped: the tile's place is found after the main loop
+            else decode(tile, tm, n0, bn_t);
             const uint32_t nsub_t = bn_t / WG_N;
 #pragma unroll
             for (int r = 0; r < NC; ++r)
@@ -326,8 +350,16 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
                     for (int sub = 0; sub < NSUB; ++sub) wg_fence_regs(acc[r][sub]);
                 if (t == 0) for (uint32_t c = 0; c < CTAS; ++c) mbar_arrive_rank(&empty[s], c);
             }
-            const uint32_t row0 = tm * TM + rank * BM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
-            epilogue<NC, NSUB, INJECT>(a, tally, acc, row0, n0, nsub_t, hints, pol_c);
+            if constexpr (GROUPED) {
+                // found here rather than before the main loop: nothing of it stays live next to the accumulators
+                const unsigned long long r0 = __ldg(ro);
+                const grp::Tile x = grp::tile_of(ro, r0, R, ts, n_grp, tiles_n, group_m, tile);
+                const uint32_t row0 = x.start + x.tm * TM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
+                epilogue<NC, NSUB, INJECT, true>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c, static_cast<float*>(a.out) + r0 * a.N, x.end);
+            } else {
+                const uint32_t row0 = tm * TM + rank * BM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
+                epilogue<NC, NSUB, INJECT>(a, tally, acc, row0, n0, nsub_t, hints, pol_c);
+            }
         }
         tally.flush(a.counters);
     }
@@ -379,3 +411,18 @@ XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc3_inj0, 3, 0, false, true, XMR_PAIR_CLUSTER)
 XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc1_inj1, 1, 1, true, true, XMR_PAIR_CLUSTER)
 XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc2_inj1, 2, 1, false, true, XMR_PAIR_CLUSTER)
 XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc3_inj1, 3, 1, false, true, XMR_PAIR_CLUSTER)
+
+// grouped (COAST_MM_GROUPED): single CTAs and 128 x 128 tiles (tf32n unprotected); `ro` = the caller's row offsets, `grp` = the
+// group block the pre-pass wrote (xmr_mm_grp.cuh)
+#define XMR_GEMM_GRP_KERNEL(NAME, NC, INJ, WIDE)                                                           \
+    extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
+    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, \
+         const unsigned long long* ro, const uint8_t* grp) {                                             \
+        xmr::gemm::gemm_body<NC, INJ != 0, WIDE, false, true>(a, &map_a, &map_b, ro, grp);               \
+    }
+XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32_grp_inj0_nc2, 2, 0, false)
+XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32_grp_inj0_nc3, 3, 0, false)
+XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32_grp_inj1_nc2, 2, 1, false)
+XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32_grp_inj1_nc3, 3, 1, false)
+XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32n_grp_inj0_nc1, 1, 0, false)
+XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32n_grp_inj1_nc1, 1, 1, false)

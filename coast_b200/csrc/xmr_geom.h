@@ -118,4 +118,11 @@ XMR_GEOM_FN unsigned xmr_mmtc_smem(unsigned nc) {
 XMR_GEOM_FN unsigned long long xmr_ragged_scratch(unsigned long long n_units) { return XMR_RAGGED_PERM + 4ull * n_units; }
 XMR_GEOM_FN unsigned long long xmr_ragged_slots(unsigned long long n_units) { return (xmr_ragged_scratch(n_units) + 127ull) & ~127ull; }
 
+/* ---- grouped matmuls (COAST_MM_GROUPED, xmr_mm_grp.cuh): a group block in scratch = the rebased TF32 A tensor map (128 bytes),
+ * then tile_start[G + 1] (u32), written by a one-CTA scan; at most XMR_MM_GRP_MAX groups per launch ---- */
+#define XMR_MM_GRP_SCAN_THREADS 1024
+#define XMR_MM_GRP_TILES        128u
+#define XMR_MM_GRP_MAX          (1u << 20)
+XMR_GEOM_FN unsigned long long xmr_mm_grp_bytes(unsigned long long groups) { return XMR_MM_GRP_TILES + 4ull * (groups + 1ull); }
+
 #endif

@@ -37,8 +37,11 @@ template <int BN> __device__ __forceinline__ void wgmma_u8(uint32_t (&d)[BN / 2]
 template <> __device__ __forceinline__ void wgmma_u8<32>(uint32_t (&d)[16], uint64_t da, uint64_t db) { wgmma_u8_m64n32k32(d, da, db); }
 template <> __device__ __forceinline__ void wgmma_u8<64>(uint32_t (&d)[32], uint64_t da, uint64_t db) { wgmma_u8_m64n64k32(d, da, db); }
 
-template <int NC, bool INJECT>
-__device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b) {
+// GROUPED (xmr_mm_grp.cuh): a.M products of their own row counts; the A planes hold the R rows from ro[0] (xmr_mm_grp_split_a),
+// the B^T planes the G products' B; tiles come from the group block's tile_start and rows past a product are masked.
+template <int NC, bool INJECT, bool GROUPED = false>
+__device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b,
+                                     const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr) {
     using G = Geom<NC>;
     constexpr int BN = G::BN, STAGES_ = G::STAGES_, R = BN / 2;
     extern __shared__ uint8_t smem_dyn[];
@@ -50,7 +53,11 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
     uint64_t* empty = bars + STAGES_;
 
     // a batch stacks its products' rows (n_units / N of them, a.M per product; no tile straddles two products)
-    const uint32_t tiles_n = a.N / BN, tiles_m = (uint32_t)(a.n_units / a.N) / TBM, n_tiles = tiles_m * tiles_n, kblocks = a.K / TBK;
+    const uint32_t tiles_n = a.N / BN, tiles_m = (uint32_t)(a.n_units / a.N) / TBM, kblocks = a.K / TBK;
+    const uint32_t n_rows = GROUPED ? (uint32_t)(a.n_units / a.N) : 0u, n_grp = GROUPED ? a.M : 0u;
+    const uint32_t* ts = GROUPED ? reinterpret_cast<const uint32_t*>(grp + XMR_MM_GRP_TILES) : nullptr;
+    const unsigned long long ro0 = GROUPED ? __ldg(ro) : 0ull;
+    const uint32_t n_tiles = GROUPED ? __ldg(ts + n_grp) * tiles_n : tiles_m * tiles_n;
     // tile order: GROUP_M tile-rows per group, column-major inside (same L2 argument as the TF32 kernel)
     auto coords = [&](uint32_t tile, uint32_t& tm, uint32_t& tn) { tile_coords(tile, tiles_m, tiles_n, GROUP_M, tm, tn); };
 
@@ -67,13 +74,20 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
         if (threadIdx.x == 0) {
             uint32_t it = 0;
             for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                uint32_t tm, tn; coords(tile, tm, tn);
-                const uint32_t nb = (tm * TBM) / a.M * a.N;     // first B^T row of the tile's product (stacked B^T planes)
+                uint32_t tm, tn, m0, nb;
+                if constexpr (GROUPED) {
+                    const grp::Tile x = grp::tile_of(ro, ro0, n_rows, ts, n_grp, tiles_n, GROUP_M, tile);
+                    tn = x.tn; m0 = x.start + x.tm * TBM; nb = x.g * a.N;
+                } else {
+                    coords(tile, tm, tn);
+                    m0 = tm * TBM;
+                    nb = (tm * TBM) / a.M * a.N;                // first B^T row of the tile's product (stacked B^T planes)
+                }
                 for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
                     const uint32_t s = it % STAGES_, ph = (it / STAGES_) & 1u;
                     mbar_wait_or_trap(&empty[s], ph ^ 1u);
                     mbar_arrive_expect_tx(&full[s], G::A_STAGE_B + G::B_STAGE_B);
-                    tma_load_3d(sA + s * G::A_STAGE_B, map_a, &full[s], (int)(kb * TBK), (int)(tm * TBM), 0);       // box {128 k, 128 m, 4 planes}
+                    tma_load_3d(sA + s * G::A_STAGE_B, map_a, &full[s], (int)(kb * TBK), (int)m0, 0);               // box {128 k, 128 m, 4 planes}
                     tma_load_3d(sB + s * G::B_STAGE_B, map_b, &full[s], (int)(kb * TBK), (int)(nb + tn * BN), 0);  // box {128 k, BN n, 4 planes}
                 }
             }
@@ -84,14 +98,16 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
         const uint32_t a_off = (uint32_t)(wg - 1) * 64u * 128u;
         const uint32_t flags = a.flags;
         const bool majority = flags & COAST_F_MAJORITY_VOTER;
-        uint32_t* C = static_cast<uint32_t*>(a.out);
-        const uint32_t* __restrict__ A32 = static_cast<const uint32_t*>(a.in);
+        uint32_t* C = static_cast<uint32_t*>(a.out) + (GROUPED ? ro0 * a.N : 0ull);          // grouped: from row ro[0]
+        const uint32_t* __restrict__ A32 = static_cast<const uint32_t*>(a.in) + (GROUPED ? ro0 * a.K : 0ull);
         const uint32_t* __restrict__ B32 = static_cast<const uint32_t*>(a.aux);
         Tally tally(a);
         uint32_t acc[NC][4][R];
         uint32_t it = 0;
         for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            uint32_t tm, tn; coords(tile, tm, tn);
+            uint32_t tm, tn;
+            if constexpr (GROUPED) tm = tn = 0;                 // grouped: found after the main loop, next to the accumulators
+            else coords(tile, tm, tn);
 #pragma unroll
             for (int r = 0; r < NC; ++r)
 #pragma unroll
@@ -130,12 +146,18 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
                     for (int d = 0; d < 4; ++d) wg_fence_regs(acc[r][d]);
                 if (t == 0) mbar_arrive(&empty[s]);
             }
-            const uint32_t row_base = tm * TBM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + (lane >> 2);
+            uint32_t row_start = 0, row_end = 0, g = 0;
+            if constexpr (GROUPED) {
+                const grp::Tile x = grp::tile_of(ro, ro0, n_rows, ts, n_grp, tiles_n, GROUP_M, tile);
+                tm = x.tm; tn = x.tn; row_start = x.start; row_end = x.end; g = x.g;
+            }
+            const uint32_t row_base = row_start + tm * TBM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + (lane >> 2);
 #pragma unroll
             for (int jj = 0; jj < BN / 8; ++jj) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const uint32_t row = row_base + 8u * h, col = tn * BN + 8u * jj + 2u * (lane & 3u);
+                    if constexpr (GROUPED) { if (row >= row_end) continue; }          // the next product's row: not ours
                     const unsigned long long local0 = (unsigned long long)row * a.N + col;
                     uint32_t o[2];
 #pragma unroll
@@ -150,7 +172,7 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
                             if (f.active) {
                                 tally.injected++;
                                 uint32_t part = 0;          // S_s = partial sum over k <= site, from the original u32 operands
-                                const uint32_t* Bp = B32 + (size_t)(row / a.M) * a.K * a.N;    // the element's own product's B
+                                const uint32_t* Bp = B32 + (size_t)(GROUPED ? g : row / a.M) * a.K * a.N;    // the element's own product's B
                                 for (uint32_t k = 0; k <= f.site; ++k) part += __ldg(A32 + (size_t)row * a.K + k) * __ldg(Bp + (size_t)k * a.N + col + e);
                                 const uint32_t mk = 1u << f.bit, delta = (part & mk) ? (0u - mk) : mk;
                                 if (f.replica == 0) r0 += delta; else if (f.replica == 1) r1 += delta; else r2 += delta;
@@ -179,8 +201,8 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
 
 // ---- limb-split pre-pass ---------------------------------------------------------------------------------------
 // A (u32, rows x K, row-major) -> planes[l][row][k] (u8).  One thread = 4 consecutive k of one row.
-extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
-xmr_mm_split_a(const uint32_t* __restrict__ A, uint8_t* __restrict__ planes, unsigned long long rows, unsigned long long K) {
+__device__ __forceinline__ void split_a_body(const uint32_t* __restrict__ A, uint8_t* __restrict__ planes, unsigned long long rows,
+                                             unsigned long long K) {
     const unsigned long long quads = rows * K / 4ull, stride = (unsigned long long)gridDim.x * blockDim.x;
     for (unsigned long long q = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; q < quads; q += stride) {
         const uint4 v = __ldg(reinterpret_cast<const uint4*>(A) + q);
@@ -194,6 +216,16 @@ xmr_mm_split_a(const uint32_t* __restrict__ A, uint8_t* __restrict__ planes, uns
         p[2ull * plane + q] = __byte_perm(hi, hi2, 0x5410u);       // plane 2
         p[3ull * plane + q] = __byte_perm(hi, hi2, 0x7632u);       // plane 3
     }
+}
+extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
+xmr_mm_split_a(const uint32_t* __restrict__ A, uint8_t* __restrict__ planes, unsigned long long rows, unsigned long long K) {
+    split_a_body(A, planes, rows, K);
+}
+// grouped launches: the R rows from row ro[0] of A
+extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
+xmr_mm_grp_split_a(const unsigned long long* __restrict__ ro, const uint32_t* __restrict__ A, uint8_t* __restrict__ planes,
+                   unsigned long long rows, unsigned long long K) {
+    split_a_body(A + __ldg(ro) * K, planes, rows, K);
 }
 // B (u32, batch x K x N, row-major) -> planes[l][b N + n][k] (u8, TRANSPOSED so the MMA's B operand is K-major; a batch's
 // products stacked along n).  32 x 32 tiles via smem.
@@ -229,3 +261,12 @@ xmr_mm_split_bt(const uint32_t* __restrict__ B, uint8_t* __restrict__ planes, un
     }
 XMR_MMTC_KERNEL(1, 0) XMR_MMTC_KERNEL(2, 0) XMR_MMTC_KERNEL(3, 0)
 XMR_MMTC_KERNEL(1, 1) XMR_MMTC_KERNEL(2, 1) XMR_MMTC_KERNEL(3, 1)
+// grouped (COAST_MM_GROUPED): `ro` = the caller's row offsets, `grp` = the group block the pre-pass wrote (xmr_mm_grp.cuh)
+#define XMR_MMTC_GRP_KERNEL(NC, INJ)                                                                     \
+    extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
+    xmr_mm_u32_tc_grp_inj##INJ##_nc##NC(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, \
+                                        const __grid_constant__ CUtensorMap map_b, const unsigned long long* ro, const uint8_t* grp) { \
+        xmr::mmtc::body<NC, INJ != 0, true>(a, &map_a, &map_b, ro, grp);                                 \
+    }
+XMR_MMTC_GRP_KERNEL(1, 0) XMR_MMTC_GRP_KERNEL(2, 0) XMR_MMTC_GRP_KERNEL(3, 0)
+XMR_MMTC_GRP_KERNEL(1, 1) XMR_MMTC_GRP_KERNEL(2, 1) XMR_MMTC_GRP_KERNEL(3, 1)

@@ -8,8 +8,12 @@
 // memory, replica 0 votes every element (one mm_t vote per unit) and stores the tile once.
 // Fault site s (= `sum` after k-step s) is applied exactly but lazily: a flip of bit b in the partial sum S_s changes the
 // final sum by +2^b or -2^b (mod 2^32) depending on bit b of S_s, so only faulted elements recompute a partial dot product.
+//
+// Grouped launches (COAST_MM_GROUPED, xmr_mm_grp.cuh): the grid is the host's bound on the tiles, each CTA finds its product and
+// tile from the group block's tile_start (surplus CTAs exit); A-row loads clamp into the product, rows past it are not stored.
 #pragma once
 #include "xmr_common.cuh"
+#include "xmr_mm_grp.cuh"
 
 namespace xmr {
 namespace mmt {
@@ -27,8 +31,8 @@ __device__ __forceinline__ Voted vote3(uint32_t x, uint32_t r1, uint32_t r2, int
     return v;
 }
 
-template <int NC, bool INJECT>
-__device__ __forceinline__ void body(const xmr_args& a) {
+template <int NC, bool INJECT, bool GROUPED = false>
+__device__ __forceinline__ void body(const xmr_args& a, const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr) {
     extern __shared__ __align__(16) uint32_t smem[];
     uint32_t* As = smem;                        // [2][BK][BM]   (k-major: transposed on the way in)
     uint32_t* Bs = smem + 2 * BK * BM;          // [2][BK][BN]
@@ -39,9 +43,23 @@ __device__ __forceinline__ void body(const xmr_args& a) {
     const int tx = vt & 15, ty = vt >> 4;        // micro-tile: rows {ty*4+i, 32+ty*4+i}, cols {tx*4+j, 64+tx*4+j}
     const uint32_t M = a.M, N = a.N, K = a.K;
     const uint32_t tiles_n = N / BN;
-    const uint32_t m0 = (blockIdx.x / tiles_n) * BM, n0 = (blockIdx.x % tiles_n) * BN;   // m0: row of the stacked problem (batch)
-    const uint32_t* __restrict__ A = static_cast<const uint32_t*>(a.in);
-    const uint32_t* __restrict__ B = static_cast<const uint32_t*>(a.aux) + (size_t)(m0 / M) * K * N;   // the tile's product's B
+    uint32_t m0, n0, row_end = 0u;
+    unsigned long long ro0 = 0ull, g = 0ull;
+    if constexpr (GROUPED) {                     // rows counted from ro[0]; the product's rows are [start, row_end)
+        const uint32_t* ts = reinterpret_cast<const uint32_t*>(grp + XMR_MM_GRP_TILES);
+        const uint32_t R = (uint32_t)(a.n_units / N), t = blockIdx.x;
+        ro0 = __ldg(ro);
+        if (t >= __ldg(ts + M) * tiles_n) return;                                       // a surplus CTA: the whole CTA leaves
+        const uint32_t gi = grp::search(M, t / tiles_n, [&](uint32_t x) { return __ldg(ts + x); });
+        uint32_t start; grp::rows_of(ro, ro0, R, gi, start, row_end);
+        const uint32_t lt = t - __ldg(ts + gi) * tiles_n;
+        m0 = start + (lt / tiles_n) * BM; n0 = (lt % tiles_n) * BN; g = gi;
+        if (m0 >= row_end) return;                                                       // only a malformed table gets here
+    } else {
+        m0 = (blockIdx.x / tiles_n) * BM; n0 = (blockIdx.x % tiles_n) * BN;            // m0: row of the stacked problem (batch)
+    }
+    const uint32_t* __restrict__ A = static_cast<const uint32_t*>(a.in) + ro0 * K;
+    const uint32_t* __restrict__ B = static_cast<const uint32_t*>(a.aux) + (size_t)(GROUPED ? g : m0 / M) * K * N;   // the tile's product's B
     constexpr int NT = NC * VT;
     constexpr int A_V4 = BM * BK / 4, B_V4 = BK * BN / 4;          // 256 + 512 uint4 per k-tile
     constexpr int PER = (A_V4 + B_V4 + NT - 1) / NT;
@@ -58,7 +76,8 @@ __device__ __forceinline__ void body(const xmr_args& a) {
         for (int p = 0; p < PER; ++p) {
             const int q = tid + p * NT;
             if (q < A_V4) {                       // A: row q/4 of the tile, k-quad q%4
-                pre[p] = __ldg(reinterpret_cast<const uint4*>(A + (size_t)(m0 + q / 4) * K + k0 + (q % 4) * 4));
+                const uint32_t row = GROUPED ? min(m0 + q / 4, row_end - 1u) : m0 + q / 4;   // grouped: clamped into the product
+                pre[p] = __ldg(reinterpret_cast<const uint4*>(A + (size_t)row * K + k0 + (q % 4) * 4));
             } else if (q < A_V4 + B_V4) {         // B: k-row (q-A)/32, column quad (q-A)%32
                 const int b = q - A_V4;
                 pre[p] = __ldg(reinterpret_cast<const uint4*>(B + (size_t)(k0 + b / 32) * N + n0 + (b % 32) * 4));
@@ -115,6 +134,7 @@ __device__ __forceinline__ void body(const xmr_args& a) {
         for (int e = 0; e < 64; ++e) {
             const int i = e >> 3, j = e & 7;
             const uint32_t row = row_of(i), col = col_of(j);
+            if constexpr (GROUPED) { if (row >= row_end) continue; }
             const unsigned long long local = (unsigned long long)row * N + col;
             Fault f = fault_for_unit(a, NC, local, [](uint32_t) { return 32u; });
             if (!f.active) continue;
@@ -141,10 +161,11 @@ __device__ __forceinline__ void body(const xmr_args& a) {
         __syncthreads();
     }
     if (r == 0) {
-        uint32_t* C = static_cast<uint32_t*>(a.out);
+        uint32_t* C = static_cast<uint32_t*>(a.out) + ro0 * N;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
             const uint32_t row = row_of(i);
+            if constexpr (GROUPED) { if (row >= row_end) continue; }
             uint32_t o[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -169,3 +190,11 @@ __device__ __forceinline__ void body(const xmr_args& a) {
     xmr_mm_u32_tiled_nc##NC##_inj##INJ(const __grid_constant__ xmr_args a) { xmr::mmt::body<NC, INJ != 0>(a); }
 XMR_MMT_KERNEL(1, 0) XMR_MMT_KERNEL(2, 0) XMR_MMT_KERNEL(3, 0)
 XMR_MMT_KERNEL(1, 1) XMR_MMT_KERNEL(2, 1) XMR_MMT_KERNEL(3, 1)
+// grouped (COAST_MM_GROUPED): `ro` = the caller's row offsets, `grp` = the group block the pre-pass wrote
+#define XMR_MMT_GRP_KERNEL(NC, INJ)                                                                      \
+    extern "C" __global__ void __launch_bounds__(xmr_mmt_threads(NC))                                    \
+    xmr_mm_u32_tiled_grp_inj##INJ##_nc##NC(const __grid_constant__ xmr_args a, const unsigned long long* ro, const uint8_t* grp) { \
+        xmr::mmt::body<NC, INJ != 0, true>(a, ro, grp);                                                  \
+    }
+XMR_MMT_GRP_KERNEL(1, 0) XMR_MMT_GRP_KERNEL(2, 0) XMR_MMT_GRP_KERNEL(3, 0)
+XMR_MMT_GRP_KERNEL(1, 1) XMR_MMT_GRP_KERNEL(2, 1) XMR_MMT_GRP_KERNEL(3, 1)

@@ -20,6 +20,7 @@ PLAN_NONE, PLAN_BERNOULLI, PLAN_TABLE = 0, 1, 2
 AES_DECRYPT, AES_KEY_PER_UNIT, AES_KEY_WRITEBACK = 1, 2, 4
 UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 / QSORT batches: aux = n_units + 1 u64 byte offsets into inp
 MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32: n_units = batch*M*N, inp / aux / out hold batch A / B / C
+MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 
@@ -46,7 +47,7 @@ class LaunchDesc(C.Structure):
                 ("n_units", C.c_uint64), ("unit_base", C.c_uint64),
                 ("unit_bytes", C.c_uint32), ("M", C.c_uint32), ("N", C.c_uint32), ("K", C.c_uint32),
                 ("d_in", C.c_void_p), ("d_out", C.c_void_p), ("d_aux", C.c_void_p),
-                ("key", C.c_uint8 * 16), ("plan", C.POINTER(_Plan)), ("d_status", C.c_void_p)]
+                ("key", C.c_uint8 * 16), ("plan", C.POINTER(_Plan)), ("d_status", C.c_void_p), ("d_rows", C.c_void_p)]
 
 
 class _Stats(C.Structure):
@@ -183,7 +184,7 @@ class Runtime:
         return s.cuda_stream
 
     def make_desc(self, kernel, num_clones, d_in, d_out, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0,
-                  d_aux=None, key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, d_status=None):
+                  d_aux=None, key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, d_status=None, d_rows=None):
         d = LaunchDesc()
         d.kernel, d.num_clones, d.flags, d.mode = kernel, num_clones, flags, mode
         d.n_units, d.unit_base, d.unit_bytes = n_units, unit_base, unit_bytes
@@ -196,11 +197,13 @@ class Runtime:
             d.key = (C.c_uint8 * 16)(*key)
         if d_status is not None:
             d.d_status = d_status.data_ptr() if hasattr(d_status, "data_ptr") else d_status
+        if d_rows is not None:
+            d.d_rows = d_rows.data_ptr() if hasattr(d_rows, "data_ptr") else d_rows
         keep = None
         if plan is not None and plan.mode != PLAN_NONE:
             keep = plan.to_c()
             d.plan = C.pointer(keep)
-        d._keep = (keep, d_in, d_out, d_aux)
+        d._keep = (keep, d_in, d_out, d_aux, d_rows)
         return d
 
     def launch(self, desc: LaunchDesc, stream=None):
@@ -268,19 +271,45 @@ class Runtime:
 
     # -- convenience: device tensors in, device tensor + Stats out ----------------------------
     def run(self, kernel, num_clones, inp, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0, aux=None,
-            key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, out=None, stream=None, status=None):
+            key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, out=None, stream=None, status=None, rows=None):
+        """rows: with MM_GROUPED, the CUDA int64/uint64 tensor of M + 1 row offsets (M = the product count)"""
         torch = self.torch
+        if mode & MM_GROUPED:
+            self._check_rows(rows, M, N, n_units, inp, K, out)
         ragged_qsort = bool(mode & UNIT_OFFSETS) and kernel == K_QSORT
         if out is None and ragged_qsort:       # the arrays are sorted into the bytes they came from: out mirrors inp
             out = torch.zeros(inp.numel() * inp.element_size(), dtype=torch.uint8, device=f"cuda:{self.device}")
         if mode & UNIT_OFFSETS:
             self._check_offsets(inp, aux, n_units, unit_bytes, kernel=kernel, out=out)
+        if out is None and mode & MM_GROUPED:   # C rows at ro[g]: out covers rows [0, ro[G]), like inp
+            R_end = int(rows[: M + 1].view(torch.int64)[-1])
+            out = torch.empty(R_end * N * 4, dtype=torch.uint8, device=f"cuda:{self.device}")
         if out is None:
             out = torch.empty(n_units * out_bytes(kernel, unit_bytes), dtype=torch.uint8, device=f"cuda:{self.device}")
         d = self.make_desc(kernel, num_clones, inp, out, n_units, flags=flags, mode=mode, unit_bytes=unit_bytes,
-                           M=M, N=N, K=K, d_aux=aux, key=key, plan=plan, unit_base=unit_base, d_status=status)
+                           M=M, N=N, K=K, d_aux=aux, key=key, plan=plan, unit_base=unit_base, d_status=status, d_rows=rows)
         self.launch(d, stream)
         return out, self.sync(stream)
+
+    def _check_rows(self, rows, G, N, n_units, inp, K, out):
+        """A grouped launch's device row offsets (int64 or uint64 tensor, G + 1 entries): they never decrease and span exactly
+        n_units / N rows, which lie within inp (K per row) and out (N per row).  The kernels only clamp; this catches a bad table
+        before it runs."""
+        torch = self.torch
+        if rows is None or not hasattr(rows, "data_ptr") or rows.dtype not in (torch.int64, torch.uint64) or not rows.is_cuda:
+            raise CoastError(ERR_BAD_ARG, "MM_GROUPED: rows must be a CUDA int64/uint64 tensor of M + 1 row offsets")
+        if G < 1 or rows.numel() < G + 1 or not rows.is_contiguous():
+            raise CoastError(ERR_BAD_ARG, f"MM_GROUPED: rows holds {rows.numel()} offsets, a contiguous M + 1 = {G + 1} are needed")
+        if N < 1 or n_units % N:
+            raise CoastError(ERR_BAD_ARG, f"MM_GROUPED: n_units ({n_units}) must be a multiple of N ({N})")
+        ro = rows[: G + 1].view(torch.int64)
+        R = n_units // N
+        in_rows = inp.numel() * inp.element_size() // (4 * K) if K else 0
+        out_rows = out.numel() * out.element_size() // (4 * N) if out is not None else None
+        bad = torch.stack([(ro < 0).any(), (ro[1:] < ro[:-1]).any(), ro[-1] - ro[0] != R, ro[-1] > in_rows]).tolist()
+        if any(bad) or (out_rows is not None and int(ro[-1]) > out_rows):
+            raise CoastError(ERR_BAD_ARG, f"MM_GROUPED: row offsets must not decrease, must span n_units / N = {R} rows and end "
+                                          "within inp and out")
 
     def _check_offsets(self, inp, aux, n_units, unit_bytes, *, kernel=None, out=None):
         """A ragged batch's device offsets (int64 or uint64 tensor, n_units + 1 entries): they never decrease, no length
@@ -310,7 +339,7 @@ class Runtime:
     # -- the reference-facing host call: HOST buffers, H2D + kernel + D2H inside ---------------
     def run_host(self, kernel, num_clones, h_in, h_out, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0,
                  h_aux=None, key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0,
-                 abort_on_dwc: bool = False) -> Stats:
+                 abort_on_dwc: bool = False, h_rows=None) -> Stats:
         """h_in/h_out/h_aux: CPU torch tensors or numpy arrays (pinned memory makes the copies async)."""
         def ptr(x):
             if x is None:
@@ -318,8 +347,8 @@ class Runtime:
             return x.data_ptr() if hasattr(x, "data_ptr") else x.ctypes.data
         d = self.make_desc(kernel, num_clones, ptr(h_in), ptr(h_out), n_units, flags=flags, mode=mode,
                            unit_bytes=unit_bytes, M=M, N=N, K=K, d_aux=ptr(h_aux), key=key, plan=plan,
-                           unit_base=unit_base)
-        d._keep2 = (h_in, h_out, h_aux)
+                           unit_base=unit_base, d_rows=ptr(h_rows))
+        d._keep2 = (h_in, h_out, h_aux, h_rows)
         st = _Stats()
         fn = self.L.coast_run_host if abort_on_dwc else self.L.coast_run_host_noabort
         self._check(fn(C.byref(d), C.byref(st)))

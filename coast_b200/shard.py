@@ -20,6 +20,35 @@ def shard_range(n_units: int, rank: int, world: int) -> tuple[int, int]:
     return lo, lo + base + (1 if rank < rem else 0)
 
 
+def shard_groups(row_offsets, rank: int, world: int) -> tuple[int, int]:
+    """Whole products [g_lo, g_hi) of a grouped matmul (COAST_MM_GROUPED) for ``rank``, balanced by rows: rank r takes the
+    products whose first row falls in its share [r R / world, (r + 1) R / world) of the R rows (a product with no rows goes
+    with the next one's start).  ``row_offsets`` is the G + 1 offset table (any sequence of ints).  The shard's launch passes
+    d_rows + g_lo, d_aux + g_lo K N, M = g_hi - g_lo, n_units = (ro[g_hi] - ro[g_lo]) N and unit_base + (ro[g_lo] - ro[0]) N."""
+    if world < 1 or not (0 <= rank < world):
+        raise ValueError("bad rank/world")
+    ro = [int(x) for x in row_offsets]
+    G, R = len(ro) - 1, ro[-1] - ro[0]
+    if G < 1:
+        raise ValueError("row_offsets needs G + 1 >= 2 entries")
+
+    def cut(r):                          # first product whose first row lies at or past rank r's share
+        if r <= 0:
+            return 0
+        if r >= world:
+            return G
+        t = ro[0] + (r * R) // world
+        lo, hi = 0, G
+        while lo < hi:
+            mid = (lo + hi) // 2
+            if ro[mid] < t:
+                lo = mid + 1
+            else:
+                hi = mid
+        return lo
+    return cut(rank), cut(rank + 1)
+
+
 def stats_to_tensor(stats: dict, torch, device="cpu"):
     f = stats["first_fault_unit"]
     return torch.tensor([stats["errors_corrected"], stats["dwc_detected"], stats["syncs"], stats["injected"],

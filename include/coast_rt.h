@@ -159,6 +159,7 @@ typedef struct coast_fault_plan {
  *            from a stream-ordered pool: any number of streams), register-tiled CUDA cores when M%64 == N%128 ==
  *            K%16 == 0, a plain kernel otherwise (e.g. the 9 x 9 tests).  COAST_MM_PATH=tc|tiled|naive overrides.
  *            With COAST_MM_BATCHED: `batch` products of one shape in one launch (see below).
+ *            With COAST_MM_GROUPED: G products that share N and K, each with its own row count (see below).
  *   GEMM_TF32 same with float.
  *   QSORT    in : n_units x unit_bytes, arrays of L = unit_bytes/4 int32 (L <= 1024)   out: the sorted arrays
  *   CHSTONE_SHA in : n_units x unit_bytes stream bytes (unit_bytes a multiple of 64, 64 <= unit_bytes < 2^29)
@@ -199,6 +200,22 @@ typedef struct coast_fault_plan {
  * bit n_units must be M*N; with batch = 1 the launch is identical to an unbatched one.  A shard takes whole matrices
  * [b_lo, b_hi): the three pointers and unit_base offset as above, n_units = (b_hi - b_lo) x M x N. */
 #define COAST_MM_BATCHED        0x20000u
+/* Grouped matmuls (MM_U32 and GEMM_TF32 only): with COAST_MM_GROUPED in `mode`, M is the number of products G (at least 1) and N
+ * and K are shared by all of them.  d_rows points to G + 1 non-decreasing uint64_t row offsets ro[] (8-byte aligned; a device
+ * pointer for coast_launch, a host pointer for coast_run_host): product g has M_g = ro[g+1] - ro[g] rows (zero is allowed),
+ * its A at d_in + ro[g]*K, its B at d_aux + g*K*N and its C at d_out + ro[g]*N (elements); d_aux holds the G dense K x N
+ * matrices end to end.  n_units = R*N with R = ro[G] - ro[0] the rows of all products.  The launch equals G single launches,
+ * product g with M = M_g and unit_base + (ro[g] - ro[0])*N: the same output elements, summed counters, minimum
+ * first_fault_unit and d_status bytes (coast_launch).  Fault plans stay keyed by the global unit index (a TABLE plan has n_units
+ * entries); the sites are those of the kernel (K for MM_U32, 1 for GEMM_TF32) and the in-loop store votes keep K + 1 votes per
+ * unit.  Each path's shape rules apply to N and K only: every M_g is allowed on every path.  The kernels clamp every offset to
+ * [ro[0], ro[0] + R] and count a decreasing pair as zero rows, so a malformed table never reads or writes outside
+ * [ro[0], ro[0] + R) rows of the buffers; coast_run_host (and Runtime.run) refuse a table that decreases or whose last offset is
+ * not ro[0] + R.  COAST_ERR_BAD_ARG for the bit on any other kernel or with COAST_MM_BATCHED or COAST_UNIT_OFFSETS, for G = 0
+ * or above 2^20, for n_units not a multiple of N, for R or G*N at or above 2^31, and for a null or misaligned d_rows.  A shard
+ * takes whole products [g_lo, g_hi): d_rows + g_lo with the same d_in and d_out, d_aux + g_lo*K*N, M = g_hi - g_lo,
+ * n_units = (ro[g_hi] - ro[g_lo])*N and unit_base + (ro[g_lo] - ro[0])*N. */
+#define COAST_MM_GROUPED        0x40000u
 #define COAST_AES_DECRYPT       0x1u
 #define COAST_AES_KEY_PER_UNIT  0x2u
 #define COAST_AES_KEY_WRITEBACK 0x4u   /* with KEY_PER_UNIT: store what aes_enc_dec() leaves in key[] (TI_aes_128.c:214-221 mutates
@@ -224,6 +241,7 @@ typedef struct coast_launch_desc {
                               replicas disagreed (saturating at 255; 0 = all agreed).  This is the per-run "F:"
                               field of the board report line (decoder.py:66) for campaign tooling.  A device
                               pointer for coast_launch, a host pointer for coast_run_host (not for the matmuls). */
+    const void* d_rows;    /* COAST_MM_GROUPED only (read only with the bit): G + 1 u64 row offsets, see above */
 } coast_launch_desc;
 
 /* Counters of everything launched since the last coast_sync(). */
@@ -343,10 +361,13 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  * unit ranges, each uploads its bytes and its slice of the offsets unchanged (QSORT also downloads the same byte range to
  * d_out + off[first]); a forced zerocopy or hybrid path gives COAST_ERR_UNSUPPORTED.  Batched matmuls (COAST_MM_BATCHED) are
  * staged in chunks of whole matrices sized by COAST_HOST_CHUNK_BYTES (a matrix larger than that is a chunk of its own): each
- * chunk uploads its A and B matrices, launches with its unit_base and downloads its C matrices.  On any failure every copy already queued on
+ * chunk uploads its A and B matrices, launches with its unit_base and downloads its C matrices.  Grouped matmuls
+ * (COAST_MM_GROUPED) are staged in chunks of whole products whose A rows, B matrices, C rows and offsets fit COAST_HOST_CHUNK_BYTES
+ * (a larger product is a chunk of its own): each uploads its slice of the offsets unchanged and launches with d_in and d_out
+ * biased by ro[first] rows.  On any failure every copy already queued on
  * the caller's buffers is drained before the call returns. */
 int  coast_run_host(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
-/* What the last host call did: "staged", "hybrid" or "zerocopy"; unbatched matmuls: "row-blocks" or "one-shot". */
+/* What the last host call did: "staged", "hybrid" or "zerocopy"; unbatched matmuls: "row-blocks" or "one-shot"; grouped: "groups". */
 const char* coast_last_host_path(void);
 /* Same, but never calls FAULT_DETECTED_DWC (fault campaigns want the count, not SIGABRT). */
 int  coast_run_host_noabort(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
