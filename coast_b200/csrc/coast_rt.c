@@ -397,16 +397,19 @@ static const struct kernel_info {
     uint32_t key_bytes;                     /* per-unit key bytes with COAST_AES_KEY_PER_UNIT */
     int store_votes;                        /* in-loop store votes are built (coast_rt.h) */
     int streams_once;                       /* reads each input byte once: may read mapped host memory directly */
+    uint32_t mm_elem;                       /* the matmuls: bytes per element of A and B (C elements are out_bytes) */
 } KINFO[COAST_K_COUNT_] = {
     [COAST_K_CRC16]       = { "crc16",       2,  1,  IN_UNIT_BYTES, 0,  1, 1 },
     [COAST_K_SHA256]      = { "sha256",      32, 32, IN_UNIT_BYTES, 0,  1, 1 },
     [COAST_K_AES128]      = { "aes128",      16, 16, 16,            16, 0, 1 },
-    [COAST_K_MM_U32]      = { "mm_u32",      4,  1,  0,             0,  1, 0 },
-    [COAST_K_GEMM_TF32]   = { "gemm_tf32",   4,  1,  0,             0,  0, 0 },
+    [COAST_K_MM_U32]      = { "mm_u32",      4,  1,  0,             0,  1, 0, 4 },
+    [COAST_K_GEMM_TF32]   = { "gemm_tf32",   4,  1,  0,             0,  0, 0, 4 },
     [COAST_K_QSORT]       = { "qsort",       0,  0,  IN_UNIT_BYTES, 0,  0, 0 },
     [COAST_K_CHSTONE_SHA] = { "chstone_sha", 20, 5,  IN_UNIT_BYTES, 0,  0, 1 },
     [COAST_K_CHSTONE_AES] = { "chstone_aes", 64, 16, 64,            64, 0, 1 },
+    [COAST_K_GEMM_BF16]   = { "gemm_bf16",   4,  1,  0,             0,  0, 0, 2 },
 };
+static int is_matmul(uint32_t kernel) { return kernel < COAST_K_COUNT_ && KINFO[kernel].mm_elem != 0; }
 
 static int store_votes_wanted(uint32_t fl) {
     return (fl & (COAST_F_STORE_DATA_SYNC | COAST_F_NO_MEM_REPLICATION)) && !(fl & COAST_F_NO_STORE_DATA_SYNC);
@@ -445,6 +448,7 @@ uint32_t coast_fault_sites(uint32_t kernel, uint32_t unit_bytes, uint32_t K) {
     case COAST_K_AES128:    return 176u;
     case COAST_K_MM_U32:    return K;
     case COAST_K_GEMM_TF32: return 1u;
+    case COAST_K_GEMM_BF16: return 1u;
     case COAST_K_QSORT:     return 33u * (unit_bytes / 4u);
     case COAST_K_CHSTONE_SHA: return 421u * (unit_bytes / 64u + 1u);
     case COAST_K_CHSTONE_AES: return 176u;
@@ -529,7 +533,8 @@ static void plan_ring(launch_plan* L, xmr_args* a, unsigned tile_rows, unsigned 
     m->swz = swz; m->l2 = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
 }
 
-/* A K-major operand of the wgmma kernels, 128-byte swizzle: rows x K elements of esize bytes, in `planes` planes. */
+/* A K-major operand of the wgmma kernels, 128-byte swizzle: rows x K elements of esize bytes, in `planes` planes (or any dense
+ * row-major matrix of `rows` rows of K elements, loaded in boxes of 128 bytes x box_rows: GEMM_BF16's B). */
 static void plan_wg_map(map_desc* m, CUtensorMapDataType dtype, unsigned esize, uintptr_t base, int in_scratch, uint32_t K,
                         uint32_t rows, unsigned planes, unsigned box_rows) {
     m->dtype = dtype; m->rank = planes > 1 ? 3 : 2; m->base = base; m->in_scratch = in_scratch;
@@ -547,17 +552,19 @@ static uint64_t mm_batch(const coast_launch_desc* d) {
     return (d->mode & COAST_MM_BATCHED) ? d->n_units / ((uint64_t)d->M * d->N) : 1u;
 }
 static int batched_check(const coast_launch_desc* d) {
-    if (d->kernel != COAST_K_MM_U32 && d->kernel != COAST_K_GEMM_TF32)
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batched products exist for MM_U32 and GEMM_TF32 only (kernel %u)", d->kernel);
+    if (!is_matmul(d->kernel))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batched products exist for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", d->kernel);
     if (!d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: M, N and K are the shape of one product and must be nonzero");
     const uint64_t mn = (uint64_t)d->M * d->N;
     if (!d->n_units || d->n_units % mn)
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: n_units must be a nonzero multiple of M*N = %llu (got %llu)",
                     (unsigned long long)mn, (unsigned long long)d->n_units);
     const uint64_t batch = d->n_units / mn;
-    if (batch * d->M >= (1ull << 31) || batch * d->N >= (1ull << 31))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batch*M and batch*N must be below 2^31 (batch %llu, M %u, N %u)",
-                    (unsigned long long)batch, d->M, d->N);
+    /* the rows of the stacked operands are tensor-map coordinates: A's batch*M, and B^T's batch*N or, for GEMM_BF16 (B in place), B's batch*K */
+    const int b_rows_k = d->kernel == COAST_K_GEMM_BF16;
+    if (batch * d->M >= (1ull << 31) || batch * (b_rows_k ? d->K : d->N) >= (1ull << 31))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batch*M and batch*%c must be below 2^31 (batch %llu, M %u, %c %u)",
+                    b_rows_k ? 'K' : 'N', (unsigned long long)batch, d->M, b_rows_k ? 'K' : 'N', b_rows_k ? d->K : d->N);
     return COAST_OK;
 }
 
@@ -582,8 +589,8 @@ static int prepass_split_limbs(const coast_launch_desc* d, CUdeviceptr pa, CUstr
 /* Grouped matmuls (COAST_MM_GROUPED): the checks shared by coast_launch and coast_run_host.  M is the product count G, the
  * stacked A and C are one R-row matrix from row ro[0] (R = n_units / N), B is G matrices end to end. */
 static int grouped_check(const coast_launch_desc* d) {
-    if (d->kernel != COAST_K_MM_U32 && d->kernel != COAST_K_GEMM_TF32)
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: grouped products exist for MM_U32 and GEMM_TF32 only (kernel %u)", d->kernel);
+    if (!is_matmul(d->kernel))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: grouped products exist for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", d->kernel);
     if (d->mode & (COAST_MM_BATCHED | COAST_UNIT_OFFSETS))
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: cannot be combined with COAST_MM_BATCHED or COAST_UNIT_OFFSETS");
     if (!d->M || d->M > XMR_MM_GRP_MAX)
@@ -592,9 +599,10 @@ static int grouped_check(const coast_launch_desc* d) {
     if (d->n_units % d->N)
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: n_units must be a multiple of N = %u (R rows x N; got %llu)", d->N,
                     (unsigned long long)d->n_units);
-    if (d->n_units / d->N >= (1ull << 31) || (uint64_t)d->M * d->N >= (1ull << 31))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the rows R and G*N must be below 2^31 (R %llu, G %u, N %u)",
-                    (unsigned long long)(d->n_units / d->N), d->M, d->N);
+    const int b_rows_k = d->kernel == COAST_K_GEMM_BF16;                /* as in batched_check */
+    if (d->n_units / d->N >= (1ull << 31) || (uint64_t)d->M * (b_rows_k ? d->K : d->N) >= (1ull << 31))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the rows R and G*%c must be below 2^31 (R %llu, G %u, %c %u)",
+                    b_rows_k ? 'K' : 'N', (unsigned long long)(d->n_units / d->N), d->M, b_rows_k ? 'K' : 'N', b_rows_k ? d->K : d->N);
     if (!d->d_rows || (((uintptr_t)d->d_rows) & 7u))
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: d_rows must point to G + 1 8-byte aligned uint64_t row offsets");
     return COAST_OK;
@@ -614,12 +622,12 @@ static int prepass_transpose_b_grouped(const coast_launch_desc* d, CUdeviceptr b
     void* params[] = { &B, &bt, &k32, &n32, &nb };
     return launch_small("xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
 }
-/* tile_start of the products (xmr_mm_group_scan, one CTA) into the group block; for TF32 (a_map) it also rebases the host's A map
+/* tile_start of the products (xmr_mm_group_scan, one CTA) into the group block; for TF32 and BF16 (a_map) it also rebases the host's A map
  * onto row ro[0] of d_in with R rows, so no host-side read of the device table is needed */
 static int prepass_group_scan(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr grp, const CUtensorMap* a_map, CUstream s) {
     const void* ro = d->d_rows; const void* base = d->d_in;
     unsigned int n_grp = d->M, R = (unsigned)(d->n_units / d->N), tm = L->grp_tm, tn = L->grp_tiles_n;
-    unsigned int row_bytes = a_map ? d->K * 4u : 0u;
+    unsigned int row_bytes = a_map ? d->K * KINFO[d->kernel].mm_elem : 0u;
     CUtensorMap none; memset(&none, 0, sizeof none);
     void* params[] = { &ro, &n_grp, &R, &tm, &tn, &grp, &base, &row_bytes, (void*)(a_map ? a_map : &none) };
     return launch_small("xmr_mm_group_scan", 1, XMR_MM_GRP_SCAN_THREADS, params, s);
@@ -681,11 +689,11 @@ static int run_plan(const launch_plan* L, const coast_launch_desc* d, xmr_args* 
     CUtensorMap maps[2];
     rc = L->prepass ? L->prepass(d, scratch, stream) : COAST_OK;
     for (int i = 0; i < L->n_maps && !rc; ++i) rc = encode_map(&L->map[i], scratch, L->cache_maps, &maps[i]);
-    /* grouped: the tile table (and TF32's rebased A map) after the other pre-passes; the kernel takes ro and the group block */
+    /* grouped: the tile table (and the GEMMs' rebased A map) after the other pre-passes; the kernel takes ro and the group block */
     const void* ro = d->d_rows;
     CUdeviceptr grp = scratch + L->grp_off;
     if (!rc && L->grouped && L->grp_tm)
-        rc = prepass_group_scan(L, d, grp, d->kernel == COAST_K_GEMM_TF32 ? &maps[0] : NULL, stream);
+        rc = prepass_group_scan(L, d, grp, d->kernel != COAST_K_MM_U32 ? &maps[0] : NULL, stream);
     if (!rc) {
         void* params[5] = { a, &maps[0], &maps[1], &ro, &grp };
         if (L->grouped && !L->n_maps) { params[1] = &ro; params[2] = &grp; }
@@ -894,16 +902,24 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         L.block = XMR_AES_THREADS; L.smem = xmr_aes_smem(dec);               /* the same shared-memory tables as the TI kernels */
         break;
     }
-    case COAST_K_GEMM_TF32: {
+    case COAST_K_GEMM_TF32:
+    case COAST_K_GEMM_BF16: {
+        /* one body for both operand types (xmr_gemm_tf32.cuh): fp32 operands read as TF32, B^T K-major from a transposing pre-pass
+         * into scratch; or bfloat16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch) */
+        const int bf16 = d->kernel == COAST_K_GEMM_BF16;
+        const char* TY = bf16 ? "BF16" : "TF32";
+        const unsigned es = KINFO[d->kernel].mm_elem, bk = bf16 ? XMR_GEMM_BF16_BK : XMR_GEMM_BK;
+        const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
         if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "GEMM needs A (d_in), B (d_aux) and M,N,K");
         if (!batched && !grouped && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "GEMM: n_units must be M*N");
-        if (grouped && (d->N % xmr_gemm_bn(0) || d->K % XMR_GEMM_BK))
-            return fail(COAST_ERR_UNSUPPORTED, "GEMM_TF32 grouped tiles are 128 x 128 x 32: N must be a multiple of 128 and K of 32 "
-                                               "(got %u, %u); the products' rows are free", d->N, d->K);
-        if (!grouped && (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % XMR_GEMM_BK))
-            return fail(COAST_ERR_UNSUPPORTED, "GEMM_TF32 tiles are 128x128x32: M,N must be multiples of 128 and K of 32 (got %u,%u,%u)", d->M, d->N, d->K);
+        if (grouped && (d->N % xmr_gemm_bn(0) || d->K % bk))
+            return fail(COAST_ERR_UNSUPPORTED, "GEMM_%s grouped tiles are 128 x 128 x %u: N must be a multiple of 128 and K of %u "
+                                               "(got %u, %u); the products' rows are free", TY, bk, bk, d->N, d->K);
+        if (!grouped && (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % bk))
+            return fail(COAST_ERR_UNSUPPORTED, "GEMM_%s tiles are 128x128x%u: M,N must be multiples of 128 and K of %u (got %u,%u,%u)",
+                        TY, bk, bk, d->M, d->N, d->K);
         if (!aligned16 || (((uintptr_t)d->d_aux) & 15u) || (((uintptr_t)d->d_out) & 15u)) return fail(COAST_ERR_BAD_ARG, "GEMM buffers must be 16-byte aligned");
-        /* xmr_gemm_tf32.cuh: unprotected 128 x 256 tiles when N allows (wide), else 128 x 128.  CTA-pair kernels (cluster 2 x 1 x 1,
+        /* unprotected 128 x 256 tiles when N allows (wide), else 128 x 128.  CTA-pair kernels (cluster 2 x 1 x 1,
          * 256-row pair tiles, B multicast) are bit-identical to the single-CTA kernels.  Default: pairs for the unprotected and
          * DWC kernels when the shape allows, the single-CTA kernel for TMR; COAST_GEMM_PAIR=0 / 1 forces one or the other.
          * A batch stacks its products' rows: a pair tile needs the rows of ONE product, so M (per product) % 256 == 0. */
@@ -911,7 +927,14 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         const char* e = getenv("COAST_GEMM_PAIR");
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
         const int pair = !grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
-        if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32n_grp_inj%d_nc1", inj);
+        if (bf16) {
+            if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_grp_inj%d_nc1", inj);
+            else if (grouped) snprintf(L.name, sizeof L.name, nc == 2 ? "xmr_gemm_bf16_grp_inj%d_nc2" : "xmr_gemm_bf16_grp_inj%d_nc3", inj);
+            else if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16p_inj%d_nc%u", inj, nc);
+            else if (nc == 1 && !wide) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_inj%d_nc1", inj);
+            else snprintf(L.name, sizeof L.name, "xmr_gemm_bf16_inj%d_nc%u", inj, nc);
+        }
+        else if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32n_grp_inj%d_nc1", inj);
         else if (grouped) snprintf(L.name, sizeof L.name, nc == 2 ? "xmr_gemm_tf32_grp_inj%d_nc2" : "xmr_gemm_tf32_grp_inj%d_nc3", inj);
         else if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32p_nc%u_inj%d", nc, inj);
         else if (nc == 1 && !wide) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32n_nc1_inj%d", inj);
@@ -926,24 +949,32 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         L.block = XMR_WG_THREADS; L.smem = xmr_gemm_smem(wide);
         const uint64_t batch = mm_batch(d), rows = batch * d->M;
         L.ctas = (rows / XMR_WG_BM) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = pair ? 2 : 1;
-        L.scratch = (size_t)batch * d->K * d->N * 4u;                          /* B^T of every product */
-        L.prepass = prepass_transpose_b;
+        if (!bf16) {
+            L.scratch = (size_t)batch * d->K * d->N * 4u;                      /* B^T of every product */
+            L.prepass = prepass_transpose_b;
+        }
         L.n_maps = 2;
         if (grouped) {
-            /* 128 x 128 tiles of every product on single CTAs (no pairs, no wide tiles); A's map is encoded here over 128 rows of the B^T
-             * scratch and rebased by the scan onto row ro[0] of d_in with R rows (the host does not read the device table) */
+            /* 128 x 128 tiles of every product on single CTAs (no pairs, no wide tiles); A's map is encoded here over 128 rows of a
+             * placeholder and rebased by the scan onto row ro[0] of d_in with R rows (the host does not read the device table).  The
+             * placeholder is the B^T scratch, or for BF16 (no scratch) B itself: d_in of a host-call chunk is biased by ro[first] rows
+             * and need not be an address of its own */
             const uint64_t R = d->n_units / d->N;
             L.grouped = 1;
             L.ctas = (R / XMR_WG_BM + d->M) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = 1;
-            L.grp_off = (size_t)d->M * d->K * d->N * 4u;                           /* after B^T of every product */
+            L.grp_off = bf16 ? 0 : (size_t)d->M * d->K * d->N * 4u;                /* after B^T of every product */
             L.scratch = L.grp_off + (size_t)xmr_mm_grp_bytes(d->M);
-            L.prepass = prepass_transpose_b_grouped; L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / xmr_gemm_bn(wide);
-            plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, XMR_WG_BM, 1, XMR_WG_BM);
-            plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, d->M * d->N, 1, xmr_gemm_b_box(0));
+            if (!bf16) L.prepass = prepass_transpose_b_grouped;
+            L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / xmr_gemm_bn(wide);
+            plan_wg_map(&L.map[0], dt, es, bf16 ? (uintptr_t)d->d_aux : 0, !bf16, d->K, XMR_WG_BM, 1, XMR_WG_BM);
+            if (bf16) plan_wg_map(&L.map[1], dt, es, (uintptr_t)d->d_aux, 0, d->N, d->M * d->K, 1, XMR_GEMM_BF16_BK);
+            else plan_wg_map(&L.map[1], dt, es, 0, 1, d->K, d->M * d->N, 1, xmr_gemm_b_box(0));
             break;
         }
-        plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uintptr_t)d->d_in, 0, d->K, (uint32_t)rows, 1, XMR_WG_BM);
-        plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 0, 1, d->K, (uint32_t)(batch * d->N), 1, xmr_gemm_b_box(pair));
+        plan_wg_map(&L.map[0], dt, es, (uintptr_t)d->d_in, 0, d->K, (uint32_t)rows, 1, XMR_WG_BM);
+        /* B: the stacked B^T in scratch, (batch N) rows of K; BF16: the caller's B, (batch K) rows of N in boxes of 64 columns x 64 k-rows */
+        if (bf16) plan_wg_map(&L.map[1], dt, es, (uintptr_t)d->d_aux, 0, d->N, (uint32_t)(batch * d->K), 1, XMR_GEMM_BF16_BK);
+        else plan_wg_map(&L.map[1], dt, es, 0, 1, d->K, (uint32_t)(batch * d->N), 1, xmr_gemm_b_box(pair));
         break;
     }
     default:
@@ -1212,13 +1243,14 @@ static void next_groups(const host_sched* s, uint64_t first, uint64_t* budget, h
     const uint64_t* ro = (const uint64_t*)s->d->d_rows;
     const uint64_t K = s->d->K, N = s->d->N;
     uint64_t e = first + 1;
-    while (e < s->total && (ro[e + 1] - ro[first]) * (K + N) * 4u + (e + 1 - first) * (K * N * 4u + 8u) + 8u <= *budget) ++e;
+    const uint64_t es = KINFO[s->d->kernel].mm_elem;         /* A and B elements; C elements are 4 bytes */
+    while (e < s->total && (ro[e + 1] - ro[first]) * (K * es + N * 4u) + (e + 1 - first) * (K * N * es + 8u) + 8u <= *budget) ++e;
     memset(c, 0, sizeof *c);
     const uint64_t rows = ro[e] - ro[first];
     c->items = e - first; c->M = (uint32_t)(e - first);
     c->n_units = rows * N; c->unit_base = (ro[first] - ro[0]) * N;
-    c->in = (byte_range){ ro[first] * K * 4u, rows * K * 4u }; c->in_bias = ro[first] * K * 4u;
-    c->aux = (byte_range){ first * K * N * 4u, (e - first) * K * N * 4u };
+    c->in = (byte_range){ ro[first] * K * es, rows * K * es }; c->in_bias = ro[first] * K * es;
+    c->aux = (byte_range){ first * K * N * es, (e - first) * K * N * es };
     c->out = (byte_range){ ro[first] * N * 4u, rows * N * 4u }; c->out_bias = ro[first] * N * 4u;
     c->rows = (byte_range){ first * 8u, (e - first + 1) * 8u };
 }
@@ -1357,9 +1389,10 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
         s.next = next_groups; s.total = d->M; s.max_bytes = chunk_bytes; s.budget = chunk_bytes; s.min_in = 16; s.path = "groups";
         return run_chunks(&s, out, dwc_fired);
     }
-    if (d->kernel == COAST_K_MM_U32 || d->kernel == COAST_K_GEMM_TF32) {
+    if (is_matmul(d->kernel)) {
         if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");
-        const uint64_t ab = (uint64_t)d->M * d->K * 4u, bb = (uint64_t)d->K * d->N * 4u, cb = (uint64_t)d->M * d->N * 4u;
+        const uint64_t es = KINFO[d->kernel].mm_elem;
+        const uint64_t ab = (uint64_t)d->M * d->K * es, bb = (uint64_t)d->K * d->N * es, cb = (uint64_t)d->M * d->N * 4u;
         if (d->mode & COAST_MM_BATCHED) {                    /* as many whole products as the chunk bytes hold, at least one */
             if (!d->d_in || !d->d_out || !d->d_aux) return fail(COAST_ERR_BAD_ARG, "null host buffer");
             s.next = next_products; s.total = d->n_units / ((uint64_t)d->M * d->N); s.upi = (uint64_t)d->M * d->N;
@@ -1373,7 +1406,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
                 const uint64_t blocks = d->M / 128u < 8u ? d->M / 128u : 8u;
                 rows = ((d->M / 128u + blocks - 1u) / blocks) * 128u;
             }
-            s.next = next_row_block; s.total = d->M; s.upi = d->N; s.ib = (uint64_t)d->K * 4u; s.ob = (uint64_t)d->N * 4u;
+            s.next = next_row_block; s.total = d->M; s.upi = d->N; s.ib = (uint64_t)d->K * es; s.ob = (uint64_t)d->N * 4u;
             s.max_items = rows; s.shared_b = bb;
             s.path = rows < d->M ? "row-blocks" : "one-shot";
         }

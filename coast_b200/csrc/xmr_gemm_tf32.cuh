@@ -15,6 +15,9 @@
 // Fault site 0 = the replica's final accumulator value (32 bits) as read for the vote.
 //
 // TF32 wgmma reads both operands K-major, so B goes through a transposing pre-pass (xmr_gemm_bt) into library scratch first.
+// The same body runs BF16 operands (xmr_gemm_bf16*, operand type Bf16 below): bfloat16 A and B, fp32 accumulators and C,
+// wgmma m64n128k16.  16-bit wgmma can read B MN-major, which is what a row-major K x N matrix is, so B is loaded in place from
+// the caller's buffer: no pre-pass and no scratch.
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, 64 rows of the 128-row tile each.
 // Persistent CTAs, one per SM.  Tiles: 128 x 256 unprotected (N % 256 == 0), 128 x 128 otherwise; the accumulators of a
 // replica are 64 x 128 wgmma fragments (64 fp32 registers per thread), so TMR holds 192 accumulator registers per thread.
@@ -29,16 +32,16 @@
 namespace xmr {
 namespace gemm {
 
-constexpr int BM = XMR_WG_BM, BK = XMR_GEMM_BK;      // BK fp32 = 128 bytes = one swizzle row
-constexpr int WG_K = 8;                              // one wgmma consumes 8 tf32 = 32 bytes of K
+constexpr int BM = XMR_WG_BM;
+constexpr uint32_t ROW_BYTES = 128;                  // a k-block of either operand type is one 128-byte swizzle row of A
 constexpr int WG_N = 128;                            // wgmma N per instruction
-constexpr uint32_t A_STAGE = BM * BK * 4;            // 16 KiB
+constexpr uint32_t A_STAGE = BM * ROW_BYTES;         // 16 KiB
 constexpr int CTA_THREADS = XMR_WG_THREADS;          // warpgroup 0 = producer, 1-2 = consumers
 template <int NC, bool WIDE = (NC == 1)> struct Geom {         // WIDE: 128 x 256 tiles (unprotected, N % 256 == 0)
     static constexpr int BN = (int)xmr_gemm_bn(WIDE);
     static constexpr int NSUB = BN / WG_N;
     static constexpr int STAGES = (int)xmr_gemm_stages(WIDE);   // 192 KiB of operand stages either way
-    static constexpr uint32_t B_STAGE = BK * BN * 4;             // [BN rows of B^T][128 B]
+    static constexpr uint32_t B_STAGE = BN * ROW_BYTES;          // TF32: [BN rows of B^T][128 B]; BF16: [BN / 64 boxes][64 k-rows][128 B]
     // 1 KiB alignment slack, the stages, then full[] and empty[]
     static_assert(1023u + STAGES * (A_STAGE + B_STAGE) + 2u * STAGES * sizeof(uint64_t) <= xmr_gemm_smem(WIDE),
                   "stages and barriers fit the launch's shared memory");
@@ -133,6 +136,45 @@ __device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], uint64_t da
         : "l"(da), "l"(db));
 }
 
+// Shared-memory matrix descriptor of an MN-major 16-bit operand in the 128-byte swizzle: what TMA (CU_TENSOR_MAP_SWIZZLE_128B)
+// leaves of a row-major K x N matrix loaded in boxes of 64 columns x 64 k-rows.  A box is 64 k-rows of 128 bytes (64 columns),
+// 8 KiB; the 16-byte chunks of a row are XORed with (k-row % 8), which is the swizzle atom of 64 columns x 8 k-rows = 1 KiB.
+// start >> 4 [0,14); LBO [16,30) = 8192 B from one 64-column box to the next; SBO [32,46) = 1024 B from one group of 8 k-rows
+// to the next; layout SWIZZLE_128B (1) [62,64).  One k16 step (two 8-row groups) is 2048 bytes further into the box: an add
+// of 128 to the start field; the next 128 columns are two boxes on: an add of 1024.
+__device__ __forceinline__ uint64_t wg_desc_mn(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+// D (+)= A . B with A K-major and B MN-major (the transpose immediates 0, 1) in shared memory; D's fragment layout as above
+__device__ __forceinline__ void wgmma_bf16_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db));
+}
+
+// The operand types of gemm_body.  Both stage 128-byte k-blocks (BK elements) and step A's descriptor by 32 bytes (WG_K elements)
+// per wgmma; they differ in the instruction and in how B reaches shared memory:
+//   Tf32: B^T rows from the transposing pre-pass, K-major like A; TMA boxes of B_BOX rows of B^T at 128 bytes per row;
+//   Bf16: B in place, MN-major; TMA boxes of 64 columns x BK k-rows (128 bytes is the widest box row this swizzle takes), 8 KiB
+//         each, so column c of the tile lies in the box at byte 128 c -- the same place B^T row c has for Tf32.
+struct Tf32 {
+    static constexpr int BK = XMR_GEMM_BK, WG_K = 8;
+    static constexpr bool B_IN_PLACE = false;
+    static constexpr uint32_t B_KSTEP = 32 >> 4;                 // descriptor start field per wgmma k step
+    static constexpr __host__ __device__ int b_box(bool pair) { return (int)xmr_gemm_b_box(pair); }
+    static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc(saddr); }
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_tf32_m64n128k8(d, da, db); }
+};
+struct Bf16 {
+    static constexpr int BK = XMR_GEMM_BF16_BK, WG_K = 16;
+    static constexpr bool B_IN_PLACE = true;
+    static constexpr uint32_t B_KSTEP = (WG_K * ROW_BYTES) >> 4;
+    static constexpr __host__ __device__ int b_box(bool) { return (int)XMR_GEMM_BF16_B_BOX; }
+    static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc_mn(saddr); }
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_bf16_m64n128k16(d, da, db); }
+};
+
 __device__ __forceinline__ void wgmma_u8_m64n32k32(uint32_t (&d)[16], uint64_t da, uint64_t db) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.u8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}"
@@ -204,15 +246,16 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float 
 // PAIR: the CTA pair of a cluster 2 x 1 x 1 computes a 256 x BN tile, rank r the rows [128 r, 128 r + 128); each rank loads half
 // of the tile's B^T rows and multicasts them to both, so a stage is released only when the consumers of BOTH CTAs are done with it.
 // GROUPED (single CTAs with 128 x 128 tiles, xmr_mm_grp.cuh): a.M products of their own row counts, `ro` their row offsets and
-// `grp` the group block: the tiles come from its tile_start table, A through its rebased map, B^T rows from g N.
-template <int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false>
+// `grp` the group block: the tiles come from its tile_start table, A through its rebased map, B^T rows from g N (Bf16: B rows from g K).
+template <class OP, int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false>
 __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b,
                                           const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr) {
     static_assert(!(GROUPED && (PAIR || WIDE)), "grouped launches run on single CTAs with 128 x 128 tiles");
     using G = Geom<NC, WIDE>;
     constexpr int BN = G::BN, NSUB = G::NSUB, STAGES = G::STAGES;
     constexpr uint32_t B_STAGE = G::B_STAGE;
-    constexpr int B_BOX = (int)xmr_gemm_b_box(PAIR);            // B^T rows per TMA box
+    constexpr int BK = OP::BK, WG_K = OP::WG_K;
+    constexpr int B_BOX = OP::b_box(PAIR);                      // B^T rows (Bf16: B columns) per TMA box
     constexpr uint32_t CTAS = PAIR ? 2u : 1u;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023u) & ~(uintptr_t)1023u);
@@ -276,22 +319,24 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
                 if constexpr (GROUPED) {
                     // rows past the product read the next product's rows (masked in the epilogue), or zeros past R
                     const grp::Tile x = grp::tile_of(ro, ro0, R, ts, n_grp, tiles_n, group_m, tile);
-                    m0 = (int)(x.start + x.tm * TM); nb = x.g * a.N; n_off = x.tn * BN; bn_t = BN;
+                    m0 = (int)(x.start + x.tm * TM); nb = x.g * (OP::B_IN_PLACE ? a.K : a.N); n_off = x.tn * BN; bn_t = BN;
                 } else {
                     decode(tile, tm, n_off, bn_t);
                     m0 = (int)(tm * TM + rank * BM);
                     nb = (tm * TM) / a.M * a.N;                     // first B^T row of the tile's product (stacked B^T)
+                    if constexpr (OP::B_IN_PLACE) nb = (tm * TM) / a.M * a.K;   // first row of the product's B (stacked B)
                 }
-                const uint32_t rows_b = bn_t / CTAS;                // B^T rows this CTA loads (for both CTAs of a pair)
+                const uint32_t rows_b = bn_t / CTAS;                // B^T rows (Bf16: B columns) this CTA loads (for both CTAs of a pair)
                 for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
                     const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
                     mbar_wait_or_trap(&empty[s], ph ^ 1u);
-                    mbar_arrive_expect_tx(&full[s], A_STAGE + bn_t * BK * 4u);
-                    tma_load_2d_hint(sA + s * A_STAGE, map_a, &full[s], (int)(kb * BK), m0, pol_a);          // box {32 k, 128 m}
+                    mbar_arrive_expect_tx(&full[s], A_STAGE + bn_t * ROW_BYTES);
+                    tma_load_2d_hint(sA + s * A_STAGE, map_a, &full[s], (int)(kb * BK), m0, pol_a);          // box {BK k, 128 m}
                     for (uint32_t c = 0; c < rows_b / B_BOX; ++c) {
-                        const uint32_t r = rank * rows_b + c * B_BOX;                                        // row of the tile's B^T
-                        if (PAIR) tma_load_2d_mcast(sB + s * B_STAGE + r * 128u, map_b, &full[s], (int)(kb * BK), (int)(nb + n_off + r), (uint16_t)3, pol_b);
-                        else tma_load_2d_hint(sB + s * B_STAGE + r * 128u, map_b, &full[s], (int)(kb * BK), (int)(nb + n_off + r), pol_b);
+                        const uint32_t r = rank * rows_b + c * B_BOX;                                        // row of the tile's B^T (Bf16: column of its B)
+                        const int c0 = OP::B_IN_PLACE ? (int)(n_off + r) : (int)(kb * BK), c1 = OP::B_IN_PLACE ? (int)(nb + kb * BK) : (int)(nb + n_off + r);
+                        if (PAIR) tma_load_2d_mcast(sB + s * B_STAGE + r * ROW_BYTES, map_b, &full[s], c0, c1, (uint16_t)3, pol_b);
+                        else tma_load_2d_hint(sB + s * B_STAGE + r * ROW_BYTES, map_b, &full[s], c0, c1, pol_b);
                     }
                 }
             }
@@ -323,20 +368,20 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
             for (uint32_t kb = 0; kb < kblocks; ++kb, ++it) {
                 const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
                 mbar_wait_or_trap(&full[s], ph);
-                const uint64_t da0 = wg_desc(smem_u32(sA + s * A_STAGE) + a_off), db0 = wg_desc(smem_u32(sB + s * B_STAGE));
+                const uint64_t da0 = wg_desc(smem_u32(sA + s * A_STAGE) + a_off), db0 = OP::desc_b(smem_u32(sB + s * B_STAGE));
                 wg_fence();
 #pragma unroll
                 for (int k = 0; k < BK / WG_K; ++k) {
 #pragma unroll
                     for (int sub = 0; sub < NSUB; ++sub) {
                         if ((uint32_t)sub >= nsub_t) break;
-                        const uint64_t da = da0 + (uint64_t)(2 * k), db = db0 + (uint64_t)(2 * k + sub * (WG_N * 128 >> 4));
+                        const uint64_t da = da0 + (uint64_t)(2 * k), db = db0 + (uint64_t)(OP::B_KSTEP * k + sub * (WG_N * ROW_BYTES >> 4));
 #pragma unroll
                         for (int r = 0; r < NC; ++r) {
                             // with several replica accumulators in flight, ptxas may move one between the asynchronous wgmmas
                             // (seen on the DWC kernel: wrong results); retiring each replica's wgmma before the next keeps them apart
                             if (NC > 1 && r > 0) { wg_commit(); wg_wait<0>(); wg_fence(); }
-                            wgmma_tf32_m64n128k8(acc[r][sub], da, db);
+                            OP::mma(acc[r][sub], da, db);
                         }
                     }
                 }
@@ -388,41 +433,63 @@ xmr_gemm_bt(const float* __restrict__ B, float* __restrict__ Bt, unsigned int K,
     }
 }
 
-#define XMR_GEMM_KERNEL(NAME, NC, INJ, WIDE, PAIR, CLUSTER)                                              \
+#define XMR_GEMM_KERNEL(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER)                                            \
     extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                      \
     NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b) { \
-        xmr::gemm::gemm_body<NC, INJ != 0, WIDE, PAIR>(a, &map_a, &map_b);                               \
+        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, PAIR>(a, &map_a, &map_b);                        \
     }
 #define XMR_NO_CLUSTER
 #define XMR_PAIR_CLUSTER __cluster_dims__(2, 1, 1)
-XMR_GEMM_KERNEL(xmr_gemm_tf32_nc1_inj0, 1, 0, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32_nc2_inj0, 2, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32_nc3_inj0, 3, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32_nc1_inj1, 1, 1, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32_nc2_inj1, 2, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32_nc3_inj1, 3, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc1_inj0, 1, 0, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc2_inj0, 2, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc3_inj0, 3, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc1_inj1, 1, 1, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc2_inj1, 2, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc3_inj1, 3, 1, false, false, XMR_NO_CLUSTER)
 // unprotected, N a multiple of 128 but not of 256: 128 x 128 tiles
-XMR_GEMM_KERNEL(xmr_gemm_tf32n_nc1_inj0, 1, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32n_nc1_inj1, 1, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32n_nc1_inj0, 1, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32n_nc1_inj1, 1, 1, false, false, XMR_NO_CLUSTER)
 // CTA pairs: 256 x 256 (unprotected) / 256 x 128 pair tiles
-XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc1_inj0, 1, 0, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc2_inj0, 2, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc3_inj0, 3, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc1_inj1, 1, 1, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc2_inj1, 2, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(xmr_gemm_tf32p_nc3_inj1, 3, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc1_inj0, 1, 0, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc2_inj0, 2, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc3_inj0, 3, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc1_inj1, 1, 1, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc2_inj1, 2, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc3_inj1, 3, 1, false, true, XMR_PAIR_CLUSTER)
 
 // grouped (COAST_MM_GROUPED): single CTAs and 128 x 128 tiles (tf32n unprotected); `ro` = the caller's row offsets, `grp` = the
 // group block the pre-pass wrote (xmr_mm_grp.cuh)
-#define XMR_GEMM_GRP_KERNEL(NAME, NC, INJ, WIDE)                                                           \
+#define XMR_GEMM_GRP_KERNEL(OP, NAME, NC, INJ, WIDE)                                                       \
     extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
     NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, \
          const unsigned long long* ro, const uint8_t* grp) {                                             \
-        xmr::gemm::gemm_body<NC, INJ != 0, WIDE, false, true>(a, &map_a, &map_b, ro, grp);               \
+        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, false, true>(a, &map_a, &map_b, ro, grp);        \
     }
-XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32_grp_inj0_nc2, 2, 0, false)
-XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32_grp_inj0_nc3, 3, 0, false)
-XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32_grp_inj1_nc2, 2, 1, false)
-XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32_grp_inj1_nc3, 3, 1, false)
-XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32n_grp_inj0_nc1, 1, 0, false)
-XMR_GEMM_GRP_KERNEL(xmr_gemm_tf32n_grp_inj1_nc1, 1, 1, false)
+XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj0_nc2, 2, 0, false)
+XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj0_nc3, 3, 0, false)
+XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj1_nc2, 2, 1, false)
+XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj1_nc3, 3, 1, false)
+XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32n_grp_inj0_nc1, 1, 0, false)
+XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32n_grp_inj1_nc1, 1, 1, false)
+
+// BF16 operands: the same variants (wide / narrow / pair / grouped), B read in place; named _inj<i>_nc<n> like the grouped kernels
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj0_nc2, 2, 0, false)
+XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj0_nc3, 3, 0, false)
+XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj1_nc2, 2, 1, false)
+XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj1_nc3, 3, 1, false)
+XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16n_grp_inj0_nc1, 1, 0, false)
+XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16n_grp_inj1_nc1, 1, 1, false)

@@ -8,7 +8,7 @@
 // The tiled paths cut every product into tiles of TM rows on its own (no tile mixes two products): a one-CTA pre-pass
 // (xmr_mm_group_scan) writes tile_start[g], the exclusive scan of ceil(M_g / TM), and the total into the group block in scratch,
 // and each tile id finds its product by binary search.  Group block layout (XMR_MM_GRP_*):
-//   [0, 128)              TF32 only: the A tensor map, rebased by the pre-pass onto row ro[0] of d_in with R rows
+//   [0, 128)              TF32 / BF16 only: the A tensor map, rebased by the pre-pass onto row ro[0] of d_in with R rows
 //   [128, 128 + 4 (G+1))  tile_start[0 .. G] (u32), tile_start[G] = row tiles of all products
 #pragma once
 #include "xmr_common.cuh"
@@ -63,7 +63,7 @@ __device__ __forceinline__ Tile tile_of(const unsigned long long* ro, unsigned l
 }  // namespace grp
 }  // namespace xmr
 
-// tile_start of a grouped launch (one CTA; G <= XMR_MM_GRP_MAX, so each thread scans at most 1024 entries), and for the TF32
+// tile_start of a grouped launch (one CTA; G <= XMR_MM_GRP_MAX, so each thread scans at most 1024 entries), and for the GEMM
 // kernels the A tensor map: the host encodes its shape, this kernel points it at row ro[0] of `a_base` with R rows
 // (tensormap.replace), so a shard or a host-call chunk needs no host-side read of the device table.
 extern "C" __global__ void __launch_bounds__(XMR_MM_GRP_SCAN_THREADS)

@@ -12,19 +12,19 @@ from dataclasses import dataclass
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
-K_CRC16, K_SHA256, K_AES128, K_MM_U32, K_GEMM_TF32, K_QSORT, K_CHSTONE_SHA, K_CHSTONE_AES = range(8)
+K_CRC16, K_SHA256, K_AES128, K_MM_U32, K_GEMM_TF32, K_QSORT, K_CHSTONE_SHA, K_CHSTONE_AES, K_GEMM_BF16 = range(9)
 F_COUNT_ERRORS, F_COUNT_SYNCS, F_NO_MEM_REPLICATION = 0x1, 0x2, 0x4
 F_INTERLEAVE, F_SEGMENT, F_VERBOSE, F_MAJORITY_VOTER = 0x8, 0x10, 0x20, 0x100
 F_STORE_DATA_SYNC, F_NO_STORE_DATA_SYNC, F_NO_LOAD_SYNC, F_NO_STORE_ADDR_SYNC = 0x200, 0x400, 0x800, 0x1000
 PLAN_NONE, PLAN_BERNOULLI, PLAN_TABLE = 0, 1, 2
 AES_DECRYPT, AES_KEY_PER_UNIT, AES_KEY_WRITEBACK = 1, 2, 4
 UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 / QSORT batches: aux = n_units + 1 u64 byte offsets into inp
-MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32: n_units = batch*M*N, inp / aux / out hold batch A / B / C
-MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
+MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32 / GEMM_BF16: n_units = batch*M*N, inp / aux / out hold batch A / B / C
+MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32 / GEMM_BF16: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 
-OUT_BYTES = {K_CRC16: 2, K_SHA256: 32, K_AES128: 16, K_MM_U32: 4, K_GEMM_TF32: 4, K_CHSTONE_SHA: 20, K_CHSTONE_AES: 64}
+OUT_BYTES = {K_CRC16: 2, K_SHA256: 32, K_AES128: 16, K_MM_U32: 4, K_GEMM_TF32: 4, K_CHSTONE_SHA: 20, K_CHSTONE_AES: 64, K_GEMM_BF16: 4}
 
 
 def out_bytes(kernel: int, unit_bytes: int = 0) -> int:
@@ -272,10 +272,11 @@ class Runtime:
     # -- convenience: device tensors in, device tensor + Stats out ----------------------------
     def run(self, kernel, num_clones, inp, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0, aux=None,
             key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, out=None, stream=None, status=None, rows=None):
-        """rows: with MM_GROUPED, the CUDA int64/uint64 tensor of M + 1 row offsets (M = the product count)"""
+        """rows: with MM_GROUPED, the CUDA int64/uint64 tensor of M + 1 row offsets (M = the product count).
+        K_GEMM_BF16: inp and aux are torch.bfloat16 tensors (or their uint16 / int16 views); the result is fp32 like K_GEMM_TF32's."""
         torch = self.torch
         if mode & MM_GROUPED:
-            self._check_rows(rows, M, N, n_units, inp, K, out)
+            self._check_rows(rows, M, N, n_units, inp, K, out, 2 if kernel == K_GEMM_BF16 else 4)
         ragged_qsort = bool(mode & UNIT_OFFSETS) and kernel == K_QSORT
         if out is None and ragged_qsort:       # the arrays are sorted into the bytes they came from: out mirrors inp
             out = torch.zeros(inp.numel() * inp.element_size(), dtype=torch.uint8, device=f"cuda:{self.device}")
@@ -291,9 +292,9 @@ class Runtime:
         self.launch(d, stream)
         return out, self.sync(stream)
 
-    def _check_rows(self, rows, G, N, n_units, inp, K, out):
+    def _check_rows(self, rows, G, N, n_units, inp, K, out, esize=4):
         """A grouped launch's device row offsets (int64 or uint64 tensor, G + 1 entries): they never decrease and span exactly
-        n_units / N rows, which lie within inp (K per row) and out (N per row).  The kernels only clamp; this catches a bad table
+        n_units / N rows, which lie within inp (K elements of esize bytes per row) and out (N per row).  The kernels only clamp; this catches a bad table
         before it runs."""
         torch = self.torch
         if rows is None or not hasattr(rows, "data_ptr") or rows.dtype not in (torch.int64, torch.uint64) or not rows.is_cuda:
@@ -304,7 +305,7 @@ class Runtime:
             raise CoastError(ERR_BAD_ARG, f"MM_GROUPED: n_units ({n_units}) must be a multiple of N ({N})")
         ro = rows[: G + 1].view(torch.int64)
         R = n_units // N
-        in_rows = inp.numel() * inp.element_size() // (4 * K) if K else 0
+        in_rows = inp.numel() * inp.element_size() // (esize * K) if K else 0
         out_rows = out.numel() * out.element_size() // (4 * N) if out is not None else None
         bad = torch.stack([(ro < 0).any(), (ro[1:] < ro[:-1]).any(), ro[-1] - ro[0] != R, ro[-1] > in_rows]).tolist()
         if any(bad) or (out_rows is not None and int(ro[-1]) > out_rows):
