@@ -551,6 +551,15 @@ static void plan_wg_map(map_desc* m, CUtensorMapDataType dtype, unsigned esize, 
 static uint64_t mm_batch(const coast_launch_desc* d) {
     return (d->mode & COAST_MM_BATCHED) ? d->n_units / ((uint64_t)d->M * d->N) : 1u;
 }
+/* B's tensor map has K rows per product only for GEMM_BF16 reading B in place; every B^T map (scratch or the caller's) has N */
+static int mm_b_rows_k(const coast_launch_desc* d) {
+    return d->kernel == COAST_K_GEMM_BF16 && !(d->mode & COAST_MM_B_TRANSPOSED);
+}
+static int b_transposed_check(const coast_launch_desc* d) {
+    if ((d->mode & COAST_MM_B_TRANSPOSED) && !is_matmul(d->kernel))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_B_TRANSPOSED: a transposed B exists for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", d->kernel);
+    return COAST_OK;
+}
 static int batched_check(const coast_launch_desc* d) {
     if (!is_matmul(d->kernel))
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batched products exist for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", d->kernel);
@@ -560,8 +569,9 @@ static int batched_check(const coast_launch_desc* d) {
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: n_units must be a nonzero multiple of M*N = %llu (got %llu)",
                     (unsigned long long)mn, (unsigned long long)d->n_units);
     const uint64_t batch = d->n_units / mn;
-    /* the rows of the stacked operands are tensor-map coordinates: A's batch*M, and B^T's batch*N or, for GEMM_BF16 (B in place), B's batch*K */
-    const int b_rows_k = d->kernel == COAST_K_GEMM_BF16;
+    /* the rows of the stacked operands are tensor-map coordinates: A's batch*M, and B^T's batch*N or, for GEMM_BF16 with B in place
+     * (no COAST_MM_B_TRANSPOSED), B's batch*K */
+    const int b_rows_k = mm_b_rows_k(d);
     if (batch * d->M >= (1ull << 31) || batch * (b_rows_k ? d->K : d->N) >= (1ull << 31))
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batch*M and batch*%c must be below 2^31 (batch %llu, M %u, %c %u)",
                     b_rows_k ? 'K' : 'N', (unsigned long long)batch, d->M, b_rows_k ? 'K' : 'N', b_rows_k ? d->K : d->N);
@@ -576,14 +586,24 @@ static int prepass_transpose_b(const coast_launch_desc* d, CUdeviceptr bt, CUstr
     void* params[] = { &B, &bt, &k32, &n32, &nb };
     return launch_small("xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
 }
+/* The B^T planes [plane][b N + n][k]: split_bt transposes B; a caller's B^T (COAST_MM_B_TRANSPOSED) already has that row order,
+ * so the streaming split of A makes them from its (batch N) rows of K. */
+static int prepass_split_b(const coast_launch_desc* d, CUdeviceptr pb, unsigned batch, CUstream s) {
+    const void* B = d->d_aux;
+    if (d->mode & COAST_MM_B_TRANSPOSED) {
+        unsigned long long rows = (unsigned long long)batch * d->N, K = d->K;
+        void* params[] = { &B, &pb, &rows, &K };
+        return launch_small("xmr_mm_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
+    }
+    unsigned int k32 = d->K, n32 = d->N, nb = batch;
+    void* params_b[] = { &B, &pb, &k32, &n32, &nb };
+    return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
+}
 static int prepass_split_limbs(const coast_launch_desc* d, CUdeviceptr pa, CUstream s) {
     unsigned long long rows = mm_batch(d) * d->M, K = d->K; const void* A = d->d_in;
     void* params_a[] = { &A, &pa, &rows, &K };
     int rc = launch_small("xmr_mm_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_a, s); if (rc) return rc;
-    CUdeviceptr pb = pa + (size_t)rows * d->K * 4u;
-    unsigned int k32 = d->K, n32 = d->N, nb = (unsigned)mm_batch(d); const void* B = d->d_aux;
-    void* params_b[] = { &B, &pb, &k32, &n32, &nb };
-    return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
+    return prepass_split_b(d, pa + (size_t)rows * d->K * 4u, (unsigned)mm_batch(d), s);
 }
 
 /* Grouped matmuls (COAST_MM_GROUPED): the checks shared by coast_launch and coast_run_host.  M is the product count G, the
@@ -599,7 +619,7 @@ static int grouped_check(const coast_launch_desc* d) {
     if (d->n_units % d->N)
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: n_units must be a multiple of N = %u (R rows x N; got %llu)", d->N,
                     (unsigned long long)d->n_units);
-    const int b_rows_k = d->kernel == COAST_K_GEMM_BF16;                /* as in batched_check */
+    const int b_rows_k = mm_b_rows_k(d);                               /* as in batched_check */
     if (d->n_units / d->N >= (1ull << 31) || (uint64_t)d->M * (b_rows_k ? d->K : d->N) >= (1ull << 31))
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the rows R and G*%c must be below 2^31 (R %llu, G %u, %c %u)",
                     b_rows_k ? 'K' : 'N', (unsigned long long)(d->n_units / d->N), d->M, b_rows_k ? 'K' : 'N', b_rows_k ? d->K : d->N);
@@ -612,10 +632,7 @@ static int prepass_split_limbs_grouped(const coast_launch_desc* d, CUdeviceptr p
     unsigned long long rows = d->n_units / d->N, K = d->K; const void* A = d->d_in; const void* ro = d->d_rows;
     void* params_a[] = { &ro, &A, &pa, &rows, &K };
     int rc = launch_small("xmr_mm_grp_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_a, s); if (rc) return rc;
-    CUdeviceptr pb = pa + (size_t)rows * d->K * 4u;
-    unsigned int k32 = d->K, n32 = d->N, nb = d->M; const void* B = d->d_aux;
-    void* params_b[] = { &B, &pb, &k32, &n32, &nb };
-    return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
+    return prepass_split_b(d, pa + (size_t)rows * d->K * 4u, d->M, s);
 }
 static int prepass_transpose_b_grouped(const coast_launch_desc* d, CUdeviceptr bt, CUstream s) {
     const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N, nb = d->M;
@@ -718,6 +735,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     if (batched && (rc = batched_check(d))) return rc;
     const int grouped = (d->mode & COAST_MM_GROUPED) != 0;
     if (grouped && (rc = grouped_check(d))) return rc;
+    if ((rc = b_transposed_check(d))) return rc;
+    const int bt = (d->mode & COAST_MM_B_TRANSPOSED) != 0;
     if (d->n_units == 0) return COAST_OK;
     if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null device buffer");
     const uint32_t nc = d->num_clones;
@@ -731,7 +750,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     a.status = (unsigned char*)d->d_status;
     /* the kernels find a batch from n_units / N (rows of the stacked problem) and a.M (rows per product): a batch of one is
      * an unbatched launch, argument block included */
-    a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~(COAST_MM_BATCHED | COAST_MM_GROUPED);
+    a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~(COAST_MM_BATCHED | COAST_MM_GROUPED | COAST_MM_B_TRANSPOSED);
     a.M = d->M; a.N = d->N; a.K = d->K;
     memcpy(a.key, d->key, 16);
     if (inj) {
@@ -821,11 +840,13 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
             const int galigned = aligned16 && !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u);
             const uint64_t R = d->n_units / d->N;
             L.grouped = 1;
-            snprintf(L.name, sizeof L.name, "xmr_mm_u32_grp_inj%d_nc%u", inj, nc);
+            snprintf(L.name, sizeof L.name, bt ? "xmr_mm_u32_bt_grp_inj%d_nc%u" : "xmr_mm_u32_grp_inj%d_nc%u", inj, nc);
             if (store_votes || !galigned) break;
             if ((!gpath || !strcmp(gpath, "tc")) && d->N % xmr_mmtc_bn(1) == 0 && d->K % XMR_MMTC_BK == 0) {
                 const unsigned bn = xmr_mmtc_bn(nc);
-                snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_grp_inj%d_nc%u", inj, nc);
+                /* B^T: the same planes (the pre-pass differs); only the fault recompute reads B itself */
+                if (bt && inj) snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_bt_grp_inj1_nc%u", nc);
+                else snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_grp_inj%d_nc%u", inj, nc);
                 L.block = XMR_WG_THREADS; L.smem = xmr_mmtc_smem(nc);
                 L.ctas = (R / XMR_WG_BM + d->M) * (d->N / bn); L.waves = 1;       /* a bound on the tiles; persistent CTAs */
                 L.grp_off = ((size_t)R * d->K + (size_t)d->M * d->K * d->N) * 4u;   /* after the limb planes */
@@ -835,7 +856,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
                 plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, (uint32_t)R, 4, XMR_WG_BM);
                 plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)R * d->K * 4u, 1, d->K, d->M * d->N, 4, bn);
             } else if (!(gpath && !strcmp(gpath, "naive")) && d->N % XMR_MMT_BN == 0 && d->K % XMR_MMT_BK == 0) {
-                snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_grp_inj%d_nc%u", inj, nc);
+                snprintf(L.name, sizeof L.name, bt ? "xmr_mm_u32_tiled_bt_grp_inj%d_nc%u" : "xmr_mm_u32_tiled_grp_inj%d_nc%u", inj, nc);
                 L.block = xmr_mmt_threads(nc); L.smem = XMR_MMT_SMEM;
                 L.ctas = (R / XMR_MMT_BM + d->M) * (d->N / XMR_MMT_BN); L.waves = 0;   /* a bound on the tiles: surplus CTAs exit */
                 L.scratch = (size_t)xmr_mm_grp_bytes(d->M);
@@ -846,14 +867,16 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         /* the plain kernel (one lane per replica per element) takes any shape and the per-k votes on `sum`; tile-aligned problems
          * go to the tensor cores (exact, u8 limbs on wgmma) or the register-tiled kernel; COAST_MM_PATH=tc|tiled|naive overrides.
          * The shape rules are those of one product; a batch stacks the products' rows (no tile straddles two of them). */
-        snprintf(L.name, sizeof L.name, "xmr_mm_u32_nc%u_inj%d", nc, inj);
+        if (bt) snprintf(L.name, sizeof L.name, "xmr_mm_u32_bt_inj%d_nc%u", inj, nc);
+        else snprintf(L.name, sizeof L.name, "xmr_mm_u32_nc%u_inj%d", nc, inj);
         const char* path = getenv("COAST_MM_PATH");
         const int aligned = aligned16 && !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u);
         const uint64_t batch = mm_batch(d), rows = batch * d->M;
         if (store_votes || !aligned) break;
         if ((!path || !strcmp(path, "tc")) && d->M % XMR_WG_BM == 0 && d->N % xmr_mmtc_bn(1) == 0 && d->K % XMR_MMTC_BK == 0) {
             const unsigned bn = xmr_mmtc_bn(nc);
-            snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_nc%u_inj%d", nc, inj);
+            if (bt && inj) snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_bt_inj1_nc%u", nc);
+            else snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_nc%u_inj%d", nc, inj);
             L.block = XMR_WG_THREADS; L.smem = xmr_mmtc_smem(nc);
             L.ctas = (rows / XMR_WG_BM) * (d->N / bn); L.waves = 1;
             L.scratch = ((size_t)rows * d->K + (size_t)batch * d->K * d->N) * 4u;     /* 4 planes of 1 byte per element */
@@ -862,7 +885,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
             plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, (uint32_t)rows, 4, XMR_WG_BM);
             plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)rows * d->K * 4u, 1, d->K, (uint32_t)(batch * d->N), 4, bn);
         } else if (!(path && !strcmp(path, "naive")) && d->M % XMR_MMT_BM == 0 && d->N % XMR_MMT_BN == 0 && d->K % XMR_MMT_BK == 0) {
-            snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_nc%u_inj%d", nc, inj);
+            if (bt) snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_bt_inj%d_nc%u", inj, nc);
+            else snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_nc%u_inj%d", nc, inj);
             L.block = xmr_mmt_threads(nc); L.smem = XMR_MMT_SMEM;
             L.ctas = (rows / XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;
         }
@@ -927,7 +951,14 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         const char* e = getenv("COAST_GEMM_PAIR");
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
         const int pair = !grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
-        if (bf16) {
+        if (bf16 && bt) {                                   /* B^T read in place, K-major (xmr_gemm_bf16*_bt_*) */
+            if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_bt_grp_inj%d_nc1", inj);
+            else if (grouped) snprintf(L.name, sizeof L.name, nc == 2 ? "xmr_gemm_bf16_bt_grp_inj%d_nc2" : "xmr_gemm_bf16_bt_grp_inj%d_nc3", inj);
+            else if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16p_bt_inj%d_nc%u", inj, nc);
+            else if (nc == 1 && !wide) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_bt_inj%d_nc1", inj);
+            else snprintf(L.name, sizeof L.name, "xmr_gemm_bf16_bt_inj%d_nc%u", inj, nc);
+        }
+        else if (bf16) {
             if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_grp_inj%d_nc1", inj);
             else if (grouped) snprintf(L.name, sizeof L.name, nc == 2 ? "xmr_gemm_bf16_grp_inj%d_nc2" : "xmr_gemm_bf16_grp_inj%d_nc3", inj);
             else if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16p_inj%d_nc%u", inj, nc);
@@ -949,32 +980,35 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         L.block = XMR_WG_THREADS; L.smem = xmr_gemm_smem(wide);
         const uint64_t batch = mm_batch(d), rows = batch * d->M;
         L.ctas = (rows / XMR_WG_BM) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = pair ? 2 : 1;
-        if (!bf16) {
-            L.scratch = (size_t)batch * d->K * d->N * 4u;                      /* B^T of every product */
+        /* B^T of every product into scratch, unless the caller holds it (COAST_MM_B_TRANSPOSED) or BF16 reads B in place */
+        const int b_scratch = !bf16 && !bt, b_in_place = bf16 && !bt;
+        if (b_scratch) {
+            L.scratch = (size_t)batch * d->K * d->N * 4u;
             L.prepass = prepass_transpose_b;
         }
         L.n_maps = 2;
         if (grouped) {
             /* 128 x 128 tiles of every product on single CTAs (no pairs, no wide tiles); A's map is encoded here over 128 rows of a
              * placeholder and rebased by the scan onto row ro[0] of d_in with R rows (the host does not read the device table).  The
-             * placeholder is the B^T scratch, or for BF16 (no scratch) B itself: d_in of a host-call chunk is biased by ro[first] rows
-             * and need not be an address of its own */
+             * placeholder is the B^T scratch, or without it (BF16, or a caller's B^T) d_aux: d_in of a host-call chunk is biased by
+             * ro[first] rows and need not be an address of its own */
             const uint64_t R = d->n_units / d->N;
             L.grouped = 1;
             L.ctas = (R / XMR_WG_BM + d->M) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = 1;
-            L.grp_off = bf16 ? 0 : (size_t)d->M * d->K * d->N * 4u;                /* after B^T of every product */
+            L.grp_off = b_scratch ? (size_t)d->M * d->K * d->N * 4u : 0;         /* after B^T of every product */
             L.scratch = L.grp_off + (size_t)xmr_mm_grp_bytes(d->M);
-            if (!bf16) L.prepass = prepass_transpose_b_grouped;
+            if (b_scratch) L.prepass = prepass_transpose_b_grouped;
             L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / xmr_gemm_bn(wide);
-            plan_wg_map(&L.map[0], dt, es, bf16 ? (uintptr_t)d->d_aux : 0, !bf16, d->K, XMR_WG_BM, 1, XMR_WG_BM);
-            if (bf16) plan_wg_map(&L.map[1], dt, es, (uintptr_t)d->d_aux, 0, d->N, d->M * d->K, 1, XMR_GEMM_BF16_BK);
-            else plan_wg_map(&L.map[1], dt, es, 0, 1, d->K, d->M * d->N, 1, xmr_gemm_b_box(0));
+            plan_wg_map(&L.map[0], dt, es, b_scratch ? 0 : (uintptr_t)d->d_aux, b_scratch, d->K, XMR_WG_BM, 1, XMR_WG_BM);
+            if (b_in_place) plan_wg_map(&L.map[1], dt, es, (uintptr_t)d->d_aux, 0, d->N, d->M * d->K, 1, XMR_GEMM_BF16_BK);
+            else plan_wg_map(&L.map[1], dt, es, b_scratch ? 0 : (uintptr_t)d->d_aux, b_scratch, d->K, d->M * d->N, 1, xmr_gemm_b_box(0));
             break;
         }
         plan_wg_map(&L.map[0], dt, es, (uintptr_t)d->d_in, 0, d->K, (uint32_t)rows, 1, XMR_WG_BM);
-        /* B: the stacked B^T in scratch, (batch N) rows of K; BF16: the caller's B, (batch K) rows of N in boxes of 64 columns x 64 k-rows */
-        if (bf16) plan_wg_map(&L.map[1], dt, es, (uintptr_t)d->d_aux, 0, d->N, (uint32_t)(batch * d->K), 1, XMR_GEMM_BF16_BK);
-        else plan_wg_map(&L.map[1], dt, es, 0, 1, d->K, (uint32_t)(batch * d->N), 1, xmr_gemm_b_box(pair));
+        /* B: the stacked B^T, (batch N) rows of K, in scratch or the caller's (COAST_MM_B_TRANSPOSED); BF16 without the bit: the
+         * caller's B, (batch K) rows of N in boxes of 64 columns x 64 k-rows */
+        if (b_in_place) plan_wg_map(&L.map[1], dt, es, (uintptr_t)d->d_aux, 0, d->N, (uint32_t)(batch * d->K), 1, XMR_GEMM_BF16_BK);
+        else plan_wg_map(&L.map[1], dt, es, b_scratch ? 0 : (uintptr_t)d->d_aux, b_scratch, d->K, (uint32_t)(batch * d->N), 1, xmr_gemm_b_box(pair));
         break;
     }
     default:
@@ -1350,6 +1384,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
     { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) chunk_bytes = (uint64_t)atoll(e); }
     host_sched s; memset(&s, 0, sizeof s);
     s.d = d; s.upi = 1; s.path = "staged";
+    if ((rc = b_transposed_check(d))) return rc;
 
     if (d->mode & COAST_UNIT_OFFSETS) {                      /* ragged: staged only */
         if ((rc = ragged_check(d))) return rc;

@@ -14,10 +14,12 @@
 // Unit = one C element (the `mm_t` store, mm_common_tmr.c:16); local unit index = i*N + j.
 // Fault site 0 = the replica's final accumulator value (32 bits) as read for the vote.
 //
-// TF32 wgmma reads both operands K-major, so B goes through a transposing pre-pass (xmr_gemm_bt) into library scratch first.
+// TF32 wgmma reads both operands K-major, so B goes through a transposing pre-pass (xmr_gemm_bt) into library scratch first;
+// a caller who holds B^T (COAST_MM_B_TRANSPOSED) skips it: the same kernels read the caller's B^T rows in place.
 // The same body runs BF16 operands (xmr_gemm_bf16*, operand type Bf16 below): bfloat16 A and B, fp32 accumulators and C,
 // wgmma m64n128k16.  16-bit wgmma can read B MN-major, which is what a row-major K x N matrix is, so B is loaded in place from
-// the caller's buffer: no pre-pass and no scratch.
+// the caller's buffer: no pre-pass and no scratch.  A BF16 B^T (COAST_MM_B_TRANSPOSED) is read in place K-major (Bf16T, the
+// xmr_gemm_bf16*_bt_* kernels).
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, 64 rows of the 128-row tile each.
 // Persistent CTAs, one per SM.  Tiles: 128 x 256 unprotected (N % 256 == 0), 128 x 128 otherwise; the accumulators of a
 // replica are 64 x 128 wgmma fragments (64 fp32 registers per thread), so TMR holds 192 accumulator registers per thread.
@@ -145,12 +147,14 @@ __device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], uint64_t da
 __device__ __forceinline__ uint64_t wg_desc_mn(uint32_t saddr) {
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// D (+)= A . B with A K-major and B MN-major (the transpose immediates 0, 1) in shared memory; D's fragment layout as above
+// D (+)= A . B with A K-major and B MN-major (the transpose immediates 0, 1) in shared memory, or, TRANS_B = 0, D (+)= A . B^T
+// with both operands K-major (0, 0); D's fragment layout as above
+template <int TRANS_B = 1>
 __device__ __forceinline__ void wgmma_bf16_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 1;\n\t}"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, %66;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(da), "l"(db));
+        : "l"(da), "l"(db), "n"(TRANS_B));
 }
 
 // The operand types of gemm_body.  Both stage 128-byte k-blocks (BK elements) and step A's descriptor by 32 bytes (WG_K elements)
@@ -158,6 +162,8 @@ __device__ __forceinline__ void wgmma_bf16_m64n128k16(float (&d)[64], uint64_t d
 //   Tf32: B^T rows from the transposing pre-pass, K-major like A; TMA boxes of B_BOX rows of B^T at 128 bytes per row;
 //   Bf16: B in place, MN-major; TMA boxes of 64 columns x BK k-rows (128 bytes is the widest box row this swizzle takes), 8 KiB
 //         each, so column c of the tile lies in the box at byte 128 c -- the same place B^T row c has for Tf32.
+//   Bf16T: the caller's B^T (COAST_MM_B_TRANSPOSED: N rows of K) read in place, K-major like A and like Tf32's B^T: the same
+//         boxes of B_BOX rows of 128 bytes (64 k), a k16 step is 32 bytes, and the wgmma's B transpose immediate is 0.
 struct Tf32 {
     static constexpr int BK = XMR_GEMM_BK, WG_K = 8;
     static constexpr bool B_IN_PLACE = false;
@@ -173,6 +179,14 @@ struct Bf16 {
     static constexpr __host__ __device__ int b_box(bool) { return (int)XMR_GEMM_BF16_B_BOX; }
     static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc_mn(saddr); }
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_bf16_m64n128k16(d, da, db); }
+};
+struct Bf16T {
+    static constexpr int BK = XMR_GEMM_BF16_BK, WG_K = 16;
+    static constexpr bool B_IN_PLACE = false;
+    static constexpr uint32_t B_KSTEP = 32 >> 4;
+    static constexpr __host__ __device__ int b_box(bool pair) { return (int)xmr_gemm_b_box(pair); }
+    static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc(saddr); }
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_bf16_m64n128k16<0>(d, da, db); }
 };
 
 __device__ __forceinline__ void wgmma_u8_m64n32k32(uint32_t (&d)[16], uint64_t da, uint64_t db) {
@@ -493,3 +507,24 @@ XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj1_nc2, 2, 1, false)
 XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj1_nc3, 3, 1, false)
 XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16n_grp_inj0_nc1, 1, 0, false)
 XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16n_grp_inj1_nc1, 1, 1, false)
+// BF16 with B^T read in place, K-major (COAST_MM_B_TRANSPOSED): the same variants
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16n_bt_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16n_bt_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj0_nc2, 2, 0, false)
+XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj0_nc3, 3, 0, false)
+XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj1_nc2, 2, 1, false)
+XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj1_nc3, 3, 1, false)
+XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16n_bt_grp_inj0_nc1, 1, 0, false)
+XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16n_bt_grp_inj1_nc1, 1, 1, false)

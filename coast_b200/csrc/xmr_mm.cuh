@@ -12,13 +12,14 @@
 //
 // Grouped launches (COAST_MM_GROUPED, xmr_mm_grp.cuh): each element finds its row's product by binary search over the row
 // offsets; a row outside every product's clamped range (a malformed table) is neither computed nor stored.
+// BT (COAST_MM_B_TRANSPOSED): aux holds B^T, N rows of K per product; element (k, j) is read at j*K + k instead of k*N + j.
 #pragma once
 #include "xmr_common.cuh"
 #include "xmr_mm_grp.cuh"
 
 namespace xmr {
 
-template <int NC, bool INJECT, bool GROUPED = false>
+template <int NC, bool INJECT, bool GROUPED = false, bool BT = false>
 __device__ __forceinline__ void mm_u32_body(const xmr_args& a, const unsigned long long* ro = nullptr) {
     constexpr int UPW = Lanes<NC>::kUnitsPerWarp;
     const int lane = threadIdx.x & 31;
@@ -54,11 +55,12 @@ __device__ __forceinline__ void mm_u32_body(const xmr_args& a, const unsigned lo
             }
         }
         const uint32_t* ap = A + (size_t)(ro0 + i) * K;         // i: row of the stacked problem; a batch's product i / M
-        const uint32_t* bp = B + (size_t)(GROUPED ? g : i / a.M) * K * N + j;
+        const uint32_t* bp = B + (size_t)(GROUPED ? g : i / a.M) * K * N + (BT ? (size_t)j * K : j);
+        const size_t bstride = BT ? 1u : N;                     // from B[k][j] to B[k + 1][j]
         uint32_t sum = 0;
         if (!(a.flags & XMR_F_STORE_VOTES)) {
             for (uint32_t k = 0; k < K; ++k) {                  // :12-14
-                sum += __ldg(ap + k) * __ldg(bp + (size_t)k * N);
+                sum += __ldg(ap + k) * __ldg(bp + k * bstride);
                 if (INJECT && fsite == k) sum ^= fmask;
             }
             Voted v = vote_u32<NC, 4>(sum, a.flags & COAST_F_MAJORITY_VOTER);
@@ -72,7 +74,7 @@ __device__ __forceinline__ void mm_u32_body(const xmr_args& a, const unsigned lo
             const bool majority = a.flags & COAST_F_MAJORITY_VOTER;
             uint32_t bad = 0;
             for (uint32_t k = 0; k < K; ++k) {
-                sum += __ldg(ap + k) * __ldg(bp + (size_t)k * N);
+                sum += __ldg(ap + k) * __ldg(bp + k * bstride);
                 bad += store_vote<NC>(sum, lane, majority);
                 if (INJECT && fsite == k) sum ^= fmask;
             }
@@ -101,3 +103,16 @@ XMR_MM_KERNEL(1, 1) XMR_MM_KERNEL(2, 1) XMR_MM_KERNEL(3, 1)
     }
 XMR_MM_GRP_KERNEL(1, 0) XMR_MM_GRP_KERNEL(2, 0) XMR_MM_GRP_KERNEL(3, 0)
 XMR_MM_GRP_KERNEL(1, 1) XMR_MM_GRP_KERNEL(2, 1) XMR_MM_GRP_KERNEL(3, 1)
+// B^T (COAST_MM_B_TRANSPOSED), uniform / batched and grouped
+#define XMR_MM_BT_KERNEL(NC, INJ)                                                                        \
+    extern "C" __global__ void __launch_bounds__(XMR_CTA_THREADS)                                        \
+    xmr_mm_u32_bt_inj##INJ##_nc##NC(const __grid_constant__ xmr_args a) { xmr::mm_u32_body<NC, INJ != 0, false, true>(a); }
+XMR_MM_BT_KERNEL(1, 0) XMR_MM_BT_KERNEL(2, 0) XMR_MM_BT_KERNEL(3, 0)
+XMR_MM_BT_KERNEL(1, 1) XMR_MM_BT_KERNEL(2, 1) XMR_MM_BT_KERNEL(3, 1)
+#define XMR_MM_BT_GRP_KERNEL(NC, INJ)                                                                    \
+    extern "C" __global__ void __launch_bounds__(XMR_CTA_THREADS)                                        \
+    xmr_mm_u32_bt_grp_inj##INJ##_nc##NC(const __grid_constant__ xmr_args a, const unsigned long long* ro) { \
+        xmr::mm_u32_body<NC, INJ != 0, true, true>(a, ro);                                               \
+    }
+XMR_MM_BT_GRP_KERNEL(1, 0) XMR_MM_BT_GRP_KERNEL(2, 0) XMR_MM_BT_GRP_KERNEL(3, 0)
+XMR_MM_BT_GRP_KERNEL(1, 1) XMR_MM_BT_GRP_KERNEL(2, 1) XMR_MM_BT_GRP_KERNEL(3, 1)

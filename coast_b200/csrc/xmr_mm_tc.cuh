@@ -39,7 +39,9 @@ template <> __device__ __forceinline__ void wgmma_u8<64>(uint32_t (&d)[32], uint
 
 // GROUPED (xmr_mm_grp.cuh): a.M products of their own row counts; the A planes hold the R rows from ro[0] (xmr_mm_grp_split_a),
 // the B^T planes the G products' B; tiles come from the group block's tile_start and rows past a product are masked.
-template <int NC, bool INJECT, bool GROUPED = false>
+// BT (COAST_MM_B_TRANSPOSED): aux holds B^T, so the planes come from xmr_mm_split_a and only the fault recompute, which reads the
+// u32 operands, differs: it reads B^T[col][k].
+template <int NC, bool INJECT, bool GROUPED = false, bool BT = false>
 __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b,
                                      const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr) {
     using G = Geom<NC>;
@@ -173,7 +175,8 @@ __device__ __forceinline__ void body(const xmr_args& a, const CUtensorMap* map_a
                                 tally.injected++;
                                 uint32_t part = 0;          // S_s = partial sum over k <= site, from the original u32 operands
                                 const uint32_t* Bp = B32 + (size_t)(GROUPED ? g : row / a.M) * a.K * a.N;    // the element's own product's B
-                                for (uint32_t k = 0; k <= f.site; ++k) part += __ldg(A32 + (size_t)row * a.K + k) * __ldg(Bp + (size_t)k * a.N + col + e);
+                                for (uint32_t k = 0; k <= f.site; ++k)
+                                    part += __ldg(A32 + (size_t)row * a.K + k) * __ldg(BT ? Bp + (size_t)(col + e) * a.K + k : Bp + (size_t)k * a.N + col + e);
                                 const uint32_t mk = 1u << f.bit, delta = (part & mk) ? (0u - mk) : mk;
                                 if (f.replica == 0) r0 += delta; else if (f.replica == 1) r1 += delta; else r2 += delta;
                             }
@@ -270,3 +273,18 @@ XMR_MMTC_KERNEL(1, 1) XMR_MMTC_KERNEL(2, 1) XMR_MMTC_KERNEL(3, 1)
     }
 XMR_MMTC_GRP_KERNEL(1, 0) XMR_MMTC_GRP_KERNEL(2, 0) XMR_MMTC_GRP_KERNEL(3, 0)
 XMR_MMTC_GRP_KERNEL(1, 1) XMR_MMTC_GRP_KERNEL(2, 1) XMR_MMTC_GRP_KERNEL(3, 1)
+// B^T (COAST_MM_B_TRANSPOSED) with a fault plan: only the lazy recompute reads B, so only these differ (the inj0 kernels serve both)
+#define XMR_MMTC_BT_KERNEL(NC)                                                                           \
+    extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
+    xmr_mm_u32_tc_bt_inj1_nc##NC(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, \
+                                 const __grid_constant__ CUtensorMap map_b) {                            \
+        xmr::mmtc::body<NC, true, false, true>(a, &map_a, &map_b);                                       \
+    }
+XMR_MMTC_BT_KERNEL(1) XMR_MMTC_BT_KERNEL(2) XMR_MMTC_BT_KERNEL(3)
+#define XMR_MMTC_BT_GRP_KERNEL(NC)                                                                       \
+    extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
+    xmr_mm_u32_tc_bt_grp_inj1_nc##NC(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, \
+                                     const __grid_constant__ CUtensorMap map_b, const unsigned long long* ro, const uint8_t* grp) { \
+        xmr::mmtc::body<NC, true, true, true>(a, &map_a, &map_b, ro, grp);                               \
+    }
+XMR_MMTC_BT_GRP_KERNEL(1) XMR_MMTC_BT_GRP_KERNEL(2) XMR_MMTC_BT_GRP_KERNEL(3)

@@ -11,6 +11,8 @@
 //
 // Grouped launches (COAST_MM_GROUPED, xmr_mm_grp.cuh): the grid is the host's bound on the tiles, each CTA finds its product and
 // tile from the group block's tile_start (surplus CTAs exit); A-row loads clamp into the product, rows past it are not stored.
+// BT (COAST_MM_B_TRANSPOSED): aux holds B^T (N rows of K per product); the B tile is loaded as 128 n-rows x 16 k, the same 512
+// uint4 per k-tile, and stored transposed into Bs[k][n] as A is, so the inner loop is unchanged.
 #pragma once
 #include "xmr_common.cuh"
 #include "xmr_mm_grp.cuh"
@@ -31,7 +33,7 @@ __device__ __forceinline__ Voted vote3(uint32_t x, uint32_t r1, uint32_t r2, int
     return v;
 }
 
-template <int NC, bool INJECT, bool GROUPED = false>
+template <int NC, bool INJECT, bool GROUPED = false, bool BT = false>
 __device__ __forceinline__ void body(const xmr_args& a, const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr) {
     extern __shared__ __align__(16) uint32_t smem[];
     uint32_t* As = smem;                        // [2][BK][BM]   (k-major: transposed on the way in)
@@ -78,9 +80,10 @@ __device__ __forceinline__ void body(const xmr_args& a, const unsigned long long
             if (q < A_V4) {                       // A: row q/4 of the tile, k-quad q%4
                 const uint32_t row = GROUPED ? min(m0 + q / 4, row_end - 1u) : m0 + q / 4;   // grouped: clamped into the product
                 pre[p] = __ldg(reinterpret_cast<const uint4*>(A + (size_t)row * K + k0 + (q % 4) * 4));
-            } else if (q < A_V4 + B_V4) {         // B: k-row (q-A)/32, column quad (q-A)%32
+            } else if (q < A_V4 + B_V4) {         // B: k-row (q-A)/32, column quad (q-A)%32; B^T: n-row (q-A)/4, k-quad (q-A)%4
                 const int b = q - A_V4;
-                pre[p] = __ldg(reinterpret_cast<const uint4*>(B + (size_t)(k0 + b / 32) * N + n0 + (b % 32) * 4));
+                if constexpr (BT) pre[p] = __ldg(reinterpret_cast<const uint4*>(B + (size_t)(n0 + b / 4) * K + k0 + (b % 4) * 4));
+                else pre[p] = __ldg(reinterpret_cast<const uint4*>(B + (size_t)(k0 + b / 32) * N + n0 + (b % 32) * 4));
             }
         }
     };
@@ -93,7 +96,12 @@ __device__ __forceinline__ void body(const xmr_args& a, const unsigned long long
                 d[0] = pre[p].x; d[BM] = pre[p].y; d[2 * BM] = pre[p].z; d[3 * BM] = pre[p].w;
             } else if (q < A_V4 + B_V4) {
                 const int b = q - A_V4;
-                *reinterpret_cast<uint4*>(Bs + buf * BK * BN + (b / 32) * BN + (b % 32) * 4) = pre[p];
+                if constexpr (BT) {
+                    uint32_t* d = Bs + buf * BK * BN + ((b % 4) * 4) * BN + b / 4;
+                    d[0] = pre[p].x; d[BN] = pre[p].y; d[2 * BN] = pre[p].z; d[3 * BN] = pre[p].w;
+                } else {
+                    *reinterpret_cast<uint4*>(Bs + buf * BK * BN + (b / 32) * BN + (b % 32) * 4) = pre[p];
+                }
             }
         }
     };
@@ -141,7 +149,8 @@ __device__ __forceinline__ void body(const xmr_args& a, const unsigned long long
             if (r == 0) tally.injected++;
             if ((int)f.replica != r) continue;
             uint32_t part = 0;                                  // S_s = sum over k <= site
-            for (uint32_t k = 0; k <= f.site; ++k) part += __ldg(A + (size_t)row * K + k) * __ldg(B + (size_t)k * N + col);
+            for (uint32_t k = 0; k <= f.site; ++k)
+                part += __ldg(A + (size_t)row * K + k) * __ldg(BT ? B + (size_t)col * K + k : B + (size_t)k * N + col);
             const uint32_t mk = 1u << f.bit;
             const uint32_t delta = (part & mk) ? (0u - mk) : mk;  // (S ^ mk) - S
 #pragma unroll
@@ -198,3 +207,16 @@ XMR_MMT_KERNEL(1, 1) XMR_MMT_KERNEL(2, 1) XMR_MMT_KERNEL(3, 1)
     }
 XMR_MMT_GRP_KERNEL(1, 0) XMR_MMT_GRP_KERNEL(2, 0) XMR_MMT_GRP_KERNEL(3, 0)
 XMR_MMT_GRP_KERNEL(1, 1) XMR_MMT_GRP_KERNEL(2, 1) XMR_MMT_GRP_KERNEL(3, 1)
+// B^T (COAST_MM_B_TRANSPOSED), uniform / batched and grouped
+#define XMR_MMT_BT_KERNEL(NC, INJ)                                                                       \
+    extern "C" __global__ void __launch_bounds__(xmr_mmt_threads(NC))                                    \
+    xmr_mm_u32_tiled_bt_inj##INJ##_nc##NC(const __grid_constant__ xmr_args a) { xmr::mmt::body<NC, INJ != 0, false, true>(a); }
+XMR_MMT_BT_KERNEL(1, 0) XMR_MMT_BT_KERNEL(2, 0) XMR_MMT_BT_KERNEL(3, 0)
+XMR_MMT_BT_KERNEL(1, 1) XMR_MMT_BT_KERNEL(2, 1) XMR_MMT_BT_KERNEL(3, 1)
+#define XMR_MMT_BT_GRP_KERNEL(NC, INJ)                                                                   \
+    extern "C" __global__ void __launch_bounds__(xmr_mmt_threads(NC))                                    \
+    xmr_mm_u32_tiled_bt_grp_inj##INJ##_nc##NC(const __grid_constant__ xmr_args a, const unsigned long long* ro, const uint8_t* grp) { \
+        xmr::mmt::body<NC, INJ != 0, true, true>(a, ro, grp);                                            \
+    }
+XMR_MMT_BT_GRP_KERNEL(1, 0) XMR_MMT_BT_GRP_KERNEL(2, 0) XMR_MMT_BT_GRP_KERNEL(3, 0)
+XMR_MMT_BT_GRP_KERNEL(1, 1) XMR_MMT_BT_GRP_KERNEL(2, 1) XMR_MMT_BT_GRP_KERNEL(3, 1)

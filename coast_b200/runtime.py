@@ -21,6 +21,7 @@ AES_DECRYPT, AES_KEY_PER_UNIT, AES_KEY_WRITEBACK = 1, 2, 4
 UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 / QSORT batches: aux = n_units + 1 u64 byte offsets into inp
 MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32 / GEMM_BF16: n_units = batch*M*N, inp / aux / out hold batch A / B / C
 MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32 / GEMM_BF16: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
+MM_B_TRANSPOSED = COAST_MM_B_TRANSPOSED = 0x80000  # MM_U32 / GEMM_TF32 / GEMM_BF16: aux holds B^T, N x K per product (nn.Linear.weight)
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 

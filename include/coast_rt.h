@@ -166,6 +166,7 @@ typedef struct coast_fault_plan {
  *            sum of the exact bf16 x bf16 products.  M%128 == N%128 == K%64 == 0 (grouped: N and K only), buffers 16-byte
  *            aligned.  A unit is one C element with one fault site of width 32, as GEMM_TF32.  COAST_MM_BATCHED and
  *            COAST_MM_GROUPED as below; the element offsets there count 2-byte elements in d_in and d_aux, 4-byte ones in d_out.
+ *   MM_U32 / GEMM_TF32 / GEMM_BF16 with COAST_MM_B_TRANSPOSED: aux: B^T, N x K row-major per product (see below).
  *   QSORT    in : n_units x unit_bytes, arrays of L = unit_bytes/4 int32 (L <= 1024)   out: the sorted arrays
  *   CHSTONE_SHA in : n_units x unit_bytes stream bytes (unit_bytes a multiple of 64, 64 <= unit_bytes < 2^29)
  *            out: n_units x 5 uint32 = sha_info_digest[5] (sha.h:38)
@@ -201,7 +202,8 @@ typedef struct coast_fault_plan {
  * minimum first_fault_unit.  Fault plans stay keyed by the global unit index (a TABLE plan has n_units entries), and the
  * in-loop store votes keep their meaning (K + 1 votes per unit on the plain kernel).  Each path's shape rules apply to the
  * per-matrix M, N and K; a TF32 / BF16 CTA pair needs the per-matrix M to be a multiple of 256.  COAST_ERR_BAD_ARG for the bit on
- * any other kernel, for n_units zero or not a multiple of M*N, and for batch*M or batch*N (GEMM_BF16: batch*K) at or above 2^31.  Without the
+ * any other kernel, for n_units zero or not a multiple of M*N, and for batch*M or batch*N (GEMM_BF16 without COAST_MM_B_TRANSPOSED:
+ * batch*K) at or above 2^31.  Without the
  * bit n_units must be M*N; with batch = 1 the launch is identical to an unbatched one.  A shard takes whole matrices
  * [b_lo, b_hi): the three pointers and unit_base offset as above, n_units = (b_hi - b_lo) x M x N. */
 #define COAST_MM_BATCHED        0x20000u
@@ -217,10 +219,21 @@ typedef struct coast_fault_plan {
  * [ro[0], ro[0] + R] and count a decreasing pair as zero rows, so a malformed table never reads or writes outside
  * [ro[0], ro[0] + R) rows of the buffers; coast_run_host (and Runtime.run) refuse a table that decreases or whose last offset is
  * not ro[0] + R.  COAST_ERR_BAD_ARG for the bit on any other kernel or with COAST_MM_BATCHED or COAST_UNIT_OFFSETS, for G = 0
- * or above 2^20, for n_units not a multiple of N, for R or G*N (GEMM_BF16: G*K) at or above 2^31, and for a null or misaligned d_rows.  A shard
+ * or above 2^20, for n_units not a multiple of N, for R or G*N (GEMM_BF16 without COAST_MM_B_TRANSPOSED: G*K) at or above 2^31,
+ * and for a null or misaligned d_rows.  A shard
  * takes whole products [g_lo, g_hi): d_rows + g_lo with the same d_in and d_out, d_aux + g_lo*K*N, M = g_hi - g_lo,
  * n_units = (ro[g_hi] - ro[g_lo])*N and unit_base + (ro[g_lo] - ro[0])*N. */
 #define COAST_MM_GROUPED        0x40000u
+/* Transposed B (MM_U32, GEMM_TF32 and GEMM_BF16 only), the layout of a linear layer's weight: with COAST_MM_B_TRANSPOSED in
+ * `mode`, d_aux holds B^T, each product's B stored as N rows of K elements, row-major: element (k, n) of product p is at
+ * d_aux[p*N*K + n*K + k].  It combines with COAST_MM_BATCHED and COAST_MM_GROUPED; the product offsets into d_aux (p*K*N
+ * elements) and the shard rules stay as documented there.  The launch equals the same launch without the bit whose d_aux holds
+ * every product's B = (B^T)^T: the same output bytes, summed counters, minimum first_fault_unit and d_status bytes.  Fault sites,
+ * their widths, TABLE plans and the in-loop store votes are unchanged.  B^T is read in place: GEMM_TF32 runs no transposing
+ * pre-pass and needs no B^T scratch, GEMM_BF16 reads B^T K-major, MM_U32's limb path splits B^T like A.  Each path's shape
+ * rules are unchanged; the 2^31 bound on B's stacked rows is on batch*N (grouped: G*N) for every kernel with the bit.
+ * COAST_ERR_BAD_ARG for the bit on any other kernel. */
+#define COAST_MM_B_TRANSPOSED   0x80000u
 #define COAST_AES_DECRYPT       0x1u
 #define COAST_AES_KEY_PER_UNIT  0x2u
 #define COAST_AES_KEY_WRITEBACK 0x4u   /* with KEY_PER_UNIT: store what aes_enc_dec() leaves in key[] (TI_aes_128.c:214-221 mutates
