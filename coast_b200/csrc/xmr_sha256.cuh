@@ -36,9 +36,24 @@ constexpr uint32_t SHA_SITES_PER_BLOCK = 536u;   // 16 m[] + 64 rounds x 8 worki
 __device__ __forceinline__ uint32_t rotr(uint32_t v, int n) { return __funnelshift_r(v, v, n); }
 __device__ __forceinline__ uint32_t bswap(uint32_t v) { return __byte_perm(v, 0u, 0x0123u); }
 
+// The compression is bound by ALU-pipe issue: its rotations, XORs and additions all go to the ALU pipe, which takes one warp
+// instruction every 2 cycles per SM sub-partition, while the IMAD pipe beside it idles.  Additions are issued there instead as
+// x * 1 + y (DESIGN.md §5.0).  The 1 lives in the constant bank: IMAD reads it as a c[][] operand, costing no register, and
+// ptxas, which cannot know its value, cannot turn the product back into an IADD3.  The shifts and rotations stay on the ALU
+// pipe: their multiply forms need IMAD.HI, which runs at half rate.
+__constant__ uint32_t sha_one = 1u;
+
+__device__ __forceinline__ uint32_t add_imad(uint32_t x, uint32_t y) {
+    uint32_t d;
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(x), "r"(sha_one), "r"(y));
+    return d;
+}
+
 // One compression.  m[0..15] holds the big-endian-packed block (:34-40) and is used as the rolling
 // 16-word schedule window (:42-58).  `fs`/`fmask`: fault site within THIS block (>= 536 = none).
-template <bool INJECT>
+// CONST_M: m[] holds compile-time constants (the padding block of a 64-byte message); its schedule is written with plain
+// additions so that it folds away, which add_imad would prevent.
+template <bool INJECT, bool CONST_M = false>
 __device__ __forceinline__ void sha_compress(uint32_t (&st)[8], uint32_t (&m)[16], uint32_t fs, uint32_t fmask) {
     if (INJECT && fs < 16u) {
 #pragma unroll
@@ -54,7 +69,8 @@ __device__ __forceinline__ void sha_compress(uint32_t (&st)[8], uint32_t (&m)[16
             uint32_t w2 = m[(t - 2) & 15], w15 = m[(t - 15) & 15];
             uint32_t s1 = rotr(w2, 17) ^ rotr(w2, 19) ^ (w2 >> 10);
             uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ (w15 >> 3);
-            m[t & 15] = s1 + m[(t - 7) & 15] + s0 + m[t & 15];
+            m[t & 15] = CONST_M ? s1 + m[(t - 7) & 15] + s0 + m[t & 15]
+                                : add_imad(s1, add_imad(s0, add_imad(m[(t - 7) & 15], m[t & 15])));
         }
         if (INJECT && fround && ft == (uint32_t)t) {
             a ^= fv == 0 ? fmask : 0u; b ^= fv == 1 ? fmask : 0u; c ^= fv == 2 ? fmask : 0u; d ^= fv == 3 ? fmask : 0u;
@@ -64,9 +80,9 @@ __device__ __forceinline__ void sha_compress(uint32_t (&st)[8], uint32_t (&m)[16
         uint32_t ep1 = rotr(e, 6) ^ rotr(e, 11) ^ rotr(e, 25);  // :73-75
         uint32_t ch = (e & f) ^ (~e & g);                       // :76
         uint32_t maj = (a & b) ^ (a & c) ^ (b & c);             // :77
-        uint32_t t1 = h + ep1 + ch + sha_k(t) + m[t & 15];      // :78
-        uint32_t t2 = ep0 + maj;                                // :79
-        h = g; g = f; f = e; e = d + t1; d = c; c = b; b = a; a = t1 + t2;   // :80-87
+        uint32_t t1 = add_imad(ep1, add_imad(ch, add_imad(h, sha_k(t) + m[t & 15])));   // :78
+        uint32_t t2 = add_imad(ep0, maj);                       // :79
+        h = g; g = f; f = e; e = add_imad(d, t1); d = c; c = b; b = a; a = add_imad(t1, t2);   // :80-87
     }
     st[0] += a; st[1] += b; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;   // :90-97
     if (INJECT && fs >= 528u && fs < 536u) {
@@ -216,7 +232,7 @@ __device__ __forceinline__ void sha256_b64_body(const xmr_args& a, const CUtenso
 #pragma unroll
         for (int i = 0; i < 16; ++i) m[i] = 0u;
         m[0] = 0x80000000u; m[15] = 512u;
-        sha_compress<INJECT>(st, m, fs1, fmask);              // :164
+        sha_compress<INJECT, true>(st, m, fs1, fmask);        // :164
 
         sha_vote_store<NC>(st, static_cast<uint8_t*>(a.out), local, gunit, valid, lane, a.flags, tally);
     }
@@ -379,7 +395,7 @@ __device__ __forceinline__ void sha256_b64_seg_body(const xmr_args& a, const CUt
 #pragma unroll
         for (int i = 0; i < 16; ++i) m[i] = 0u;
         m[0] = 0x80000000u; m[15] = 512u;
-        sha_compress<INJECT>(st, m, fs1, fmask);
+        sha_compress<INJECT, true>(st, m, fs1, fmask);
 
         uint32_t* ex = exch + ((it & 1u) * SEG_GROUPS + g) * SEG_EXCH_WORDS;
         if (r > 0) {
