@@ -38,7 +38,7 @@ __device__ __forceinline__ uint32_t bswap(uint32_t v) { return __byte_perm(v, 0u
 
 // The compression is bound by ALU-pipe issue: its rotations, XORs and additions all go to the ALU pipe, which takes one warp
 // instruction every 2 cycles per SM sub-partition, while the IMAD pipe beside it idles.  Additions are issued there instead as
-// x * 1 + y (DESIGN.md §5.0).  The 1 lives in the constant bank: IMAD reads it as a c[][] operand, costing no register, and
+// x * 1 + y (DESIGN.md §5.0).  The 1 lives in the constant bank: IMAD reads it from a uniform register, costing no register, and
 // ptxas, which cannot know its value, cannot turn the product back into an IADD3.  The shifts and rotations stay on the ALU
 // pipe: their multiply forms need IMAD.HI, which runs at half rate.
 __constant__ uint32_t sha_one = 1u;
@@ -46,6 +46,19 @@ __constant__ uint32_t sha_one = 1u;
 __device__ __forceinline__ uint32_t add_imad(uint32_t x, uint32_t y) {
     uint32_t d;
     asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(x), "r"(sha_one), "r"(y));
+    return d;
+}
+
+// x + k for a compile-time k (the padding block's K + W), as IMAD one, k, x.  The 1 has to be in a per-thread register here
+// (an IMAD with an immediate takes no constant-bank or uniform operand besides it), so it is a constant of its own: were it
+// sha_one, ptxas would read that register in every add_imad as well, a third register source per IMAD where the uniform
+// register serves, and the kernel runs 9% slower so (DESIGN.md §5.0).  The alignment keeps it out of sha_one's 8 bytes, which
+// ptxas would otherwise fetch together with one LDC.64 into registers.
+__constant__ __align__(16) uint32_t sha_one_imm = 1u;
+
+__device__ __forceinline__ uint32_t add_imad_imm(uint32_t x, uint32_t k) {
+    uint32_t d;
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(sha_one_imm), "r"(k), "r"(x));
     return d;
 }
 
@@ -80,7 +93,8 @@ __device__ __forceinline__ void sha_compress(uint32_t (&st)[8], uint32_t (&m)[16
         uint32_t ep1 = rotr(e, 6) ^ rotr(e, 11) ^ rotr(e, 25);  // :73-75
         uint32_t ch = (e & f) ^ (~e & g);                       // :76
         uint32_t maj = (a & b) ^ (a & c) ^ (b & c);             // :77
-        uint32_t t1 = add_imad(ep1, add_imad(ch, add_imad(h, sha_k(t) + m[t & 15])));   // :78
+        const uint32_t hkw = CONST_M ? add_imad_imm(h, sha_k(t) + m[t & 15]) : add_imad(h, sha_k(t) + m[t & 15]);   // K + W
+        uint32_t t1 = add_imad(ep1, add_imad(ch, hkw));         // :78
         uint32_t t2 = add_imad(ep0, maj);                       // :79
         h = g; g = f; f = e; e = add_imad(d, t1); d = c; c = b; b = a; a = add_imad(t1, t2);   // :80-87
     }

@@ -6,9 +6,11 @@
    through the driver API (cuModuleLoadData, as coast_rt.c does) and times each stream with clock64().  Every stream
    is 8 independent dependency chains per thread, 8 warps per sub-partition, so issue, not latency, bounds it.
    The loop body's SASS is read back: the report gives the opcodes that really ran, not the ones the source asked for.
+   The viadd+shf mix decides which pipe VIADD issues on (viadd_pipe).
 2. Runs `bench.py --workload sha256` and sets its roofline.kernel_ms (at the delivered SM clock) against the static
    ALU floor of xmr_sha256_b64_seg_nc3_inj0: ALU-pipe instructions in its SASS x warps / sub-partitions / measured
-   ALU rate.  Above 1.25x the floor the ALU pipe is not what bounds the kernel.
+   ALU rate, with VIADD on the pipe measured for it; the floors with and without VIADD on the ALU pipe are reported
+   beside it.  Above 1.25x the floor the ALU pipe is not what bounds the kernel.
 3. Times the other SHA-256 kernels (interleaved 64-byte NC 1/2/3, general length) with CUDA events.
 
 Rates are warp instructions per clock per SM sub-partition (4 per SM).  The card's name and power limit are read in
@@ -43,6 +45,17 @@ def pipe_of(op: str) -> str:
     return "other"
 
 
+def viadd_pipe(rates: dict) -> str:
+    """'alu' or 'imad': the pipe VIADD issues on, from the measured viadd+shf mix.  Each pipe takes one warp instruction
+    every 2 cycles; a VIADD + SHF stream reaches about 1 per cycle only if the two go to different pipes."""
+    return "imad" if rates["viadd_shf_1_1"]["warp_inst_per_clk_per_smsp"]["all"] > 0.75 else "alu"
+
+
+def pipe_of_measured(op: str, viadd: str) -> str:
+    """pipe_of, with VIADD (which pipe_of leaves under "other") on the pipe the probe measured for it"""
+    return viadd if op.split(".")[0] == "VIADD" else pipe_of(op)
+
+
 # --- 1. the probe cubin ------------------------------------------------------------------------------------------------
 # Each op updates chain x[i] from itself and its neighbour x[(i+1)&7] (so ptxas cannot fuse a chain into fewer
 # instructions) and from values it cannot know (loaded from memory).  Multipliers come from the constant bank, as in
@@ -61,6 +74,12 @@ PROBE_OPS = {
                      'X = (uint32_t)w ^ (uint32_t)(w >> 32); }', "IMAD.WIDE"),
     "viadd":        ('X = X + Y + 0x1234567u;', "VIADD"),
 }
+# Ops that only run inside a mix: alone, ptxas folds a chain of them into one instruction per loop trip.  An immediate
+# add is a VIADD only where ptxas chooses it: next to a shift it emits VIADD, next to an IMAD mostly IADD3 (the report
+# prints the opcodes that ran).
+MIX_OPS = {
+    "viadd_imm":    ('X = X + 0x1234567u;', "VIADD"),
+}
 MIXES = {  # ALU form : IMAD form, in the ratio given (per chain, back to back)
     "shf+imad_const 1:1": (["shf_r_w", "imad_const"]),
     "shf+imad_hi 1:1":    (["shf_r_w", "imad_hi"]),
@@ -68,6 +87,10 @@ MIXES = {  # ALU form : IMAD form, in the ratio given (per chain, back to back)
     "shf+imad_wide 1:1":  (["shf_r_w", "imad_wide"]),
     "shf+lop3+imad_const 2:1": (["shf_r_w", "lop3", "imad_const"]),
     "shf+lop3+imad_hi 2:1":    (["shf_r_w", "lop3", "imad_hi"]),
+    # which pipe VIADD issues on: it co-issues with the one it does not share.  The shift is the variable-count
+    # SHF.R.U32.HI because ptxas fuses a funnel shift and an immediate add into one LEA.HI.
+    "viadd+shf 1:1":      (["shf_r_u32_hi", "viadd_imm"]),
+    "viadd+imad 1:1":     (["imad_const", "viadd_imm"]),
 }
 UNROLL = 8          # ops per chain per loop trip (x 8 chains = 64 per form per trip)
 
@@ -77,7 +100,7 @@ def _kernel_src(name: str, forms: list[str]) -> str:
     for _ in range(UNROLL):
         for i in range(8):
             for f in forms:
-                body.append(PROBE_OPS[f][0].replace("X", f"x{i}").replace("Y", f"x{(i + 1) & 7}"))
+                body.append({**PROBE_OPS, **MIX_OPS}[f][0].replace("X", f"x{i}").replace("Y", f"x{(i + 1) & 7}"))
     return f"""
 extern "C" __global__ void __launch_bounds__(256) probe_{name}(const uint32_t* in, uint32_t* out, long long* cyc, int iters) {{
     const uint32_t mr = in[0], s = in[1], v = in[2] + threadIdx.x;
@@ -242,16 +265,19 @@ def measure_rates(drv: Driver, cubin: str, kernels: dict[str, list[str]], iters:
 
 
 # --- 2. the headline kernel against its ALU floor ----------------------------------------------------------------------
-def kernel_pipe_counts(fun: str = SEG_KERNEL) -> dict:
+def kernel_pipe_counts(fun: str = SEG_KERNEL, viadd: str = "alu") -> dict:
     cubin = os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")
     hist = histogram(sass_ops(cubin, fun))
     pipes = {"alu": 0, "imad": 0, "other": 0}
+    measured = dict(pipes)
     for op, n in hist.items():
         pipes[pipe_of(op)] += n
-    return {"function": fun, "pipes": pipes, "top": dict(list(hist.items())[:12])}
+        measured[pipe_of_measured(op, viadd)] += n
+    return {"function": fun, "pipes": pipes, "pipes_viadd_measured": measured, "viadd_pipe": viadd,
+            "viadd": sum(n for op, n in hist.items() if op.split(".")[0] == "VIADD"), "top": dict(list(hist.items())[:12])}
 
 
-def headline(alu_rate: float, sms: int) -> dict:
+def headline(alu_rate: float, sms: int, viadd: str) -> dict:
     cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--workload", "sha256", "--steps", "50", "--warmup", "10",
            "--no-cpu-baseline"]
     out = subprocess.run(cmd, capture_output=True, text=True, cwd=ROOT)
@@ -259,13 +285,16 @@ def headline(alu_rate: float, sms: int) -> dict:
         raise RuntimeError(out.stdout[-2000:] + out.stderr[-2000:])
     line = json.loads([ln for ln in out.stdout.splitlines() if ln.startswith("{")][-1])
     k_ms, mhz = line["roofline"]["kernel_ms"], line["clocks"]["sm_mhz_in_timed_region"] or line["clocks"]["sm_mhz"]
-    counts = kernel_pipe_counts()
+    counts = kernel_pipe_counts(viadd=viadd)
     warps = (1 << 20) // 32 * 3
-    floor_cycles = counts["pipes"]["alu"] * warps / (sms * 4) / alu_rate
-    floor_ms = floor_cycles / (mhz * 1e3)
+    floor_ms = lambda n_alu: n_alu * warps / (sms * 4) / alu_rate / (mhz * 1e3)
+    without = floor_ms(counts["pipes"]["alu"])
+    with_viadd = floor_ms(counts["pipes"]["alu"] + counts["viadd"])
+    floor = floor_ms(counts["pipes_viadd_measured"]["alu"])
     return {"value_mbs": line["value"], "kernel_ms": k_ms, "sm_mhz_in_timed_region": mhz, "sass": counts,
-            "alu_floor_ms": round(floor_ms, 5), "kernel_over_alu_floor": round(k_ms / floor_ms, 3),
-            "gate": "ALU-bound" if k_ms <= 1.25 * floor_ms else "not ALU-bound (above 1.25x the ALU floor)"}
+            "alu_floor_ms_without_viadd": round(without, 5), "alu_floor_ms_with_viadd": round(with_viadd, 5),
+            "alu_floor_ms": round(floor, 5), "kernel_over_alu_floor": round(k_ms / floor, 3),
+            "gate": "ALU-bound" if k_ms <= 1.25 * floor else "not ALU-bound (above 1.25x the ALU floor)"}
 
 
 # --- 3. the other SHA-256 kernels --------------------------------------------------------------------------------------
@@ -311,8 +340,10 @@ def main():
         cubin, kernels = build_probe(tmp)
         report["rates"] = measure_rates(drv, cubin, kernels)
     alu_rate = report["rates"]["shf_r_w"]["warp_inst_per_clk_per_smsp"]["alu"]
+    report["viadd_pipe"] = viadd_pipe(report["rates"])
+    print("VIADD issues on the", report["viadd_pipe"], "pipe", flush=True)
     if not args.skip_bench:
-        report["headline"] = headline(alu_rate, card["sms"])
+        report["headline"] = headline(alu_rate, card["sms"], report["viadd_pipe"])
         print("headline:", json.dumps(report["headline"]), flush=True)
     if not args.skip_sha:
         report["other_sha_kernels"] = other_sha_kernels()
