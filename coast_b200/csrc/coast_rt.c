@@ -497,8 +497,21 @@ static int encode_map(const map_desc* want, CUdeviceptr scratch, int cached, CUt
     return COAST_OK;
 }
 
-/* What kernel selection decides about a launch; run_plan() does the rest. */
+/* The shape of a matmul launch, read off its descriptor once.  Batched (COAST_MM_BATCHED): the stacked A and C are one
+ * (batch*M)-row matrix and only B changes from one product to the next.  Grouped (COAST_MM_GROUPED): M is the product count G,
+ * the stacked A and C are one R-row matrix from row ro[0] (R = n_units / N) and B is G matrices end to end. */
 typedef struct {
+    unsigned es;                  /* bytes per element of A and B; C elements are 4 bytes */
+    int batched, grouped, bt;     /* the mode bits */
+    uint64_t P;                   /* products: 1, the batch or G */
+    uint64_t rows;                /* stacked rows of A and C: batch*M or R */
+    int b_rows_k;                 /* B's map has K rows per product (GEMM_BF16 reading B in place); every B^T map has N */
+    uint32_t b_rows;              /* rows per product of B's map */
+} mm_shape;
+
+/* What kernel selection decides about a launch; run_plan() does the rest. */
+typedef struct launch_plan launch_plan;
+struct launch_plan {
     char name[64];
     unsigned block, smem;
     uint64_t ctas;                /* CTAs the work needs (0: one warp per 32/nc units, the lane-interleaved kernels) */
@@ -509,13 +522,13 @@ typedef struct {
     size_t scratch;               /* stream-ordered scratch for the pre-pass and the maps */
     size_t scratch_per_cta;       /* plus this much per CTA of the grid, handed to the kernel as xmr_args.aux */
     int scratch_as_aux;           /* hand the scratch to the kernel as xmr_args.aux even without per-CTA scratch */
-    int (*prepass)(const coast_launch_desc* d, CUdeviceptr scratch, CUstream s);
+    int (*prepass)(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr scratch, CUstream s);
+    mm_shape mm;                  /* the matmuls */
     /* grouped matmuls: the kernel takes the row offsets and the group block (at grp_off in scratch) after its maps; the scan
      * pre-pass cuts the products into tiles of grp_tm rows, grp_tiles_n per tile row (grp_tm 0: no scan, the plain kernel) */
-    int grouped;
     size_t grp_off;
     unsigned grp_tm, grp_tiles_n;
-} launch_plan;
+};
 
 /* The TMA-ring kernels: tiles of tile_rows units of row_bytes each, loaded as equal boxes of at most 256 rows.  With a row
  * pack shift p the same dense bytes are described as rows 2^p times longer. */
@@ -544,107 +557,105 @@ static void plan_wg_map(map_desc* m, CUtensorMapDataType dtype, unsigned esize, 
     m->swz = CU_TENSOR_MAP_SWIZZLE_128B; m->l2 = CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
 }
 
-/* Pre-passes of the wgmma kernels: TF32 wgmma reads both operands K-major, so B (K x N, row-major) is transposed into scratch;
- * the limb kernel splits A and B into u8 limb planes ([plane][M][K] and, transposed, [plane][N][K]). */
-/* Batched matmuls (COAST_MM_BATCHED): the products in the launch (1 without the bit), and the checks shared by coast_launch
- * and coast_run_host.  The stacked A and C are one (batch*M)-row matrix; only B changes from one product to the next. */
-static uint64_t mm_batch(const coast_launch_desc* d) {
-    return (d->mode & COAST_MM_BATCHED) ? d->n_units / ((uint64_t)d->M * d->N) : 1u;
+/* rows of the stacked operands are tensor-map coordinates: A's rows and B's P * b_rows */
+static int mm_rows_fit(const mm_shape* m) { return m->rows < (1ull << 31) && m->P * m->b_rows < (1ull << 31); }
+
+/* a matmul mode bit on another kernel */
+static int mm_bit_refused(const coast_launch_desc* d, uint32_t bit) {
+    if (!(d->mode & bit) || is_matmul(d->kernel)) return COAST_OK;
+    const char* what = bit == COAST_MM_BATCHED ? "COAST_MM_BATCHED: batched products exist"
+                     : bit == COAST_MM_GROUPED ? "COAST_MM_GROUPED: grouped products exist" : "COAST_MM_B_TRANSPOSED: a transposed B exists";
+    return fail(COAST_ERR_BAD_ARG, "%s for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", what, d->kernel);
 }
-/* B's tensor map has K rows per product only for GEMM_BF16 reading B in place; every B^T map (scratch or the caller's) has N */
-static int mm_b_rows_k(const coast_launch_desc* d) {
-    return d->kernel == COAST_K_GEMM_BF16 && !(d->mode & COAST_MM_B_TRANSPOSED);
-}
-static int b_transposed_check(const coast_launch_desc* d) {
-    if ((d->mode & COAST_MM_B_TRANSPOSED) && !is_matmul(d->kernel))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_B_TRANSPOSED: a transposed B exists for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", d->kernel);
+/* The checks shared by coast_launch and coast_run_host: a matmul mode bit on another kernel, then the shape of a batch or of
+ * groups.  Fills *m for the matmul kernels. */
+static int mm_check(const coast_launch_desc* d, mm_shape* m) {
+    int rc;
+    memset(m, 0, sizeof *m);
+    if ((rc = mm_bit_refused(d, COAST_MM_BATCHED)) || (rc = mm_bit_refused(d, COAST_MM_GROUPED)) ||
+        (rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)))
+        return rc;
+    if (!is_matmul(d->kernel)) return COAST_OK;
+    m->es = KINFO[d->kernel].mm_elem;
+    m->batched = (d->mode & COAST_MM_BATCHED) != 0;
+    m->grouped = (d->mode & COAST_MM_GROUPED) != 0;
+    m->bt = (d->mode & COAST_MM_B_TRANSPOSED) != 0;
+    m->b_rows_k = d->kernel == COAST_K_GEMM_BF16 && !m->bt;
+    m->b_rows = m->b_rows_k ? d->K : d->N;
+    const char bc = m->b_rows_k ? 'K' : 'N';
+    m->P = 1; m->rows = d->M;
+    if (m->batched) {
+        if (!d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: M, N and K are the shape of one product and must be nonzero");
+        const uint64_t mn = (uint64_t)d->M * d->N;
+        if (!d->n_units || d->n_units % mn)
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: n_units must be a nonzero multiple of M*N = %llu (got %llu)",
+                        (unsigned long long)mn, (unsigned long long)d->n_units);
+        m->P = d->n_units / mn; m->rows = m->P * d->M;
+        if (!mm_rows_fit(m))
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batch*M and batch*%c must be below 2^31 (batch %llu, M %u, %c %u)",
+                        bc, (unsigned long long)m->P, d->M, bc, m->b_rows);
+    }
+    if (m->grouped) {
+        if (d->mode & (COAST_MM_BATCHED | COAST_UNIT_OFFSETS))
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: cannot be combined with COAST_MM_BATCHED or COAST_UNIT_OFFSETS");
+        if (!d->M || d->M > XMR_MM_GRP_MAX)
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: M is the product count G, 1..%u (got %u)", XMR_MM_GRP_MAX, d->M);
+        if (!d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: N and K are shared by every product and must be nonzero");
+        if (d->n_units % d->N)
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: n_units must be a multiple of N = %u (R rows x N; got %llu)", d->N,
+                        (unsigned long long)d->n_units);
+        m->P = d->M; m->rows = d->n_units / d->N;
+        if (!mm_rows_fit(m))
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the rows R and G*%c must be below 2^31 (R %llu, G %u, %c %u)",
+                        bc, (unsigned long long)m->rows, d->M, bc, m->b_rows);
+        if (!d->d_rows || (((uintptr_t)d->d_rows) & 7u))
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: d_rows must point to G + 1 8-byte aligned uint64_t row offsets");
+    }
     return COAST_OK;
 }
-static int batched_check(const coast_launch_desc* d) {
-    if (!is_matmul(d->kernel))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batched products exist for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", d->kernel);
-    if (!d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: M, N and K are the shape of one product and must be nonzero");
-    const uint64_t mn = (uint64_t)d->M * d->N;
-    if (!d->n_units || d->n_units % mn)
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: n_units must be a nonzero multiple of M*N = %llu (got %llu)",
-                    (unsigned long long)mn, (unsigned long long)d->n_units);
-    const uint64_t batch = d->n_units / mn;
-    /* the rows of the stacked operands are tensor-map coordinates: A's batch*M, and B^T's batch*N or, for GEMM_BF16 with B in place
-     * (no COAST_MM_B_TRANSPOSED), B's batch*K */
-    const int b_rows_k = mm_b_rows_k(d);
-    if (batch * d->M >= (1ull << 31) || batch * (b_rows_k ? d->K : d->N) >= (1ull << 31))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_BATCHED: batch*M and batch*%c must be below 2^31 (batch %llu, M %u, %c %u)",
-                    b_rows_k ? 'K' : 'N', (unsigned long long)batch, d->M, b_rows_k ? 'K' : 'N', b_rows_k ? d->K : d->N);
-    return COAST_OK;
+/* tiles of bm rows over the stacked rows; a grouped launch's products start anywhere, so it gets one more per product (a bound) */
+static uint64_t mm_row_tiles(const mm_shape* m, unsigned bm) { return m->rows / bm + (m->grouped ? m->P : 0); }
+
+/* A matmul kernel's name: stem, path variant, [_bt], [_grp], then _nc<n>_inj<i> for the kernels that came before batched,
+ * grouped, BF16 and transposed-B launches and _inj<i>_nc<n> for the others */
+static void mm_kernel_name(char* name, const char* stem, const char* variant, int bt, int grouped, int bf16, uint32_t nc, int inj) {
+    if (bt || grouped || bf16) snprintf(name, 64, "%s%s%s%s_inj%d_nc%u", stem, variant, bt ? "_bt" : "", grouped ? "_grp" : "", inj, nc);
+    else snprintf(name, 64, "%s%s_nc%u_inj%d", stem, variant, nc, inj);
 }
 
 /* Pre-passes of the wgmma kernels: TF32 wgmma reads both operands K-major, so B (K x N, row-major) is transposed into scratch;
- * the limb kernel splits A and B into u8 limb planes ([plane][M][K] and, transposed, [plane][N][K]).  A batch's B matrices
- * become one stacked (batch*N) x K operand, its A matrices are already one (batch*M) x K matrix. */
-static int prepass_transpose_b(const coast_launch_desc* d, CUdeviceptr bt, CUstream s) {
-    const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N, nb = (unsigned)mm_batch(d);
+ * the limb kernel splits A and B into u8 limb planes ([plane][rows][K] and, transposed, [plane][P N][K]).  The products' B
+ * matrices become one stacked (P N) x K operand; their A matrices already are one matrix. */
+static int prepass_transpose_b(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr bt, CUstream s) {
+    const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N, nb = (unsigned)L->mm.P;
     void* params[] = { &B, &bt, &k32, &n32, &nb };
     return launch_small("xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
 }
-/* The B^T planes [plane][b N + n][k]: split_bt transposes B; a caller's B^T (COAST_MM_B_TRANSPOSED) already has that row order,
- * so the streaming split of A makes them from its (batch N) rows of K. */
-static int prepass_split_b(const coast_launch_desc* d, CUdeviceptr pb, unsigned batch, CUstream s) {
-    const void* B = d->d_aux;
-    if (d->mode & COAST_MM_B_TRANSPOSED) {
-        unsigned long long rows = (unsigned long long)batch * d->N, K = d->K;
-        void* params[] = { &B, &pb, &rows, &K };
+/* A's rows (groups: the R rows from row ro[0]), then the B^T planes [plane][p N + n][k]: split_bt transposes B; a caller's B^T
+ * (COAST_MM_B_TRANSPOSED) already has that row order, so the streaming split of A makes them from its (P N) rows of K. */
+static int prepass_split_limbs(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr pa, CUstream s) {
+    unsigned long long rows = L->mm.rows, K = d->K; const void* A = d->d_in; const void* ro = d->d_rows; const void* B = d->d_aux;
+    void* params_a[] = { &A, &pa, &rows, &K };
+    void* params_grp[] = { &ro, &A, &pa, &rows, &K };
+    int rc = launch_small(L->mm.grouped ? "xmr_mm_grp_split_a" : "xmr_mm_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS,
+                          L->mm.grouped ? params_grp : params_a, s);
+    if (rc) return rc;
+    CUdeviceptr pb = pa + (size_t)rows * d->K * 4u;
+    if (L->mm.bt) {
+        unsigned long long b_rows = L->mm.P * d->N;
+        void* params[] = { &B, &pb, &b_rows, &K };
         return launch_small("xmr_mm_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
     }
-    unsigned int k32 = d->K, n32 = d->N, nb = batch;
+    unsigned int k32 = d->K, n32 = d->N, nb = (unsigned)L->mm.P;
     void* params_b[] = { &B, &pb, &k32, &n32, &nb };
     return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
-}
-static int prepass_split_limbs(const coast_launch_desc* d, CUdeviceptr pa, CUstream s) {
-    unsigned long long rows = mm_batch(d) * d->M, K = d->K; const void* A = d->d_in;
-    void* params_a[] = { &A, &pa, &rows, &K };
-    int rc = launch_small("xmr_mm_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_a, s); if (rc) return rc;
-    return prepass_split_b(d, pa + (size_t)rows * d->K * 4u, (unsigned)mm_batch(d), s);
-}
-
-/* Grouped matmuls (COAST_MM_GROUPED): the checks shared by coast_launch and coast_run_host.  M is the product count G, the
- * stacked A and C are one R-row matrix from row ro[0] (R = n_units / N), B is G matrices end to end. */
-static int grouped_check(const coast_launch_desc* d) {
-    if (!is_matmul(d->kernel))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: grouped products exist for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", d->kernel);
-    if (d->mode & (COAST_MM_BATCHED | COAST_UNIT_OFFSETS))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: cannot be combined with COAST_MM_BATCHED or COAST_UNIT_OFFSETS");
-    if (!d->M || d->M > XMR_MM_GRP_MAX)
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: M is the product count G, 1..%u (got %u)", XMR_MM_GRP_MAX, d->M);
-    if (!d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: N and K are shared by every product and must be nonzero");
-    if (d->n_units % d->N)
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: n_units must be a multiple of N = %u (R rows x N; got %llu)", d->N,
-                    (unsigned long long)d->n_units);
-    const int b_rows_k = mm_b_rows_k(d);                               /* as in batched_check */
-    if (d->n_units / d->N >= (1ull << 31) || (uint64_t)d->M * (b_rows_k ? d->K : d->N) >= (1ull << 31))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the rows R and G*%c must be below 2^31 (R %llu, G %u, %c %u)",
-                    b_rows_k ? 'K' : 'N', (unsigned long long)(d->n_units / d->N), d->M, b_rows_k ? 'K' : 'N', b_rows_k ? d->K : d->N);
-    if (!d->d_rows || (((uintptr_t)d->d_rows) & 7u))
-        return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: d_rows must point to G + 1 8-byte aligned uint64_t row offsets");
-    return COAST_OK;
-}
-/* The limb kernel's pre-pass for groups: the R rows of A from row ro[0], then every product's B (as a batch). */
-static int prepass_split_limbs_grouped(const coast_launch_desc* d, CUdeviceptr pa, CUstream s) {
-    unsigned long long rows = d->n_units / d->N, K = d->K; const void* A = d->d_in; const void* ro = d->d_rows;
-    void* params_a[] = { &ro, &A, &pa, &rows, &K };
-    int rc = launch_small("xmr_mm_grp_split_a", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_a, s); if (rc) return rc;
-    return prepass_split_b(d, pa + (size_t)rows * d->K * 4u, d->M, s);
-}
-static int prepass_transpose_b_grouped(const coast_launch_desc* d, CUdeviceptr bt, CUstream s) {
-    const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N, nb = d->M;
-    void* params[] = { &B, &bt, &k32, &n32, &nb };
-    return launch_small("xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
 }
 /* tile_start of the products (xmr_mm_group_scan, one CTA) into the group block; for TF32 and BF16 (a_map) it also rebases the host's A map
  * onto row ro[0] of d_in with R rows, so no host-side read of the device table is needed */
 static int prepass_group_scan(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr grp, const CUtensorMap* a_map, CUstream s) {
     const void* ro = d->d_rows; const void* base = d->d_in;
-    unsigned int n_grp = d->M, R = (unsigned)(d->n_units / d->N), tm = L->grp_tm, tn = L->grp_tiles_n;
-    unsigned int row_bytes = a_map ? d->K * KINFO[d->kernel].mm_elem : 0u;
+    unsigned int n_grp = d->M, R = (unsigned)L->mm.rows, tm = L->grp_tm, tn = L->grp_tiles_n;
+    unsigned int row_bytes = a_map ? d->K * L->mm.es : 0u;
     CUtensorMap none; memset(&none, 0, sizeof none);
     void* params[] = { &ro, &n_grp, &R, &tm, &tn, &grp, &base, &row_bytes, (void*)(a_map ? a_map : &none) };
     return launch_small("xmr_mm_group_scan", 1, XMR_MM_GRP_SCAN_THREADS, params, s);
@@ -675,7 +686,8 @@ static int ragged_check(const coast_launch_desc* d) {
 
 /* Cost-ordering pre-pass of the ragged kernels (xmr_ragged.cuh): zero the header and the bucket counts, histogram, one-CTA scan
  * (which also stores the offset table's address in the header), scatter into the permutation.  All on the launch's stream. */
-static int prepass_ragged(const coast_launch_desc* d, CUdeviceptr scratch, CUstream s) {
+static int prepass_ragged(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr scratch, CUstream s) {
+    (void)L;
     DRV(p_cuMemsetD8Async(scratch, 0, XMR_RAGGED_PERM, s));
     const void* off = d->d_aux;
     unsigned long long n = d->n_units;
@@ -704,16 +716,18 @@ static int run_plan(const launch_plan* L, const coast_launch_desc* d, xmr_args* 
     if (bytes) DRV(p_cuMemAllocFromPoolAsync(&scratch, bytes, G.pool, stream));
     if (L->scratch_per_cta || L->scratch_as_aux) a->aux = (const void*)scratch;
     CUtensorMap maps[2];
-    rc = L->prepass ? L->prepass(d, scratch, stream) : COAST_OK;
+    rc = L->prepass ? L->prepass(L, d, scratch, stream) : COAST_OK;
     for (int i = 0; i < L->n_maps && !rc; ++i) rc = encode_map(&L->map[i], scratch, L->cache_maps, &maps[i]);
     /* grouped: the tile table (and the GEMMs' rebased A map) after the other pre-passes; the kernel takes ro and the group block */
     const void* ro = d->d_rows;
     CUdeviceptr grp = scratch + L->grp_off;
-    if (!rc && L->grouped && L->grp_tm)
+    if (!rc && L->mm.grouped && L->grp_tm)
         rc = prepass_group_scan(L, d, grp, d->kernel != COAST_K_MM_U32 ? &maps[0] : NULL, stream);
     if (!rc) {
-        void* params[5] = { a, &maps[0], &maps[1], &ro, &grp };
-        if (L->grouped && !L->n_maps) { params[1] = &ro; params[2] = &grp; }
+        void* params[5] = { a };
+        int n_params = 1;
+        for (int i = 0; i < L->n_maps; ++i) params[n_params++] = &maps[i];
+        if (L->mm.grouped) { params[n_params++] = &ro; params[n_params++] = &grp; }
         if (d->flags & COAST_F_VERBOSE)
             fprintf(stderr, "coast_rt: %s grid=%u block=%u smem=%u units=%llu\n", L->name, grid, L->block, L->smem,
                     (unsigned long long)d->n_units);
@@ -731,12 +745,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     if (d->num_clones < 1 || d->num_clones > 3) return fail(COAST_ERR_BAD_ARG, "num_clones must be 1, 2 (DWC) or 3 (TMR)");
     const int ragged = (d->mode & COAST_UNIT_OFFSETS) != 0;
     if (ragged && (rc = ragged_check(d))) return rc;
-    const int batched = (d->mode & COAST_MM_BATCHED) != 0;
-    if (batched && (rc = batched_check(d))) return rc;
-    const int grouped = (d->mode & COAST_MM_GROUPED) != 0;
-    if (grouped && (rc = grouped_check(d))) return rc;
-    if ((rc = b_transposed_check(d))) return rc;
-    const int bt = (d->mode & COAST_MM_B_TRANSPOSED) != 0;
+    mm_shape m;
+    if ((rc = mm_check(d, &m))) return rc;
     if (d->n_units == 0) return COAST_OK;
     if (!d->d_in || !d->d_out) return fail(COAST_ERR_BAD_ARG, "null device buffer");
     const uint32_t nc = d->num_clones;
@@ -781,6 +791,12 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     L.block = XMR_CTA_THREADS; L.waves = 4; L.cluster = 1;
     const int aligned16 = (((uintptr_t)d->d_in) & 15u) == 0;
     const int ring_ok = d->unit_bytes == 64 && aligned16 && d->n_units < 0x7FFFFF00ull && !store_votes;   /* 64-byte rows through TMA */
+    L.mm = m;
+    if (is_matmul(d->kernel)) {
+        const char* fam = d->kernel == COAST_K_MM_U32 ? "MM" : "GEMM";
+        if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "%s needs A (d_in), B (d_aux) and M,N,K", fam);
+        if (!m.batched && !m.grouped && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "%s: n_units must be M*N", fam);
+    }
     switch (d->kernel) {
     case COAST_K_SHA256:
         if (((uintptr_t)d->d_out) & 15u) return fail(COAST_ERR_BAD_ARG, "SHA output must be 16-byte aligned");
@@ -833,63 +849,36 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         break;
     }
     case COAST_K_MM_U32: {
-        if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "MM needs A (d_in), B (d_aux) and M,N,K");
-        if (!batched && !grouped && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "MM: n_units must be M*N");
-        if (grouped) {                                       /* the shape rules are N's and K's; every product's rows are free */
-            const char* gpath = getenv("COAST_MM_PATH");
-            const int galigned = aligned16 && !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u);
-            const uint64_t R = d->n_units / d->N;
-            L.grouped = 1;
-            snprintf(L.name, sizeof L.name, bt ? "xmr_mm_u32_bt_grp_inj%d_nc%u" : "xmr_mm_u32_grp_inj%d_nc%u", inj, nc);
-            if (store_votes || !galigned) break;
-            if ((!gpath || !strcmp(gpath, "tc")) && d->N % xmr_mmtc_bn(1) == 0 && d->K % XMR_MMTC_BK == 0) {
-                const unsigned bn = xmr_mmtc_bn(nc);
-                /* B^T: the same planes (the pre-pass differs); only the fault recompute reads B itself */
-                if (bt && inj) snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_bt_grp_inj1_nc%u", nc);
-                else snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_grp_inj%d_nc%u", inj, nc);
-                L.block = XMR_WG_THREADS; L.smem = xmr_mmtc_smem(nc);
-                L.ctas = (R / XMR_WG_BM + d->M) * (d->N / bn); L.waves = 1;       /* a bound on the tiles; persistent CTAs */
-                L.grp_off = ((size_t)R * d->K + (size_t)d->M * d->K * d->N) * 4u;   /* after the limb planes */
-                L.scratch = L.grp_off + (size_t)xmr_mm_grp_bytes(d->M);
-                L.prepass = prepass_split_limbs_grouped; L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / bn;
-                L.n_maps = 2;
-                plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, (uint32_t)R, 4, XMR_WG_BM);
-                plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)R * d->K * 4u, 1, d->K, d->M * d->N, 4, bn);
-            } else if (!(gpath && !strcmp(gpath, "naive")) && d->N % XMR_MMT_BN == 0 && d->K % XMR_MMT_BK == 0) {
-                snprintf(L.name, sizeof L.name, bt ? "xmr_mm_u32_tiled_bt_grp_inj%d_nc%u" : "xmr_mm_u32_tiled_grp_inj%d_nc%u", inj, nc);
-                L.block = xmr_mmt_threads(nc); L.smem = XMR_MMT_SMEM;
-                L.ctas = (R / XMR_MMT_BM + d->M) * (d->N / XMR_MMT_BN); L.waves = 0;   /* a bound on the tiles: surplus CTAs exit */
-                L.scratch = (size_t)xmr_mm_grp_bytes(d->M);
-                L.grp_tm = XMR_MMT_BM; L.grp_tiles_n = d->N / XMR_MMT_BN;
-            }
-            break;
-        }
         /* the plain kernel (one lane per replica per element) takes any shape and the per-k votes on `sum`; tile-aligned problems
          * go to the tensor cores (exact, u8 limbs on wgmma) or the register-tiled kernel; COAST_MM_PATH=tc|tiled|naive overrides.
-         * The shape rules are those of one product; a batch stacks the products' rows (no tile straddles two of them). */
-        if (bt) snprintf(L.name, sizeof L.name, "xmr_mm_u32_bt_inj%d_nc%u", inj, nc);
-        else snprintf(L.name, sizeof L.name, "xmr_mm_u32_nc%u_inj%d", nc, inj);
+         * The shape rules are those of one product; a batch stacks the products' rows (no tile straddles two of them), and the
+         * rows of grouped products are free. */
         const char* path = getenv("COAST_MM_PATH");
         const int aligned = aligned16 && !(((uintptr_t)d->d_aux) & 15u) && !(((uintptr_t)d->d_out) & 15u);
-        const uint64_t batch = mm_batch(d), rows = batch * d->M;
-        if (store_votes || !aligned) break;
-        if ((!path || !strcmp(path, "tc")) && d->M % XMR_WG_BM == 0 && d->N % xmr_mmtc_bn(1) == 0 && d->K % XMR_MMTC_BK == 0) {
+        const int tiles_ok = !store_votes && aligned;
+        const char* variant = "";
+        int bt_name = m.bt;
+        if (tiles_ok && (!path || !strcmp(path, "tc")) && (m.grouped || d->M % XMR_WG_BM == 0) && d->N % xmr_mmtc_bn(1) == 0 &&
+            d->K % XMR_MMTC_BK == 0) {
             const unsigned bn = xmr_mmtc_bn(nc);
-            if (bt && inj) snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_bt_inj1_nc%u", nc);
-            else snprintf(L.name, sizeof L.name, "xmr_mm_u32_tc_nc%u_inj%d", nc, inj);
+            variant = "_tc";
+            bt_name = m.bt && inj;                           /* B^T: the same planes (the pre-pass differs); only the fault recompute reads B itself */
             L.block = XMR_WG_THREADS; L.smem = xmr_mmtc_smem(nc);
-            L.ctas = (rows / XMR_WG_BM) * (d->N / bn); L.waves = 1;
-            L.scratch = ((size_t)rows * d->K + (size_t)batch * d->K * d->N) * 4u;     /* 4 planes of 1 byte per element */
+            L.ctas = mm_row_tiles(&m, XMR_WG_BM) * (d->N / bn); L.waves = 1;           /* persistent CTAs */
+            L.scratch = ((size_t)m.rows * d->K + (size_t)m.P * d->K * d->N) * 4u;       /* 4 planes of 1 byte per element */
             L.prepass = prepass_split_limbs;
+            L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / bn;
             L.n_maps = 2;
-            plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, (uint32_t)rows, 4, XMR_WG_BM);
-            plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)rows * d->K * 4u, 1, d->K, (uint32_t)(batch * d->N), 4, bn);
-        } else if (!(path && !strcmp(path, "naive")) && d->M % XMR_MMT_BM == 0 && d->N % XMR_MMT_BN == 0 && d->K % XMR_MMT_BK == 0) {
-            if (bt) snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_bt_inj%d_nc%u", inj, nc);
-            else snprintf(L.name, sizeof L.name, "xmr_mm_u32_tiled_nc%u_inj%d", nc, inj);
+            plan_wg_map(&L.map[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 0, 1, d->K, (uint32_t)m.rows, 4, XMR_WG_BM);
+            plan_wg_map(&L.map[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, (size_t)m.rows * d->K * 4u, 1, d->K, (uint32_t)(m.P * d->N), 4, bn);
+        } else if (tiles_ok && !(path && !strcmp(path, "naive")) && (m.grouped || d->M % XMR_MMT_BM == 0) && d->N % XMR_MMT_BN == 0 &&
+                   d->K % XMR_MMT_BK == 0) {
+            variant = "_tiled";
             L.block = xmr_mmt_threads(nc); L.smem = XMR_MMT_SMEM;
-            L.ctas = (rows / XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;
+            L.ctas = mm_row_tiles(&m, XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;   /* grouped: surplus CTAs exit */
+            L.grp_tm = XMR_MMT_BM; L.grp_tiles_n = d->N / XMR_MMT_BN;
         }
+        mm_kernel_name(L.name, "xmr_mm_u32", variant, bt_name, m.grouped, 0, nc, inj);
         break;
     }
     case COAST_K_QSORT:
@@ -932,44 +921,27 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
          * into scratch; or bfloat16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch) */
         const int bf16 = d->kernel == COAST_K_GEMM_BF16;
         const char* TY = bf16 ? "BF16" : "TF32";
-        const unsigned es = KINFO[d->kernel].mm_elem, bk = bf16 ? XMR_GEMM_BF16_BK : XMR_GEMM_BK;
+        const unsigned bk = bf16 ? XMR_GEMM_BF16_BK : XMR_GEMM_BK;
         const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-        if (!d->d_aux || !d->M || !d->N || !d->K) return fail(COAST_ERR_BAD_ARG, "GEMM needs A (d_in), B (d_aux) and M,N,K");
-        if (!batched && !grouped && d->n_units != (uint64_t)d->M * d->N) return fail(COAST_ERR_BAD_ARG, "GEMM: n_units must be M*N");
-        if (grouped && (d->N % xmr_gemm_bn(0) || d->K % bk))
+        if (m.grouped && (d->N % xmr_gemm_bn(0) || d->K % bk))
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_%s grouped tiles are 128 x 128 x %u: N must be a multiple of 128 and K of %u "
                                                "(got %u, %u); the products' rows are free", TY, bk, bk, d->N, d->K);
-        if (!grouped && (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % bk))
+        if (!m.grouped && (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % bk))
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_%s tiles are 128x128x%u: M,N must be multiples of 128 and K of %u (got %u,%u,%u)",
                         TY, bk, bk, d->M, d->N, d->K);
         if (!aligned16 || (((uintptr_t)d->d_aux) & 15u) || (((uintptr_t)d->d_out) & 15u)) return fail(COAST_ERR_BAD_ARG, "GEMM buffers must be 16-byte aligned");
         /* unprotected 128 x 256 tiles when N allows (wide), else 128 x 128.  CTA-pair kernels (cluster 2 x 1 x 1,
          * 256-row pair tiles, B multicast) are bit-identical to the single-CTA kernels.  Default: pairs for the unprotected and
          * DWC kernels when the shape allows, the single-CTA kernel for TMR; COAST_GEMM_PAIR=0 / 1 forces one or the other.
-         * A batch stacks its products' rows: a pair tile needs the rows of ONE product, so M (per product) % 256 == 0. */
-        const int wide = !grouped && nc == 1 && d->N % xmr_gemm_bn(1) == 0;          /* grouped: 128 x 128 tiles */
+         * A batch stacks its products' rows: a pair tile needs the rows of ONE product, so M (per product) % 256 == 0.
+         * Groups take 128 x 128 tiles on single CTAs. */
+        const int wide = !m.grouped && nc == 1 && d->N % xmr_gemm_bn(1) == 0;
         const char* e = getenv("COAST_GEMM_PAIR");
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
-        const int pair = !grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
-        if (bf16 && bt) {                                   /* B^T read in place, K-major (xmr_gemm_bf16*_bt_*) */
-            if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_bt_grp_inj%d_nc1", inj);
-            else if (grouped) snprintf(L.name, sizeof L.name, nc == 2 ? "xmr_gemm_bf16_bt_grp_inj%d_nc2" : "xmr_gemm_bf16_bt_grp_inj%d_nc3", inj);
-            else if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16p_bt_inj%d_nc%u", inj, nc);
-            else if (nc == 1 && !wide) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_bt_inj%d_nc1", inj);
-            else snprintf(L.name, sizeof L.name, "xmr_gemm_bf16_bt_inj%d_nc%u", inj, nc);
-        }
-        else if (bf16) {
-            if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_grp_inj%d_nc1", inj);
-            else if (grouped) snprintf(L.name, sizeof L.name, nc == 2 ? "xmr_gemm_bf16_grp_inj%d_nc2" : "xmr_gemm_bf16_grp_inj%d_nc3", inj);
-            else if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16p_inj%d_nc%u", inj, nc);
-            else if (nc == 1 && !wide) snprintf(L.name, sizeof L.name, "xmr_gemm_bf16n_inj%d_nc1", inj);
-            else snprintf(L.name, sizeof L.name, "xmr_gemm_bf16_inj%d_nc%u", inj, nc);
-        }
-        else if (grouped && nc == 1) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32n_grp_inj%d_nc1", inj);
-        else if (grouped) snprintf(L.name, sizeof L.name, nc == 2 ? "xmr_gemm_tf32_grp_inj%d_nc2" : "xmr_gemm_tf32_grp_inj%d_nc3", inj);
-        else if (pair) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32p_nc%u_inj%d", nc, inj);
-        else if (nc == 1 && !wide) snprintf(L.name, sizeof L.name, "xmr_gemm_tf32n_nc1_inj%d", inj);
-        else snprintf(L.name, sizeof L.name, "xmr_gemm_tf32_nc%u_inj%d", nc, inj);
+        const int pair = !m.grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
+        /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it, TF32 only skips the transposing pre-pass */
+        mm_kernel_name(L.name, bf16 ? "xmr_gemm_bf16" : "xmr_gemm_tf32", pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt,
+                       m.grouped, bf16, nc, inj);
         { const char* g = getenv("COAST_GEMM_GROUP_M");
           if (g && atoi(g) > 0 && atoi(g) <= (int)XMR_MODE_GROUP_M_MASK) a.mode = (a.mode & ~XMR_MODE_GROUP_M_MASK) | (unsigned)atoi(g); }
         /* L2 eviction priorities: A evict_last, B and C evict_first; COAST_GEMM_L2_HINTS=0 loads and stores with the normal policy */
@@ -978,41 +950,33 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         { const char* h = getenv("COAST_GEMM_TAIL_SPLIT"); if (h && !strcmp(h, "0")) a.mode |= XMR_MODE_NO_TAIL_SPLIT; }
         /* persistent CTAs, one per SM (their shared memory allows no second); pairs: an even grid */
         L.block = XMR_WG_THREADS; L.smem = xmr_gemm_smem(wide);
-        const uint64_t batch = mm_batch(d), rows = batch * d->M;
-        L.ctas = (rows / XMR_WG_BM) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = pair ? 2 : 1;
+        L.ctas = mm_row_tiles(&m, XMR_WG_BM) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = pair ? 2 : 1;
+        L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / xmr_gemm_bn(wide);
         /* B^T of every product into scratch, unless the caller holds it (COAST_MM_B_TRANSPOSED) or BF16 reads B in place */
-        const int b_scratch = !bf16 && !bt, b_in_place = bf16 && !bt;
+        const int b_scratch = !bf16 && !m.bt;
+        const uintptr_t b_base = b_scratch ? 0 : (uintptr_t)d->d_aux;
         if (b_scratch) {
-            L.scratch = (size_t)batch * d->K * d->N * 4u;
+            L.scratch = (size_t)m.P * d->K * d->N * 4u;
             L.prepass = prepass_transpose_b;
         }
         L.n_maps = 2;
-        if (grouped) {
-            /* 128 x 128 tiles of every product on single CTAs (no pairs, no wide tiles); A's map is encoded here over 128 rows of a
-             * placeholder and rebased by the scan onto row ro[0] of d_in with R rows (the host does not read the device table).  The
-             * placeholder is the B^T scratch, or without it (BF16, or a caller's B^T) d_aux: d_in of a host-call chunk is biased by
-             * ro[first] rows and need not be an address of its own */
-            const uint64_t R = d->n_units / d->N;
-            L.grouped = 1;
-            L.ctas = (R / XMR_WG_BM + d->M) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = 1;
-            L.grp_off = b_scratch ? (size_t)d->M * d->K * d->N * 4u : 0;         /* after B^T of every product */
-            L.scratch = L.grp_off + (size_t)xmr_mm_grp_bytes(d->M);
-            if (b_scratch) L.prepass = prepass_transpose_b_grouped;
-            L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / xmr_gemm_bn(wide);
-            plan_wg_map(&L.map[0], dt, es, b_scratch ? 0 : (uintptr_t)d->d_aux, b_scratch, d->K, XMR_WG_BM, 1, XMR_WG_BM);
-            if (b_in_place) plan_wg_map(&L.map[1], dt, es, (uintptr_t)d->d_aux, 0, d->N, d->M * d->K, 1, XMR_GEMM_BF16_BK);
-            else plan_wg_map(&L.map[1], dt, es, b_scratch ? 0 : (uintptr_t)d->d_aux, b_scratch, d->K, d->M * d->N, 1, xmr_gemm_b_box(0));
-            break;
-        }
-        plan_wg_map(&L.map[0], dt, es, (uintptr_t)d->d_in, 0, d->K, (uint32_t)rows, 1, XMR_WG_BM);
-        /* B: the stacked B^T, (batch N) rows of K, in scratch or the caller's (COAST_MM_B_TRANSPOSED); BF16 without the bit: the
-         * caller's B, (batch K) rows of N in boxes of 64 columns x 64 k-rows */
-        if (b_in_place) plan_wg_map(&L.map[1], dt, es, (uintptr_t)d->d_aux, 0, d->N, (uint32_t)(batch * d->K), 1, XMR_GEMM_BF16_BK);
-        else plan_wg_map(&L.map[1], dt, es, b_scratch ? 0 : (uintptr_t)d->d_aux, b_scratch, d->K, (uint32_t)(batch * d->N), 1, xmr_gemm_b_box(pair));
+        /* A: the stacked rows of d_in; for groups a placeholder of 128 rows that the scan rebases onto row ro[0] of d_in with R rows
+         * (the host does not read the device table).  The placeholder is the B^T scratch, or without it d_aux: d_in of a host-call
+         * chunk is biased by ro[first] rows and need not be an address of its own */
+        if (m.grouped) plan_wg_map(&L.map[0], dt, m.es, b_base, b_scratch, d->K, XMR_WG_BM, 1, XMR_WG_BM);
+        else plan_wg_map(&L.map[0], dt, m.es, (uintptr_t)d->d_in, 0, d->K, (uint32_t)m.rows, 1, XMR_WG_BM);
+        /* B: the stacked B^T, (P N) rows of K, in scratch or the caller's; BF16 without COAST_MM_B_TRANSPOSED: the caller's B,
+         * (P K) rows of N in boxes of 64 columns x 64 k-rows */
+        plan_wg_map(&L.map[1], dt, m.es, b_base, b_scratch, m.b_rows_k ? d->N : d->K, (uint32_t)(m.P * m.b_rows), 1,
+                    m.b_rows_k ? XMR_GEMM_BF16_BK : xmr_gemm_b_box(pair));
         break;
     }
     default:
         return fail(COAST_ERR_UNSUPPORTED, "kernel %u is not built into this library yet", d->kernel);
+    }
+    if (m.grouped && L.grp_tm) {                             /* the group block follows the other scratch */
+        L.grp_off = L.scratch;
+        L.scratch += (size_t)xmr_mm_grp_bytes(d->M);
     }
     if (ragged) {                                            /* one resident wave pulling cost-ordered warp-tiles (xmr_ragged.cuh) */
         L.waves = 1;
@@ -1269,23 +1233,23 @@ static void next_products(const host_sched* s, uint64_t done, uint64_t* budget, 
     item_chunk(s, done, left < s->max_items ? left : s->max_items, c);
 }
 
-/* Grouped matmuls (COAST_MM_GROUPED, d_rows = the caller's host row offsets ro[]): a chunk is the longest run of whole products
- * whose A rows, B matrices, C rows and offsets fit COAST_HOST_CHUNK_BYTES; a larger product is a chunk of its own.  The chunk
+/* Grouped matmuls (COAST_MM_GROUPED, d_rows = the caller's host row offsets ro[]; ib, ab and ob are the bytes of a row of A, of
+ * one product's B and of a row of C): a chunk is the longest run of whole products whose A rows, B matrices, C rows and offsets
+ * fit COAST_HOST_CHUNK_BYTES; a larger product is a chunk of its own.  The chunk
  * uploads its offset slice ro[first .. end] unchanged and launches with the slots' addresses minus ro[first] rows as d_in and
  * d_out (exact under u64 wraparound, as next_ragged), so the caller's offsets are never rewritten. */
 static void next_groups(const host_sched* s, uint64_t first, uint64_t* budget, host_chunk* c) {
     const uint64_t* ro = (const uint64_t*)s->d->d_rows;
-    const uint64_t K = s->d->K, N = s->d->N;
+    const uint64_t N = s->d->N;
     uint64_t e = first + 1;
-    const uint64_t es = KINFO[s->d->kernel].mm_elem;         /* A and B elements; C elements are 4 bytes */
-    while (e < s->total && (ro[e + 1] - ro[first]) * (K * es + N * 4u) + (e + 1 - first) * (K * N * es + 8u) + 8u <= *budget) ++e;
+    while (e < s->total && (ro[e + 1] - ro[first]) * (s->ib + s->ob) + (e + 1 - first) * (s->ab + 8u) + 8u <= *budget) ++e;
     memset(c, 0, sizeof *c);
     const uint64_t rows = ro[e] - ro[first];
     c->items = e - first; c->M = (uint32_t)(e - first);
     c->n_units = rows * N; c->unit_base = (ro[first] - ro[0]) * N;
-    c->in = (byte_range){ ro[first] * K * es, rows * K * es }; c->in_bias = ro[first] * K * es;
-    c->aux = (byte_range){ first * K * N * es, (e - first) * K * N * es };
-    c->out = (byte_range){ ro[first] * N * 4u, rows * N * 4u }; c->out_bias = ro[first] * N * 4u;
+    c->in = (byte_range){ ro[first] * s->ib, rows * s->ib }; c->in_bias = ro[first] * s->ib;
+    c->aux = (byte_range){ first * s->ab, (e - first) * s->ab };
+    c->out = (byte_range){ ro[first] * s->ob, rows * s->ob }; c->out_bias = ro[first] * s->ob;
     c->rows = (byte_range){ first * 8u, (e - first + 1) * 8u };
 }
 
@@ -1384,7 +1348,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
     { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) chunk_bytes = (uint64_t)atoll(e); }
     host_sched s; memset(&s, 0, sizeof s);
     s.d = d; s.upi = 1; s.path = "staged";
-    if ((rc = b_transposed_check(d))) return rc;
+    if ((rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED))) return rc;
 
     if (d->mode & COAST_UNIT_OFFSETS) {                      /* ragged: staged only */
         if ((rc = ragged_check(d))) return rc;
@@ -1408,31 +1372,28 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
         s.budget = (1ull << 20) < chunk_bytes ? (1ull << 20) : chunk_bytes; s.max_bytes = chunk_bytes;
         return run_chunks(&s, out, dwc_fired);
     }
-    if ((d->mode & COAST_MM_BATCHED) && (rc = batched_check(d))) return rc;
-    if (d->mode & COAST_MM_GROUPED) {                        /* whole products per chunk, the offsets checked first */
-        if ((rc = grouped_check(d))) return rc;
-        if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");
-        const uint64_t* ro = (const uint64_t*)d->d_rows, R = d->n_units / d->N;
-        for (uint32_t g = 0; g < d->M; ++g)
-            if (ro[g + 1] < ro[g])
-                return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: product %u runs from row %llu to %llu; row offsets must not decrease",
-                            g, (unsigned long long)ro[g], (unsigned long long)ro[g + 1]);
-        if (ro[d->M] - ro[0] != R)
-            return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the products hold %llu rows but n_units / N is %llu",
-                        (unsigned long long)(ro[d->M] - ro[0]), (unsigned long long)R);
-        if (R && (!d->d_in || !d->d_out || !d->d_aux)) return fail(COAST_ERR_BAD_ARG, "null host buffer");
-        s.next = next_groups; s.total = d->M; s.max_bytes = chunk_bytes; s.budget = chunk_bytes; s.min_in = 16; s.path = "groups";
-        return run_chunks(&s, out, dwc_fired);
-    }
+    mm_shape m;
+    if ((rc = mm_check(d, &m))) return rc;
     if (is_matmul(d->kernel)) {
         if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");
-        const uint64_t es = KINFO[d->kernel].mm_elem;
-        const uint64_t ab = (uint64_t)d->M * d->K * es, bb = (uint64_t)d->K * d->N * es, cb = (uint64_t)d->M * d->N * 4u;
-        if (d->mode & COAST_MM_BATCHED) {                    /* as many whole products as the chunk bytes hold, at least one */
+        const uint64_t a_row = (uint64_t)d->K * m.es, c_row = (uint64_t)d->N * 4u, bb = (uint64_t)d->K * d->N * m.es;
+        if (m.grouped) {                                     /* whole products per chunk, the offsets checked first */
+            const uint64_t* ro = (const uint64_t*)d->d_rows;
+            for (uint32_t g = 0; g < d->M; ++g)
+                if (ro[g + 1] < ro[g])
+                    return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: product %u runs from row %llu to %llu; row offsets must not decrease",
+                                g, (unsigned long long)ro[g], (unsigned long long)ro[g + 1]);
+            if (ro[d->M] - ro[0] != m.rows)
+                return fail(COAST_ERR_BAD_ARG, "COAST_MM_GROUPED: the products hold %llu rows but n_units / N is %llu",
+                            (unsigned long long)(ro[d->M] - ro[0]), (unsigned long long)m.rows);
+            if (m.rows && (!d->d_in || !d->d_out || !d->d_aux)) return fail(COAST_ERR_BAD_ARG, "null host buffer");
+            s.next = next_groups; s.total = m.P; s.ib = a_row; s.ab = bb; s.ob = c_row;
+            s.max_bytes = chunk_bytes; s.budget = chunk_bytes; s.min_in = 16; s.path = "groups";
+        } else if (m.batched) {                              /* as many whole products as the chunk bytes hold, at least one */
             if (!d->d_in || !d->d_out || !d->d_aux) return fail(COAST_ERR_BAD_ARG, "null host buffer");
-            s.next = next_products; s.total = d->n_units / ((uint64_t)d->M * d->N); s.upi = (uint64_t)d->M * d->N;
-            s.ib = ab; s.ab = bb; s.ob = cb;
-            s.max_items = chunk_bytes / (ab + bb + cb) ? chunk_bytes / (ab + bb + cb) : 1u;
+            s.next = next_products; s.total = m.P; s.upi = (uint64_t)d->M * d->N;
+            s.ib = d->M * a_row; s.ab = bb; s.ob = d->M * c_row;
+            s.max_items = chunk_bytes / (s.ib + s.ab + s.ob) ? chunk_bytes / (s.ib + s.ab + s.ob) : 1u;
         } else {
             /* B (the replicated operand) goes up once; C comes in at most 8 blocks of whole 128-row groups.  Small or oddly
              * shaped problems go in one block. */
@@ -1441,7 +1402,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
                 const uint64_t blocks = d->M / 128u < 8u ? d->M / 128u : 8u;
                 rows = ((d->M / 128u + blocks - 1u) / blocks) * 128u;
             }
-            s.next = next_row_block; s.total = d->M; s.upi = d->N; s.ib = (uint64_t)d->K * es; s.ob = (uint64_t)d->N * 4u;
+            s.next = next_row_block; s.total = d->M; s.upi = d->N; s.ib = a_row; s.ob = c_row;
             s.max_items = rows; s.shared_b = bb;
             s.path = rows < d->M ? "row-blocks" : "one-shot";
         }

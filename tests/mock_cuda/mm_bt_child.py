@@ -3,7 +3,7 @@
 Each op gives `kernel`, M, N, K and either nothing (one product), `batch` (COAST_MM_BATCHED) or a row-offset table `ro`
 (COAST_MM_GROUPED; M = G unless the op gives M); `bt` sets COAST_MM_B_TRANSPOSED.  A and B have the kernel's element size
 (2 bytes for GEMM_BF16, else 4), C 4 bytes; `alloc` overrides the element counts [A, B, C], `shift` = [in, aux, out] byte
-offsets misalign a buffer, `mode` and `n` override what the op implies.  Prints one JSON object."""
+offsets misalign a buffer (`rows_shift` the row offsets), `mode` and `n` override what the op implies.  Prints one JSON object."""
 import ctypes as C
 import json
 import os
@@ -64,7 +64,7 @@ def main():
             if ro:
                 assert L.coast_malloc(C.byref(rows), 8 * len(ro)) == 0
                 assert L.coast_memcpy_h2d(rows, table, 8 * len(ro), None) == 0
-                d.d_rows = rows.value
+                d.d_rows = rows.value + op.get("rows_shift", 0)
             d.d_in, d.d_aux, d.d_out = [b.value + s for b, s in zip(bufs, shift)]
             rc = L.coast_launch(C.byref(d), None)
             out.append({"rc": rc, "err": L.coast_last_error().decode() if rc else "", "in": d.d_in, "aux": d.d_aux, "out": d.d_out,

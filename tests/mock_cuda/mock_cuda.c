@@ -8,6 +8,7 @@
  * appended as one JSON line to $MOCK_CUDA_LOG.
  */
 #include <cuda.h>
+#include <elf.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -45,7 +46,7 @@ static CUresult do_alloc(CUdeviceptr* out, size_t n, int host) {
     void* p = NULL;
     if (posix_memalign(&p, 512, n)) return CUDA_ERROR_OUT_OF_MEMORY;      /* cuMemAlloc returns >= 256-byte aligned memory */
     allocs[n_allocs].base = (uintptr_t)p; allocs[n_allocs].size = n; allocs[n_allocs].live = 1; allocs[n_allocs].host = host;
-    LOG("{\"op\":\"alloc\",\"id\":%d,\"bytes\":%zu,\"host\":%d}", n_allocs, n, host);
+    LOG("{\"op\":\"alloc\",\"id\":%d,\"bytes\":%zu,\"host\":%d,\"ptr\":%llu}", n_allocs, n, host, (unsigned long long)(uintptr_t)p);
     n_allocs++;
     *out = (CUdeviceptr)(uintptr_t)p;
     return CUDA_SUCCESS;
@@ -91,14 +92,33 @@ CUresult cuDevicePrimaryCtxRelease_v2(CUdevice d) { (void)d; return CUDA_SUCCESS
 static CUcontext cur_ctx;
 CUresult cuCtxSetCurrent(CUcontext c) { cur_ctx = c; return CUDA_SUCCESS; }
 CUresult cuCtxGetCurrent(CUcontext* c) { *c = cur_ctx; return CUDA_SUCCESS; }
+static const unsigned char* module_image;
 CUresult cuModuleLoadData(CUmodule* m, const void* image) {
     if (memcmp(image, "\x7f" "ELF", 4)) return bad("module image is not an ELF cubin");
+    module_image = image;
     *m = (CUmodule)&fake_mod; return CUDA_SUCCESS;
 }
 CUresult cuModuleUnload(CUmodule m) { (void)m; return CUDA_SUCCESS; }
+/* as the driver: a name is found only if it is a function symbol of the loaded cubin's .symtab */
+static int image_has_function(const char* name) {
+    const Elf64_Ehdr* eh = (const Elf64_Ehdr*)module_image;
+    const Elf64_Shdr* sh = (const Elf64_Shdr*)(module_image + eh->e_shoff);
+    for (int i = 0; i < eh->e_shnum; ++i) {
+        if (sh[i].sh_type != SHT_SYMTAB) continue;
+        const Elf64_Sym* sym = (const Elf64_Sym*)(module_image + sh[i].sh_offset);
+        const char* str = (const char*)module_image + sh[sh[i].sh_link].sh_offset;
+        for (size_t k = 0; k < sh[i].sh_size / sizeof *sym; ++k)
+            if (ELF64_ST_TYPE(sym[k].st_info) == STT_FUNC && !strcmp(str + sym[k].st_name, name)) return 1;
+    }
+    return 0;
+}
 CUresult cuModuleGetFunction(CUfunction* f, CUmodule m, const char* name) {
     (void)m;
     for (int i = 0; i < n_fns; ++i) if (!strcmp(fns[i].name, name)) { *f = (CUfunction)&fns[i]; return CUDA_SUCCESS; }
+    if (!module_image || !image_has_function(name)) {
+        LOG("{\"op\":\"error\",\"what\":\"no function %s in the module\"}", name);
+        return CUDA_ERROR_NOT_FOUND;
+    }
     if (n_fns >= 512) return CUDA_ERROR_INVALID_VALUE;
     snprintf(fns[n_fns].name, sizeof fns[0].name, "%s", name); fns[n_fns].max_dyn_smem = 48 * 1024;
     *f = (CUfunction)&fns[n_fns++];

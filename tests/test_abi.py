@@ -40,8 +40,9 @@ def test_sm90a_cubin_is_embedded(built_lib):
     assert cubin[:4] == b"\x7fELF" and cubin in blob
 
 
-def test_every_kernel_the_host_code_can_name_is_in_the_cubin(built_lib):
-    """coast_rt.c builds kernel names with snprintf; a typo would only show up as a launch failure on a GPU box"""
+def test_every_non_matmul_kernel_name_format_is_in_the_cubin(built_lib):
+    """coast_rt.c builds kernel names with snprintf; a typo would only show up as a launch failure on a GPU box.  The matmul
+    kernels' names follow one rule from their stems (mm_kernel_name); tests/test_mm_plan_sweep.py launches every one of them."""
     import itertools
     import re
     import subprocess
@@ -49,8 +50,9 @@ def test_every_kernel_the_host_code_can_name_is_in_the_cubin(built_lib):
     fmts = set(re.findall(r'"(xmr_[A-Za-z0-9_%]+)"', src))
     stems = {"xmr_qsort", "xmr_qsortn", "xmr_aes128_enc", "xmr_aes128_dec", "xmr_aes128_enck", "xmr_aes128_deck",
              "xmr_chaes_enc", "xmr_chaes_dec"}               # stems of a "%s_nc%u_inj%d"
-    assert stems <= fmts
-    fmts = (fmts - stems) | {s + "_nc%u_inj%d" for s in stems}
+    mm_stems = {"xmr_mm_u32", "xmr_gemm_tf32", "xmr_gemm_bf16"}
+    assert stems <= fmts and mm_stems <= fmts
+    fmts = (fmts - stems - mm_stems) | {s + "_nc%u_inj%d" for s in stems}
     names = set()
     for f in fmts:
         opts = [["tc"] if tok == "%s" else ["1", "2", "3"] if tok == "%u" else ["0", "1"] for tok in re.findall(r"%[sud]", f)]
@@ -60,7 +62,7 @@ def test_every_kernel_the_host_code_can_name_is_in_the_cubin(built_lib):
     sass = subprocess.run(["cuobjdump", "-elf", os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")],
                           capture_output=True, text=True).stdout
     have = set(re.findall(r"\.text\.(xmr_\w+)", sass))
-    assert len(names) > 80 and not (names - have), sorted(names - have)
+    assert len(names) > 100 and not (names - have), sorted(names - have)
 
 
 @pytest.mark.parametrize("s,nc,fl", [

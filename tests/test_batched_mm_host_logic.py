@@ -140,7 +140,7 @@ def test_a_batch_of_one_is_the_unbatched_launch(mock_dir, tmp_path, kernel, nc, 
                                             unit_base=77, flags=3)], env_extra=env)
     assert res["ops"][0]["rc"] == [0, 0]
     start = [i for i, e in enumerate(ev) if e["op"] == "alloc"][4] + 1          # after the counters and the caller's three buffers
-    seen = [{k: v for k, v in e.items() if k != "id"} for e in ev[start:] if e["op"] in ("launch", "tmap", "alloc")]
+    seen = [{k: v for k, v in e.items() if k not in ("id", "ptr")} for e in ev[start:] if e["op"] in ("launch", "tmap", "alloc")]
     assert len(seen) % 2 == 0 and len(seen) >= 2
     assert seen[: len(seen) // 2] == seen[len(seen) // 2:]
     assert sum(e["op"] == "launch" for e in seen) >= 2
