@@ -408,13 +408,16 @@ static const struct kernel_info {
     [COAST_K_CHSTONE_SHA] = { "chstone_sha", 20, 5,  IN_UNIT_BYTES, 0,  0, 1 },
     [COAST_K_CHSTONE_AES] = { "chstone_aes", 64, 16, 64,            64, 0, 1 },
     [COAST_K_GEMM_BF16]   = { "gemm_bf16",   4,  1,  0,             0,  0, 0, 2 },
+    [COAST_K_GEMM_FP8]    = { "gemm_fp8",    4,  1,  0,             0,  0, 0, 1 },
 };
-static int is_matmul(uint32_t kernel) { return kernel < COAST_K_COUNT_ && KINFO[kernel].mm_elem != 0; }
+/* an id with a row above; the ids between are unassigned (9) and unknown like those past the table */
+static int known_kernel(uint32_t kernel) { return kernel < COAST_K_COUNT_ && KINFO[kernel].name; }
+static int is_matmul(uint32_t kernel) { return known_kernel(kernel) && KINFO[kernel].mm_elem != 0; }
 
 static int store_votes_wanted(uint32_t fl) {
     return (fl & (COAST_F_STORE_DATA_SYNC | COAST_F_NO_MEM_REPLICATION)) && !(fl & COAST_F_NO_STORE_DATA_SYNC);
 }
-static int store_votes_built(uint32_t kernel) { return kernel < COAST_K_COUNT_ && KINFO[kernel].store_votes; }
+static int store_votes_built(uint32_t kernel) { return known_kernel(kernel) && KINFO[kernel].store_votes; }
 
 uint32_t coast_flags_honoured(uint32_t kernel, uint32_t nc, uint32_t fl) {
     uint32_t h = fl & (COAST_F_COUNT_ERRORS | COAST_F_COUNT_SYNCS | COAST_F_VERBOSE | COAST_F_MAJORITY_VOTER);
@@ -449,6 +452,7 @@ uint32_t coast_fault_sites(uint32_t kernel, uint32_t unit_bytes, uint32_t K) {
     case COAST_K_MM_U32:    return K;
     case COAST_K_GEMM_TF32: return 1u;
     case COAST_K_GEMM_BF16: return 1u;
+    case COAST_K_GEMM_FP8:  return 1u;
     case COAST_K_QSORT:     return 33u * (unit_bytes / 4u);
     case COAST_K_CHSTONE_SHA: return 421u * (unit_bytes / 64u + 1u);
     case COAST_K_CHSTONE_AES: return 176u;
@@ -461,18 +465,18 @@ uint32_t coast_fault_site_bits(uint32_t kernel, uint32_t unit_bytes, uint32_t K,
     if (kernel == COAST_K_AES128 || kernel == COAST_K_CHSTONE_AES) return 8u;
     return 32u;
 }
-uint32_t coast_out_bytes_per_unit(uint32_t kernel) { return kernel < COAST_K_COUNT_ ? KINFO[kernel].out_bytes : 0; }
-uint32_t coast_votes_per_unit(uint32_t kernel) { return kernel < COAST_K_COUNT_ ? KINFO[kernel].votes : 0; }
+uint32_t coast_out_bytes_per_unit(uint32_t kernel) { return known_kernel(kernel) ? KINFO[kernel].out_bytes : 0; }
+uint32_t coast_votes_per_unit(uint32_t kernel) { return known_kernel(kernel) ? KINFO[kernel].votes : 0; }
 uint32_t coast_out_bytes(uint32_t kernel, uint32_t unit_bytes) {
     return kernel == COAST_K_QSORT ? unit_bytes : coast_out_bytes_per_unit(kernel);
 }
 static uint64_t in_bytes_per_unit(const coast_launch_desc* d) {
-    if (d->kernel >= COAST_K_COUNT_) return 0;
+    if (!known_kernel(d->kernel)) return 0;
     return KINFO[d->kernel].in_bytes == IN_UNIT_BYTES ? d->unit_bytes : KINFO[d->kernel].in_bytes;
 }
 /* bytes of per-unit aux data the host call stages next to the input (AES keys) */
 static uint64_t aux_bytes_per_unit(const coast_launch_desc* d) {
-    return d->kernel < COAST_K_COUNT_ && (d->mode & COAST_AES_KEY_PER_UNIT) ? KINFO[d->kernel].key_bytes : 0;
+    return known_kernel(d->kernel) && (d->mode & COAST_AES_KEY_PER_UNIT) ? KINFO[d->kernel].key_bytes : 0;
 }
 
 /* ------------------------------------------------------------------ */
@@ -505,7 +509,8 @@ typedef struct {
     int batched, grouped, bt;     /* the mode bits */
     uint64_t P;                   /* products: 1, the batch or G */
     uint64_t rows;                /* stacked rows of A and C: batch*M or R */
-    int b_rows_k;                 /* B's map has K rows per product (GEMM_BF16 reading B in place); every B^T map has N */
+    int b_rows_k;                 /* B's map has K rows per product (GEMM_BF16 reading B in place); every B^T map has N (GEMM_FP8's
+                                     always: a B^T map over the pre-pass's scratch or the caller's B^T) */
     uint32_t b_rows;              /* rows per product of B's map */
 } mm_shape;
 
@@ -565,7 +570,7 @@ static int mm_bit_refused(const coast_launch_desc* d, uint32_t bit) {
     if (!(d->mode & bit) || is_matmul(d->kernel)) return COAST_OK;
     const char* what = bit == COAST_MM_BATCHED ? "COAST_MM_BATCHED: batched products exist"
                      : bit == COAST_MM_GROUPED ? "COAST_MM_GROUPED: grouped products exist" : "COAST_MM_B_TRANSPOSED: a transposed B exists";
-    return fail(COAST_ERR_BAD_ARG, "%s for MM_U32, GEMM_TF32 and GEMM_BF16 only (kernel %u)", what, d->kernel);
+    return fail(COAST_ERR_BAD_ARG, "%s for MM_U32, GEMM_TF32 and GEMM_BF16 only, plus GEMM_FP8 (kernel %u)", what, d->kernel);
 }
 /* The checks shared by coast_launch and coast_run_host: a matmul mode bit on another kernel, then the shape of a batch or of
  * groups.  Fills *m for the matmul kernels. */
@@ -617,19 +622,29 @@ static int mm_check(const coast_launch_desc* d, mm_shape* m) {
 static uint64_t mm_row_tiles(const mm_shape* m, unsigned bm) { return m->rows / bm + (m->grouped ? m->P : 0); }
 
 /* A matmul kernel's name: stem, path variant, [_bt], [_grp], then _nc<n>_inj<i> for the kernels that came before batched,
- * grouped, BF16 and transposed-B launches and _inj<i>_nc<n> for the others */
-static void mm_kernel_name(char* name, const char* stem, const char* variant, int bt, int grouped, int bf16, uint32_t nc, int inj) {
-    if (bt || grouped || bf16) snprintf(name, 64, "%s%s%s%s_inj%d_nc%u", stem, variant, bt ? "_bt" : "", grouped ? "_grp" : "", inj, nc);
+ * grouped, BF16 and transposed-B launches and _inj<i>_nc<n> for the others.  GEMM_FP8's names are whole formats: one set of
+ * kernels serves B and B^T, the narrow kernel exists at NC 1 only, and the grouped ones (always 128 x 128 tiles) carry no variant. */
+static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, uint32_t nc, int inj) {
+    if (kernel == COAST_K_GEMM_FP8) {
+        const char* f = grouped ? "xmr_gemm_fp8_grp_inj%d_nc%u" : *variant == 'p' ? "xmr_gemm_fp8p_inj%d_nc%u"
+                      : *variant == 'n' ? "xmr_gemm_fp8n_inj%d_nc1" : "xmr_gemm_fp8_inj%d_nc%u";
+        snprintf(name, 64, f, inj, nc);
+        return;
+    }
+    const char* stem = kernel == COAST_K_MM_U32 ? "xmr_mm_u32" : kernel == COAST_K_GEMM_BF16 ? "xmr_gemm_bf16" : "xmr_gemm_tf32";
+    if (bt || grouped || kernel == COAST_K_GEMM_BF16)
+        snprintf(name, 64, "%s%s%s%s_inj%d_nc%u", stem, variant, bt ? "_bt" : "", grouped ? "_grp" : "", inj, nc);
     else snprintf(name, 64, "%s%s_nc%u_inj%d", stem, variant, nc, inj);
 }
 
-/* Pre-passes of the wgmma kernels: TF32 wgmma reads both operands K-major, so B (K x N, row-major) is transposed into scratch;
+/* Pre-passes of the wgmma kernels: TF32 and FP8 wgmma read both operands K-major, so B (K x N, row-major) is transposed into
+ * scratch (4-byte or 1-byte elements);
  * the limb kernel splits A and B into u8 limb planes ([plane][rows][K] and, transposed, [plane][P N][K]).  The products' B
  * matrices become one stacked (P N) x K operand; their A matrices already are one matrix. */
 static int prepass_transpose_b(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr bt, CUstream s) {
     const void* B = d->d_aux; unsigned int k32 = d->K, n32 = d->N, nb = (unsigned)L->mm.P;
     void* params[] = { &B, &bt, &k32, &n32, &nb };
-    return launch_small("xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
+    return launch_small(L->mm.es == 1 ? "xmr_gemm_bt_u8" : "xmr_gemm_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params, s);
 }
 /* A's rows (groups: the R rows from row ro[0]), then the B^T planes [plane][p N + n][k]: split_bt transposes B; a caller's B^T
  * (COAST_MM_B_TRANSPOSED) already has that row order, so the streaming split of A makes them from its (P N) rows of K. */
@@ -650,7 +665,7 @@ static int prepass_split_limbs(const launch_plan* L, const coast_launch_desc* d,
     void* params_b[] = { &B, &pb, &k32, &n32, &nb };
     return launch_small("xmr_mm_split_bt", (unsigned)G.sm_count * 8u, XMR_PREPASS_THREADS, params_b, s);
 }
-/* tile_start of the products (xmr_mm_group_scan, one CTA) into the group block; for TF32 and BF16 (a_map) it also rebases the host's A map
+/* tile_start of the products (xmr_mm_group_scan, one CTA) into the group block; for TF32, BF16 and FP8 (a_map) it also rebases the host's A map
  * onto row ro[0] of d_in with R rows, so no host-side read of the device table is needed */
 static int prepass_group_scan(const launch_plan* L, const coast_launch_desc* d, CUdeviceptr grp, const CUtensorMap* a_map, CUstream s) {
     const void* ro = d->d_rows; const void* base = d->d_in;
@@ -741,7 +756,7 @@ static int run_plan(const launch_plan* L, const coast_launch_desc* d, xmr_args* 
 static int launch_impl(const coast_launch_desc* d, void* stream) {
     int rc = ensure_ctx(); if (rc) return rc;
     if (!d) return fail(COAST_ERR_BAD_ARG, "null descriptor");
-    if (d->kernel >= COAST_K_COUNT_) return fail(COAST_ERR_BAD_ARG, "unknown kernel id %u", d->kernel);
+    if (!known_kernel(d->kernel)) return fail(COAST_ERR_BAD_ARG, "unknown kernel id %u", d->kernel);
     if (d->num_clones < 1 || d->num_clones > 3) return fail(COAST_ERR_BAD_ARG, "num_clones must be 1, 2 (DWC) or 3 (TMR)");
     const int ragged = (d->mode & COAST_UNIT_OFFSETS) != 0;
     if (ragged && (rc = ragged_check(d))) return rc;
@@ -878,7 +893,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
             L.ctas = mm_row_tiles(&m, XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;   /* grouped: surplus CTAs exit */
             L.grp_tm = XMR_MMT_BM; L.grp_tiles_n = d->N / XMR_MMT_BN;
         }
-        mm_kernel_name(L.name, "xmr_mm_u32", variant, bt_name, m.grouped, 0, nc, inj);
+        mm_kernel_name(L.name, d->kernel, variant, bt_name, m.grouped, nc, inj);
         break;
     }
     case COAST_K_QSORT:
@@ -916,13 +931,16 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         break;
     }
     case COAST_K_GEMM_TF32:
-    case COAST_K_GEMM_BF16: {
-        /* one body for both operand types (xmr_gemm_tf32.cuh): fp32 operands read as TF32, B^T K-major from a transposing pre-pass
-         * into scratch; or bfloat16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch) */
-        const int bf16 = d->kernel == COAST_K_GEMM_BF16;
-        const char* TY = bf16 ? "BF16" : "TF32";
-        const unsigned bk = bf16 ? XMR_GEMM_BF16_BK : XMR_GEMM_BK;
-        const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    case COAST_K_GEMM_BF16:
+    case COAST_K_GEMM_FP8: {
+        /* one body for every operand type (xmr_gemm_tf32.cuh): fp32 operands read as TF32, B^T K-major from a transposing pre-pass
+         * into scratch; bfloat16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch); or E4M3 operands,
+         * 128-element k-blocks and, as for TF32, B^T K-major from a byte-transposing pre-pass */
+        const int bf16 = d->kernel == COAST_K_GEMM_BF16, fp8 = d->kernel == COAST_K_GEMM_FP8;
+        const char* TY = fp8 ? "FP8" : bf16 ? "BF16" : "TF32";
+        const unsigned bk = fp8 ? XMR_GEMM_FP8_BK : bf16 ? XMR_GEMM_BF16_BK : XMR_GEMM_BK;
+        const CUtensorMapDataType dt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                                                 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
         if (m.grouped && (d->N % xmr_gemm_bn(0) || d->K % bk))
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_%s grouped tiles are 128 x 128 x %u: N must be a multiple of 128 and K of %u "
                                                "(got %u, %u); the products' rows are free", TY, bk, bk, d->N, d->K);
@@ -939,9 +957,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         const char* e = getenv("COAST_GEMM_PAIR");
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
         const int pair = !m.grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
-        /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it, TF32 only skips the transposing pre-pass */
-        mm_kernel_name(L.name, bf16 ? "xmr_gemm_bf16" : "xmr_gemm_tf32", pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt,
-                       m.grouped, bf16, nc, inj);
+        /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it, TF32 and FP8 only skip the transposing pre-pass */
+        mm_kernel_name(L.name, d->kernel, pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt, m.grouped, nc, inj);
         { const char* g = getenv("COAST_GEMM_GROUP_M");
           if (g && atoi(g) > 0 && atoi(g) <= (int)XMR_MODE_GROUP_M_MASK) a.mode = (a.mode & ~XMR_MODE_GROUP_M_MASK) | (unsigned)atoi(g); }
         /* L2 eviction priorities: A evict_last, B and C evict_first; COAST_GEMM_L2_HINTS=0 loads and stores with the normal policy */
@@ -956,7 +973,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         const int b_scratch = !bf16 && !m.bt;
         const uintptr_t b_base = b_scratch ? 0 : (uintptr_t)d->d_aux;
         if (b_scratch) {
-            L.scratch = (size_t)m.P * d->K * d->N * 4u;
+            L.scratch = (size_t)m.P * d->K * d->N * m.es;
             L.prepass = prepass_transpose_b;
         }
         L.n_maps = 2;

@@ -20,6 +20,9 @@
 // wgmma m64n128k16.  16-bit wgmma can read B MN-major, which is what a row-major K x N matrix is, so B is loaded in place from
 // the caller's buffer: no pre-pass and no scratch.  A BF16 B^T (COAST_MM_B_TRANSPOSED) is read in place K-major (Bf16T, the
 // xmr_gemm_bf16*_bt_* kernels).
+// And FP8 operands (xmr_gemm_fp8*, operand type Fp8): E4M3 A and B, fp32 C, wgmma m64n128k32.  The 8-bit wgmma has no transpose
+// immediates, so B is read K-major only: as for TF32, a byte-transposing pre-pass (xmr_gemm_bt_u8) writes B^T into scratch, and
+// a caller's B^T (COAST_MM_B_TRANSPOSED) is read in place by the same kernels.
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, 64 rows of the 128-row tile each.
 // Persistent CTAs, one per SM.  Tiles: 128 x 256 unprotected (N % 256 == 0), 128 x 128 otherwise; the accumulators of a
 // replica are 64 x 128 wgmma fragments (64 fp32 registers per thread), so TMR holds 192 accumulator registers per thread.
@@ -157,6 +160,14 @@ __device__ __forceinline__ void wgmma_bf16_m64n128k16(float (&d)[64], uint64_t d
         : "l"(da), "l"(db), "n"(TRANS_B));
 }
 
+// D (+)= A . B^T with both operands K-major, E4M3 x E4M3 (the 8-bit wgmma takes no transpose immediates); D's fragment layout as above
+__device__ __forceinline__ void wgmma_e4m3_m64n128k32(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db));
+}
+
 // The operand types of gemm_body.  Both stage 128-byte k-blocks (BK elements) and step A's descriptor by 32 bytes (WG_K elements)
 // per wgmma; they differ in the instruction and in how B reaches shared memory:
 //   Tf32: B^T rows from the transposing pre-pass, K-major like A; TMA boxes of B_BOX rows of B^T at 128 bytes per row;
@@ -187,6 +198,17 @@ struct Bf16T {
     static constexpr __host__ __device__ int b_box(bool pair) { return (int)xmr_gemm_b_box(pair); }
     static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc(saddr); }
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_bf16_m64n128k16<0>(d, da, db); }
+};
+//   Fp8: E4M3 operands, B^T K-major like Tf32's (the pre-pass's scratch or the caller's B^T): a k-block is 128 elements, the same
+//        128-byte row, and a k32 step is 32 bytes, the same descriptor step as Tf32's.  The accumulator is the wgmma's own
+//        (DESIGN.md §6: for FP8 it is narrower than fp32), as with torch._scaled_mm(use_fast_accum=True).
+struct Fp8 {
+    static constexpr int BK = XMR_GEMM_FP8_BK, WG_K = 32;
+    static constexpr bool B_IN_PLACE = false;
+    static constexpr uint32_t B_KSTEP = 32 >> 4;
+    static constexpr __host__ __device__ int b_box(bool pair) { return (int)xmr_gemm_b_box(pair); }
+    static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc(saddr); }
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_e4m3_m64n128k32(d, da, db); }
 };
 
 __device__ __forceinline__ void wgmma_u8_m64n32k32(uint32_t (&d)[16], uint64_t da, uint64_t db) {
@@ -447,6 +469,32 @@ xmr_gemm_bt(const float* __restrict__ B, float* __restrict__ Bt, unsigned int K,
     }
 }
 
+// B (batch x K x N bytes, row-major) -> B^T ((batch N) x K bytes): xmr_gemm_bt for 1-byte elements (GEMM_FP8).  64 x 64-byte
+// tiles through shared memory; each thread moves 4-byte words both ways and packs four bytes of a column into one word.
+extern "C" __global__ void __launch_bounds__(XMR_PREPASS_THREADS)
+xmr_gemm_bt_u8(const uint8_t* __restrict__ B, uint8_t* __restrict__ Bt, unsigned int K, unsigned int N, unsigned int batch) {
+    __shared__ uint32_t tile[64][17];                    // [k][n / 4]: a 68-byte row keeps a column's bytes on different banks
+    const uint8_t* t8 = reinterpret_cast<const uint8_t*>(tile);
+    const unsigned int tiles_n = N / 64u, tiles_k = K / 64u;
+    const unsigned long long per = (unsigned long long)tiles_n * tiles_k, n_tiles = per * batch;
+    for (unsigned long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const unsigned long long b = t / per;
+        const unsigned int w = (unsigned int)(t - b * per), k0 = (w / tiles_n) * 64u, n0 = (w % tiles_n) * 64u;
+        const uint8_t* Bb = B + b * K * N;
+        uint8_t* Btb = Bt + b * N * K;
+        for (int i = threadIdx.x; i < 1024; i += XMR_PREPASS_THREADS)
+            tile[i >> 4][i & 15] = __ldg(reinterpret_cast<const uint32_t*>(Bb + (size_t)(k0 + (i >> 4)) * N + n0) + (i & 15));
+        __syncthreads();
+        for (int i = threadIdx.x; i < 1024; i += XMR_PREPASS_THREADS) {
+            const int n = i >> 4, k = 4 * (i & 15);
+            const uint32_t v = (uint32_t)t8[k * 68 + n] | (uint32_t)t8[(k + 1) * 68 + n] << 8 | (uint32_t)t8[(k + 2) * 68 + n] << 16 |
+                               (uint32_t)t8[(k + 3) * 68 + n] << 24;
+            reinterpret_cast<uint32_t*>(Btb + (size_t)(n0 + n) * K + k0)[i & 15] = v;
+        }
+        __syncthreads();
+    }
+}
+
 #define XMR_GEMM_KERNEL(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER)                                            \
     extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                      \
     NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b) { \
@@ -528,3 +576,25 @@ XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj1_nc2, 2, 1, false)
 XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj1_nc3, 3, 1, false)
 XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16n_bt_grp_inj0_nc1, 1, 0, false)
 XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16n_bt_grp_inj1_nc1, 1, 1, false)
+// FP8 (E4M3) operands: the variants of TF32, one set for B and B^T (B^T from the byte pre-pass or the caller); named
+// _inj<i>_nc<n>, the grouped nc1 kernel without the n (grouped tiles are always 128 x 128)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj0_nc1, 1, 0, false)
+XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj0_nc2, 2, 0, false)
+XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj0_nc3, 3, 0, false)
+XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc1, 1, 1, false)
+XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc2, 2, 1, false)
+XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc3, 3, 1, false)

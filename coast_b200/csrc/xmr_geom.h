@@ -91,6 +91,8 @@ XMR_GEOM_FN unsigned xmr_gemm_smem(int wide) {
  * (128 bytes, the widest row the 128-byte swizzle takes) x BK k-rows, for single CTAs and pairs alike */
 #define XMR_GEMM_BF16_BK    64u
 #define XMR_GEMM_BF16_B_BOX 64u
+/* FP8 (E4M3): BK = 128 bytes, the same row again; B^T only (8-bit wgmma reads B K-major), in TF32's boxes of B^T rows */
+#define XMR_GEMM_FP8_BK     128u
 /* limbs: BK = 128 u8 of 4 planes, 2 stages; BN = 64 unprotected, 32 protected (register accumulators) */
 #define XMR_MMTC_BK     128u
 #define XMR_MMTC_STAGES 2u
@@ -122,7 +124,7 @@ XMR_GEOM_FN unsigned xmr_mmtc_smem(unsigned nc) {
 XMR_GEOM_FN unsigned long long xmr_ragged_scratch(unsigned long long n_units) { return XMR_RAGGED_PERM + 4ull * n_units; }
 XMR_GEOM_FN unsigned long long xmr_ragged_slots(unsigned long long n_units) { return (xmr_ragged_scratch(n_units) + 127ull) & ~127ull; }
 
-/* ---- grouped matmuls (COAST_MM_GROUPED, xmr_mm_grp.cuh): a group block in scratch = the rebased TF32 / BF16 A tensor map (128 bytes),
+/* ---- grouped matmuls (COAST_MM_GROUPED, xmr_mm_grp.cuh): a group block in scratch = the rebased TF32 / BF16 / FP8 A tensor map (128 bytes),
  * then tile_start[G + 1] (u32), written by a one-CTA scan; at most XMR_MM_GRP_MAX groups per launch ---- */
 #define XMR_MM_GRP_SCAN_THREADS 1024
 #define XMR_MM_GRP_TILES        128u

@@ -13,19 +13,22 @@ from dataclasses import dataclass
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 K_CRC16, K_SHA256, K_AES128, K_MM_U32, K_GEMM_TF32, K_QSORT, K_CHSTONE_SHA, K_CHSTONE_AES, K_GEMM_BF16 = range(9)
+K_GEMM_FP8 = 10                              # FP8 E4M3 operands, fp32 out; id 9 is unassigned
 F_COUNT_ERRORS, F_COUNT_SYNCS, F_NO_MEM_REPLICATION = 0x1, 0x2, 0x4
 F_INTERLEAVE, F_SEGMENT, F_VERBOSE, F_MAJORITY_VOTER = 0x8, 0x10, 0x20, 0x100
 F_STORE_DATA_SYNC, F_NO_STORE_DATA_SYNC, F_NO_LOAD_SYNC, F_NO_STORE_ADDR_SYNC = 0x200, 0x400, 0x800, 0x1000
 PLAN_NONE, PLAN_BERNOULLI, PLAN_TABLE = 0, 1, 2
 AES_DECRYPT, AES_KEY_PER_UNIT, AES_KEY_WRITEBACK = 1, 2, 4
 UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 / QSORT batches: aux = n_units + 1 u64 byte offsets into inp
-MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32 / GEMM_BF16: n_units = batch*M*N, inp / aux / out hold batch A / B / C
-MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32 / GEMM_BF16: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
-MM_B_TRANSPOSED = COAST_MM_B_TRANSPOSED = 0x80000  # MM_U32 / GEMM_TF32 / GEMM_BF16: aux holds B^T, N x K per product (nn.Linear.weight)
+MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8: n_units = batch*M*N, inp / aux / out hold batch A / B / C
+MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
+MM_B_TRANSPOSED = COAST_MM_B_TRANSPOSED = 0x80000  # MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8: aux holds B^T, N x K per product (nn.Linear.weight)
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 
-OUT_BYTES = {K_CRC16: 2, K_SHA256: 32, K_AES128: 16, K_MM_U32: 4, K_GEMM_TF32: 4, K_CHSTONE_SHA: 20, K_CHSTONE_AES: 64, K_GEMM_BF16: 4}
+OUT_BYTES = {K_CRC16: 2, K_SHA256: 32, K_AES128: 16, K_MM_U32: 4, K_GEMM_TF32: 4, K_CHSTONE_SHA: 20, K_CHSTONE_AES: 64, K_GEMM_BF16: 4,
+             K_GEMM_FP8: 4}
+MM_ELEM_BYTES = {K_GEMM_BF16: 2, K_GEMM_FP8: 1}   # bytes per A and B element of the matmuls; 4 for MM_U32 and GEMM_TF32
 
 
 def out_bytes(kernel: int, unit_bytes: int = 0) -> int:
@@ -274,10 +277,11 @@ class Runtime:
     def run(self, kernel, num_clones, inp, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0, aux=None,
             key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, out=None, stream=None, status=None, rows=None):
         """rows: with MM_GROUPED, the CUDA int64/uint64 tensor of M + 1 row offsets (M = the product count).
-        K_GEMM_BF16: inp and aux are torch.bfloat16 tensors (or their uint16 / int16 views); the result is fp32 like K_GEMM_TF32's."""
+        K_GEMM_BF16: inp and aux are torch.bfloat16 tensors (or their uint16 / int16 views); the result is fp32 like K_GEMM_TF32's.
+        K_GEMM_FP8: inp and aux are torch.float8_e4m3fn tensors (or their uint8 views); the result is fp32."""
         torch = self.torch
         if mode & MM_GROUPED:
-            self._check_rows(rows, M, N, n_units, inp, K, out, 2 if kernel == K_GEMM_BF16 else 4)
+            self._check_rows(rows, M, N, n_units, inp, K, out, MM_ELEM_BYTES.get(kernel, 4))
         ragged_qsort = bool(mode & UNIT_OFFSETS) and kernel == K_QSORT
         if out is None and ragged_qsort:       # the arrays are sorted into the bytes they came from: out mirrors inp
             out = torch.zeros(inp.numel() * inp.element_size(), dtype=torch.uint8, device=f"cuda:{self.device}")
