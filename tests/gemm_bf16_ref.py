@@ -1,4 +1,4 @@
-"""The CPU reference of COAST_K_GEMM_BF16, shared by tests/test_gemm_bf16_oracle.py and tests/test_gpu_gemm_bf16.py.
+"""The CPU reference of COAST_K_GEMM_BF16, shared by tests/test_gemm_bf16_oracle.py and tests/test_gpu_gemm_bf16_fp8.py.
 
 numpy has no bfloat16: operands are uint16 bit patterns.  A bfloat16 is an fp32 whose low 16 bits are zero, so widening is a
 shift and exact for every pattern (zeros, denormals, infinities, NaNs), and the TF32 truncation of the oracle's GEMM_TF32

@@ -1,4 +1,4 @@
-"""The CPU reference of COAST_K_GEMM_FP8, shared by tests/test_gemm_fp8_oracle.py and tests/test_gpu_gemm_fp8.py.
+"""The CPU reference of COAST_K_GEMM_FP8, shared by tests/test_gemm_fp8_oracle.py and tests/test_gpu_gemm_bf16_fp8.py.
 
 numpy has no FP8: operands are uint8 bit patterns of E4M3, the OCP encoding torch.float8_e4m3fn uses (sign, 4 exponent bits
 with bias 7, 3 mantissa bits; exponent 0 is subnormal, S.1111.111 is NaN and there are no infinities).  Every E4M3 value is an

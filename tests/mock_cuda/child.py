@@ -201,6 +201,7 @@ def main():
             out.append(r)
         elif kind == "shutdown":
             out.append({"rc": L.coast_shutdown()})
+    L.coast_shutdown()                                      # a no-op after a "shutdown" op; the mock reports what is still live
     res["ops"] = out
     print(json.dumps(res))
 

@@ -1,11 +1,11 @@
 /*
  * mock_cuda.c -- a stand-in for libcuda.so.1 that lets the HOST logic of libcoast_rt.so run on a GPU-less box.
  *
- * TEST INFRASTRUCTURE ONLY (tests/test_host_logic.py builds it into a temp dir and puts that dir on LD_LIBRARY_PATH of a
+ * TEST INFRASTRUCTURE ONLY (tests/mock_run.py builds it into a temp dir and puts that dir on LD_LIBRARY_PATH of a
  * child process).  It executes NO workload: kernels are recorded, not run.  What it does check, the way the real driver
  * would fail: every copy stays inside a live allocation, launch geometry and dynamic shared memory are within sm_90
- * limits, tensor maps obey the cuTensorMapEncodeTiled constraints, nothing leaks at exit.  Every call that matters is
- * appended as one JSON line to $MOCK_CUDA_LOG.
+ * limits, tensor maps obey the cuTensorMapEncodeTiled constraints for their element type (UINT8, BFLOAT16, UINT32,
+ * FLOAT32), nothing leaks at exit.  Every call that matters is appended as one JSON line to $MOCK_CUDA_LOG.
  */
 #include <cuda.h>
 #include <elf.h>
@@ -224,7 +224,13 @@ CUresult cuTensorMapEncodeTiled(CUtensorMap* map, CUtensorMapDataType dt, cuuint
                                 const cuuint64_t* gstr, const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapInterleave il,
                                 CUtensorMapSwizzle swz, CUtensorMapL2promotion l2, CUtensorMapFloatOOBfill oob) {
     (void)l2; (void)oob;
-    const size_t es = dt == CU_TENSOR_MAP_DATA_TYPE_UINT8 ? 1 : 4;
+    size_t es;
+    switch (dt) {
+    case CU_TENSOR_MAP_DATA_TYPE_UINT8: es = 1; break;
+    case CU_TENSOR_MAP_DATA_TYPE_BFLOAT16: es = 2; break;
+    case CU_TENSOR_MAP_DATA_TYPE_UINT32: case CU_TENSOR_MAP_DATA_TYPE_FLOAT32: es = 4; break;
+    default: return bad("tensor map data type");
+    }
     if (rank < 1 || rank > 5) return bad("tensor map rank");
     if (((uintptr_t)addr) & 15u) return bad("tensor map: global address must be 16-byte aligned");
     if (il != CU_TENSOR_MAP_INTERLEAVE_NONE) return bad("tensor map interleave");
@@ -245,7 +251,7 @@ CUresult cuTensorMapEncodeTiled(CUtensorMap* map, CUtensorMapDataType dt, cuuint
     if (find_alloc((uintptr_t)addr, extent) < 0) return bad("tensor map covers memory outside a live allocation");
     size_t box_bytes = es; for (cuuint32_t i = 0; i < rank; ++i) box_bytes *= box[i];
     memset(map, 0, sizeof *map);
-    LOG("{\"op\":\"tmap\",\"rank\":%u,\"elem\":%zu,\"dim0\":%llu,\"dim1\":%llu,\"box0\":%u,\"box1\":%u,\"box_bytes\":%zu,\"swizzle\":%d}", rank, es,
-        (unsigned long long)gdim[0], (unsigned long long)(rank > 1 ? gdim[1] : 1), box[0], rank > 1 ? box[1] : 1, box_bytes, (int)swz);
+    LOG("{\"op\":\"tmap\",\"addr\":%llu,\"rank\":%u,\"elem\":%zu,\"dim0\":%llu,\"dim1\":%llu,\"box0\":%u,\"box1\":%u,\"box_bytes\":%zu,\"swizzle\":%d}",
+        (unsigned long long)(uintptr_t)addr, rank, es, (unsigned long long)gdim[0], (unsigned long long)(rank > 1 ? gdim[1] : 1), box[0], rank > 1 ? box[1] : 1, box_bytes, (int)swz);
     return CUDA_SUCCESS;
 }

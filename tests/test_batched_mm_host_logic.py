@@ -1,43 +1,13 @@
 """Host logic of batched matmuls (COAST_MM_BATCHED with COAST_K_MM_U32 and COAST_K_GEMM_TF32) on a GPU-less box, against the
-mock driver (tests/mock_cuda/mock_cuda.c).  A batch is `batch` products of one shape: the stacked A and C are one (batch*M)-row
+mock driver (tests/mock_cuda/mock_cuda.c) through tests/mock_cuda/mm_child.py.  A batch is `batch` products of one shape: the stacked A and C are one (batch*M)-row
 matrix, and the B matrices become one stacked (batch*N) x K operand in the pre-pass.  Pinned here: the kernel and pre-passes
 each path selects, the tensor maps of the stacked operands, the scratch and the grid; the TF32 CTA pair's need for a per-product
 M that is a multiple of 256; every refusal; a batch of one being the unbatched launch, event for event; and the chunks of whole
 products of the host call."""
-import json
-import os
-import subprocess
-import sys
-
 import pytest
 
-from test_host_logic import ROOT, args_of, mock_dir  # noqa: F401  (mock_dir is a fixture)
-
-MM_BATCHED = 0x20000
-K_CRC16, K_MM_U32, K_GEMM_TF32 = 0, 3, 4
-BAD_ARG, UNSUPPORTED = -100003, -100004
-SMS = 132
-
-
-def run(mock_dir, tmp_path, ops, env_extra=None):
-    log = tmp_path / "mock.log"
-    if log.exists():
-        log.unlink()
-    env = dict(os.environ, LD_LIBRARY_PATH=f"{mock_dir}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=str(log))
-    for k in ("COAST_MM_PATH", "COAST_GEMM_PAIR", "COAST_HOST_CHUNK_BYTES", "COAST_HOST_PATH"):
-        env.pop(k, None)
-    env.update(env_extra or {})
-    res = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mock_cuda", "batched_mm_child.py"),
-                          json.dumps({"ops": ops})], capture_output=True, text=True, env=env, timeout=300)
-    assert res.returncode == 0, res.stdout + res.stderr
-    events = [json.loads(ln) for ln in open(log)] if log.exists() else []
-    assert not [e for e in events if e["op"] == "error"], [e for e in events if e["op"] == "error"]
-    assert events[-1] == {"op": "exit", "live_allocations": 0}
-    return json.loads(res.stdout.strip().splitlines()[-1]), events
-
-
-def work(ev):
-    return [e for e in ev if e["op"] == "launch" and e["name"] != "xmr_counters_reset"]
+from mock_run import (BAD_ARG, K_CRC16, K_GEMM_TF32, K_MM_U32, MM_BATCHED, SMS, UNSUPPORTED, args_of, mock_dir,  # noqa: F401
+                      run, spans, work)
 
 
 # (id, kernel, nc, M, N, K, batch, env, launches in order, grid, scratch bytes or None)
@@ -60,10 +30,10 @@ PATHS = [
 @pytest.mark.parametrize("case", PATHS, ids=[c[0] for c in PATHS])
 def test_each_path_runs_its_prepasses_and_kernel_on_the_stacked_operands(mock_dir, tmp_path, case):
     _, kernel, nc, M, N, K, batch, env, want, grid, scratch = case
-    res, ev = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=nc, M=M, N=N, K=K, batch=batch, unit_base=1 << 32,
-                                            flags=3)], env_extra=env)
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=nc, M=M, N=N, K=K, batch=batch, unit_base=1 << 32,
+                                               flags=3)], env_extra=env)
     r = res["ops"][0]
-    assert r["rc"] == [0], r["err"]
+    assert r["rc"] == 0, r["err"]
     la = work(ev)
     assert [e["name"] for e in la] == want and len({e["stream"] for e in la}) == 1
     k = la[-1]
@@ -75,7 +45,7 @@ def test_each_path_runs_its_prepasses_and_kernel_on_the_stacked_operands(mock_di
     tm = [e for e in ev if e["op"] == "tmap"]
     allocs = [e for e in ev if e["op"] == "alloc"]
     if scratch is None:
-        assert not tm and allocs[-1]["bytes"] == batch * M * N * 4   # the caller's C buffer was the last allocation
+        assert not tm and allocs[-1]["ptr"] == r["out"]             # the caller's C buffer was the last allocation
         return
     assert [(t["dim0"], t["dim1"]) for t in tm] == [(K, batch * M), (K, batch * N)]   # A: batch*M rows; B^T: batch*N rows
     assert allocs[-1]["bytes"] == scratch                             # the launch's one scratch allocation
@@ -89,19 +59,20 @@ def test_each_path_runs_its_prepasses_and_kernel_on_the_stacked_operands(mock_di
     (2, 256, 128, {}, "xmr_gemm_tf32p_nc2_inj0"),                    # M = 256 per product: pairs
 ])
 def test_a_cta_pair_needs_the_per_product_rows(mock_dir, tmp_path, nc, M, N, env, want):
-    res, ev = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=nc, M=M, N=N, K=32, batch=4)], env_extra=env)
-    assert res["ops"][0]["rc"] == [0]
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=nc, M=M, N=N, K=32, batch=4)], env_extra=env)
+    assert res["ops"][0]["rc"] == 0
     assert work(ev)[-1]["name"] == want
 
 
+TINY = [16, 16, 16]                                   # element counts of A, B and C: a refusal needs no memory
 REFUSALS = [
     ("other_kernel", dict(kernel=K_CRC16, M=8, N=8, K=8, batch=2), BAD_ARG, "COAST_MM_BATCHED"),
-    ("zero_units", dict(M=8, N=8, K=8, batch=0, alloc_batch=1), BAD_ARG, "COAST_MM_BATCHED"),
+    ("zero_units", dict(M=8, N=8, K=8, batch=0, alloc=TINY), BAD_ARG, "COAST_MM_BATCHED"),
     ("not_a_multiple", dict(M=8, N=8, K=8, n=2 * 64 + 1, batch=3), BAD_ARG, "multiple of M*N"),
-    ("zero_M", dict(M=0, N=8, K=8, n=64, batch=1, alloc_batch=1), BAD_ARG, "COAST_MM_BATCHED"),
-    ("batch_M_2p31", dict(M=1 << 16, N=1, K=1, batch=1 << 15, alloc_batch=1), BAD_ARG, "below 2^31"),
-    ("batch_N_2p31", dict(M=1, N=1 << 16, K=1, batch=1 << 15, alloc_batch=1), BAD_ARG, "below 2^31"),
-    ("tf32_batch_M_2p31", dict(kernel=K_GEMM_TF32, M=128, N=128, K=32, batch=1 << 24, alloc_batch=1), BAD_ARG, "below 2^31"),
+    ("zero_M", dict(M=0, N=8, K=8, n=64, batch=1, alloc=TINY), BAD_ARG, "COAST_MM_BATCHED"),
+    ("batch_M_2p31", dict(M=1 << 16, N=1, K=1, batch=1 << 15, alloc=TINY), BAD_ARG, "below 2^31"),
+    ("batch_N_2p31", dict(M=1, N=1 << 16, K=1, batch=1 << 15, alloc=TINY), BAD_ARG, "below 2^31"),
+    ("tf32_batch_M_2p31", dict(kernel=K_GEMM_TF32, M=128, N=128, K=32, batch=1 << 24, alloc=TINY), BAD_ARG, "below 2^31"),
     ("tf32_shape", dict(kernel=K_GEMM_TF32, M=100, N=128, K=64, batch=4), UNSUPPORTED, "multiples of 128"),
     ("unbatched_n", dict(M=8, N=8, K=8, n=2 * 64, batch=2, mode=0), BAD_ARG, "n_units must be M*N"),
     ("unbatched_tf32_n", dict(kernel=K_GEMM_TF32, M=128, N=128, K=32, n=2 * 128 * 128, batch=2, mode=0), BAD_ARG,
@@ -116,10 +87,9 @@ CALLS = [(call, c) for call in ("launch", "run_host") for c in REFUSALS if call 
 @pytest.mark.parametrize("call,case", CALLS, ids=[f"{call}-{c[0]}" for call, c in CALLS])
 def test_refusals_fail_loudly_before_any_work(mock_dir, tmp_path, call, case):
     _, op, code, needle = case
-    res, ev = run(mock_dir, tmp_path, [dict(op=call, **op)])
+    res, ev, _ = run(mock_dir, tmp_path, [{"op": call, "kernel": K_MM_U32, **op}])
     r = res["ops"][0]
-    rc, err = (r["rc"][0], r["err"][0]) if call == "launch" else (r["rc"], r["err"])
-    assert rc == code and needle in err, r
+    assert r["rc"] == code and needle in r["err"], r
     assert not work(ev)
     if code == BAD_ARG:                    # the batch checks come before any copy; a path's shape rule at the first chunk's launch
         assert not [e for e in ev if e["op"] in ("h2d", "d2h")]
@@ -136,11 +106,12 @@ def test_refusals_fail_loudly_before_any_work(mock_dir, tmp_path, call, case):
 ])
 def test_a_batch_of_one_is_the_unbatched_launch(mock_dir, tmp_path, kernel, nc, M, N, K, env):
     """the same buffers launched with and without the bit: the same kernels, grids, argument blocks, tensor maps and scratch"""
-    res, ev = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=nc, M=M, N=N, K=K, batch=1, twice=True, p=0.5,
-                                            unit_base=77, flags=3)], env_extra=env)
-    assert res["ops"][0]["rc"] == [0, 0]
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=nc, M=M, N=N, K=K, batch=1, twice=True, p=0.5,
+                                               unit_base=77, flags=3)], env_extra=env)
+    assert [r["rc"] for r in res["ops"]] == [0, 0]
     start = [i for i, e in enumerate(ev) if e["op"] == "alloc"][4] + 1          # after the counters and the caller's three buffers
-    seen = [{k: v for k, v in e.items() if k not in ("id", "ptr")} for e in ev[start:] if e["op"] in ("launch", "tmap", "alloc")]
+    # each launch allocates its own scratch: its address, and the maps' on it, may differ
+    seen = [{k: v for k, v in e.items() if k not in ("id", "ptr", "addr")} for e in ev[start:] if e["op"] in ("launch", "tmap", "alloc")]
     assert len(seen) % 2 == 0 and len(seen) >= 2
     assert seen[: len(seen) // 2] == seen[len(seen) // 2:]
     assert sum(e["op"] == "launch" for e in seen) >= 2
@@ -155,16 +126,13 @@ def test_a_batch_of_one_is_the_unbatched_launch(mock_dir, tmp_path, kernel, nc, 
 ])
 def test_host_call_chunks_are_whole_products(mock_dir, tmp_path, kernel, M, N, K, batch, budget, per, pinned):
     env = {"COAST_HOST_CHUNK_BYTES": str(budget)} if budget else {}
-    res, ev = run(mock_dir, tmp_path, [dict(op="run_host", kernel=kernel, nc=3, M=M, N=N, K=K, batch=batch, unit_base=1000,
-                                            pinned=pinned)], env_extra=env)
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=kernel, nc=3, M=M, N=N, K=K, batch=batch, unit_base=1000,
+                                               pinned=pinned)], env_extra=env)
     r = res["ops"][0]
     assert r["rc"] == 0 and r["path"] == "staged", r
     ab, bb, cb = 4 * M * K, 4 * K * N, 4 * M * N
-
-    def spans(op, base, size):
-        return [((e["host"] - base), e["bytes"], e["stream"]) for e in ev if e["op"] == op and base <= e["host"] < base + size]
-    ups_a, ups_b = spans("h2d", r["host_in"], batch * ab), spans("h2d", r["host_aux"], batch * bb)
-    downs = spans("d2h", r["host_out"], batch * cb)
+    ups_a, ups_b = spans(ev, "h2d", r["host_in"], batch * ab), spans(ev, "h2d", r["host_aux"], batch * bb)
+    downs = spans(ev, "d2h", r["host_out"], batch * cb)
     la = [e for e in work(ev) if "_nc" in e["name"]]
     chunks = [(f, min(per, batch - f)) for f in range(0, batch, per)]
     assert len(ups_a) == len(ups_b) == len(downs) == len(la) == len(chunks)

@@ -1,65 +1,21 @@
-"""Host logic of COAST_K_GEMM_FP8 on a GPU-less box, against the mock driver (tests/mock_cuda/mock_cuda_bt.c, which logs where
-each tensor map starts) and the transposed-B child (tests/mock_cuda/mm_bt_child.py; it sizes the buffers generously).  Pinned
-here: the kernel each shape gets (single CTA wide / narrow, CTA pair, grouped), grid and shared memory, both UINT8 tensor maps
-(A rows x K and B^T (P N) rows x K, boxes of 128 bytes), the byte-transposing pre-pass and its P K N bytes of scratch without
-COAST_MM_B_TRANSPOSED and neither with it, every refusal with its message, that a batch of one is the unbatched launch, the bytes
-the host call copies per chunk (1-byte A and B, 4-byte C), that every xmr_gemm_fp8 function of the cubin is reached, that each
-runs the E4M3 wgmma, and that none keeps more stack than its TF32 or BF16 twin."""
-import json
+"""Host logic of COAST_K_GEMM_FP8 on a GPU-less box, against the mock driver (tests/mock_cuda/mock_cuda.c) through
+tests/mock_cuda/mm_child.py, whose A and B buffers hold 1-byte elements.  Pinned here: the kernel each shape gets (single CTA
+wide / narrow, CTA pair, grouped), grid and shared memory, both UINT8 tensor maps (A rows x K and B^T (P N) rows x K, boxes of
+128 bytes), the byte-transposing pre-pass and its P K N bytes of scratch without COAST_MM_B_TRANSPOSED and neither with it,
+every refusal with its message, that a batch of one is the unbatched launch, the bytes the host call copies per chunk (1-byte A
+and B, 4-byte C), that every xmr_gemm_fp8 function of the cubin runs the E4M3 wgmma, and that none keeps more stack than its
+TF32 or BF16 twin.  tests/test_mm_plan_sweep.py shows that each is reached."""
 import os
 import re
 import subprocess
-import sys
 
 import pytest
 
-from test_host_logic import ROOT, args_of
+from mock_run import (BAD_ARG, GRP_BYTES, K_CRC16, K_GEMM_FP8, MM_B_TRANSPOSED as MM_BT, MM_BATCHED, MM_GROUPED, ROOT, SMS,  # noqa: F401
+                      UNSUPPORTED, arg0_ptr, args_of, maps, mock_dir, run, spans, work)
 
-MM_BATCHED, MM_GROUPED, MM_BT = 0x20000, 0x40000, 0x80000
-K_CRC16, K_GEMM_FP8 = 0, 10
-BAD_ARG, UNSUPPORTED = -100003, -100004
-SMS = 132
 SMEM = 6 * (128 * 128 + 128 * 128) + 1024 + 256          # xmr_gemm_smem: the same bytes wide and narrow
-GRP_BYTES = lambda G: 128 + 4 * (G + 1)                  # noqa: E731  (xmr_mm_grp_bytes)
 CUBIN = os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")
-KNOBS = ("COAST_GEMM_PAIR", "COAST_GEMM_GROUP_M", "COAST_GEMM_L2_HINTS", "COAST_GEMM_TAIL_SPLIT", "COAST_HOST_CHUNK_BYTES",
-         "COAST_HOST_PATH", "COAST_STRICT_FLAGS")
-
-
-@pytest.fixture(scope="session")
-def mock_dir(tmp_path_factory, built_lib):
-    d = tmp_path_factory.mktemp("mockcuda_fp8")
-    subprocess.run(["gcc", "-O1", "-shared", "-fPIC", "-Wall", "-I/usr/local/cuda/include", "-o", str(d / "libcuda.so.1"),
-                    os.path.join(ROOT, "tests", "mock_cuda", "mock_cuda_bt.c")], check=True)
-    return d
-
-
-def run(mock_dir, tmp_path, ops, env_extra=None):
-    log = tmp_path / "mock.log"
-    if log.exists():
-        log.unlink()
-    env = dict(os.environ, LD_LIBRARY_PATH=f"{mock_dir}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=str(log))
-    for k in KNOBS:
-        env.pop(k, None)
-    env.update(env_extra or {})
-    ops = [dict({"kernel": K_GEMM_FP8}, **op) for op in ops]
-    res = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mock_cuda", "mm_bt_child.py"), json.dumps({"ops": ops})],
-                         capture_output=True, text=True, env=env, timeout=600)
-    assert res.returncode == 0, res.stdout + res.stderr
-    events = [json.loads(ln) for ln in open(log)] if log.exists() else []
-    assert not [e for e in events if e["op"] == "error"], [e for e in events if e["op"] == "error"]
-    assert events[-1] == {"op": "exit", "live_allocations": 0}
-    return json.loads(res.stdout.strip().splitlines()[-1]), events, res.stderr
-
-
-def work(ev):
-    return [e for e in ev if e["op"] == "launch" and e["name"] != "xmr_counters_reset"]
-
-
-def tmaps(ev):
-    """(start address, element bytes, dim0, dim1, box0, box1) of every map"""
-    at = [e["addr"] for e in ev if e["op"] == "tmap_at"]
-    return [(a, t["elem"], t["dim0"], t["dim1"], t["box0"], t["box1"]) for a, t in zip(at, [e for e in ev if e["op"] == "tmap"])]
 
 
 # (id, nc, M, N, K, batch or None, environment, kernel, grid)
@@ -81,7 +37,7 @@ LAUNCHES = [
 @pytest.mark.parametrize("case", LAUNCHES, ids=[c[0] for c in LAUNCHES])
 def test_launch_records(mock_dir, tmp_path, case, bt):
     _, nc, M, N, K, batch, env, name, grid = case
-    op = dict(op="launch", nc=nc, M=M, N=N, K=K, unit_base=1 << 32, flags=3, bt=bt)
+    op = dict(op="launch", kernel=K_GEMM_FP8, nc=nc, M=M, N=N, K=K, unit_base=1 << 32, flags=3, bt=bt)
     if batch:
         op["batch"] = batch
     b = batch or 1
@@ -102,11 +58,11 @@ def test_launch_records(mock_dir, tmp_path, case, bt):
         b_at = r["aux"]
     else:                                                          # B^T of every product into P K N bytes of scratch first
         assert [e["name"] for e in la] == ["xmr_gemm_bt_u8", name] and [e["bytes"] for e in scratch] == [b * K * N]
-        assert int.from_bytes(bytes.fromhex(la[0]["arg0"]), "little") == r["aux"] and la[0]["stream"] == k["stream"]
+        assert arg0_ptr(la[0]) == r["aux"] and la[0]["stream"] == k["stream"]
         b_at = scratch[0]["ptr"]
         assert {"op": "free", "id": scratch[0]["id"]} in ev[ev.index(k):]
     # A: (batch M) rows of K bytes, boxes of one 128-byte k-block x 128 rows; B^T: (batch N) rows of K, 128 bytes x 128 (pairs: 64)
-    assert tmaps(ev) == [(r["in"], 1, K, b * M, 128, 128), (b_at, 1, K, b * N, 128, 64 if "fp8p" in name else 128)]
+    assert maps(ev) == [(r["in"], 1, K, b * M, 128, 128), (b_at, 1, K, b * N, 128, 64 if "fp8p" in name else 128)]
 
 
 RO = [3, 3, 100, 101, 101, 500, 700]
@@ -116,7 +72,7 @@ R, G = RO[-1] - RO[0], len(RO) - 1
 @pytest.mark.parametrize("bt", [False, True], ids=["B", "Bt"])
 @pytest.mark.parametrize("nc,N,K", [(3, 128, 128), (2, 256, 256), (1, 256, 128)])
 def test_grouped_launch(mock_dir, tmp_path, nc, N, K, bt):
-    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", nc=nc, N=N, K=K, ro=RO, unit_base=1 << 32, flags=3, bt=bt)],
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_FP8, nc=nc, N=N, K=K, ro=RO, unit_base=1 << 32, flags=3, bt=bt)],
                      env_extra={"COAST_GEMM_PAIR": "1"})
     r = res["ops"][0]
     assert r["rc"] == 0, r["err"]
@@ -133,10 +89,10 @@ def test_grouped_launch(mock_dir, tmp_path, nc, N, K, bt):
     assert [e["bytes"] for e in allocs[-1:]] == [(0 if bt else G * K * N) + GRP_BYTES(G)]
     base = r["aux"] if bt else allocs[-1]["ptr"]
     # A is a 128-row placeholder over B^T that the scan rebases; B^T is the G stacked N x K matrices
-    assert tmaps(ev) == [(base, 1, K, 128, 128, 128), (base, 1, K, G * N, 128, 128)]
+    assert maps(ev) == [(base, 1, K, 128, 128, 128), (base, 1, K, G * N, 128, 128)]
 
 
-OK = dict(M=128, N=128, K=128)
+OK = dict(kernel=K_GEMM_FP8, M=128, N=128, K=128)
 REFUSALS = [
     ("k_64", dict(OK, K=64), UNSUPPORTED, "GEMM_FP8 tiles are 128x128x128: M,N must be multiples of 128 and K of 128"),
     ("n_64", dict(OK, N=64), UNSUPPORTED, "multiples of 128"),
@@ -166,14 +122,14 @@ REFUSALS = [
 @pytest.mark.parametrize("case", REFUSALS, ids=[c[0] for c in REFUSALS])
 def test_refusals_name_their_rule_and_launch_nothing(mock_dir, tmp_path, case):
     _, op, code, needle = case
-    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", **op)])
+    res, ev, _ = run(mock_dir, tmp_path, [{"op": "launch", "kernel": K_GEMM_FP8, **op}])
     r = res["ops"][0]
     assert r["rc"] == code and needle in r["err"], r
     assert not work(ev)
 
 
 def test_unassigned_id_9_is_refused_by_the_host_call(mock_dir, tmp_path):
-    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=9, **OK)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(OK, op="run_host", kernel=9)])
     assert res["ops"][0]["rc"] == UNSUPPORTED and not work(ev)
 
 
@@ -190,23 +146,19 @@ def test_store_vote_flags_warn_or_refuse(mock_dir, tmp_path):
 def test_a_batch_of_one_is_the_unbatched_launch(mock_dir, tmp_path, nc, M, N, env, bt):
     recs = []
     for extra in (dict(batch=1), {}):
-        res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", nc=nc, M=M, N=N, K=256, unit_base=77, flags=3, bt=bt, **extra)], env_extra=env)
+        res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_FP8, nc=nc, M=M, N=N, K=256, unit_base=77, flags=3, bt=bt, **extra)], env_extra=env)
         assert res["ops"][0]["rc"] == 0
         la = work(ev)
         a = args_of(la[-1])
-        recs.append(([(e["name"], e["grid"], e["block"], e["smem"]) for e in la], [t[1:] for t in tmaps(ev)],
+        recs.append(([(e["name"], e["grid"], e["block"], e["smem"]) for e in la], [m[1:] for m in maps(ev)],
                      (a.n_units, a.unit_base, a.M, a.N, a.K, a.mode, a.flags, a.n_sites), [e["bytes"] for e in ev if e["op"] == "alloc"]))
     assert recs[0] == recs[1]
-
-
-def spans(ev, op, base, size):
-    return [(e["host"] - base, e["bytes"], e["stream"]) for e in ev if e["op"] == op and base <= e["host"] < base + size]
 
 
 @pytest.mark.parametrize("pinned", [False, True])
 def test_host_call_row_blocks_copy_one_byte_operands(mock_dir, tmp_path, pinned):
     M, N, K = 1024, 128, 128
-    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", nc=3, M=M, N=N, K=K, pinned=pinned, unit_base=5)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_GEMM_FP8, nc=3, M=M, N=N, K=K, pinned=pinned, unit_base=5)])
     r = res["ops"][0]
     assert r["rc"] == 0 and r["path"] == "row-blocks", r
     ups_a, ups_b = spans(ev, "h2d", r["host_in"], M * K), spans(ev, "h2d", r["host_aux"], K * N)
@@ -224,7 +176,7 @@ def test_host_call_row_blocks_copy_one_byte_operands(mock_dir, tmp_path, pinned)
 def test_host_call_whole_products_per_chunk(mock_dir, tmp_path, pinned, bt):
     M, N, K, batch = 128, 128, 256, 5
     ab, bb, cb = M * K, K * N, M * N * 4
-    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", nc=2, M=M, N=N, K=K, batch=batch, pinned=pinned, bt=bt)],
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_GEMM_FP8, nc=2, M=M, N=N, K=K, batch=batch, pinned=pinned, bt=bt)],
                      env_extra={"COAST_HOST_CHUNK_BYTES": str(2 * (ab + bb + cb) + 100)})
     r = res["ops"][0]
     assert r["rc"] == 0, r
@@ -240,7 +192,7 @@ def test_host_call_whole_products_per_chunk(mock_dir, tmp_path, pinned, bt):
 @pytest.mark.parametrize("pinned", [False, True])
 def test_host_call_groups_per_chunk(mock_dir, tmp_path, pinned):
     N, K, ro, budget = 128, 128, [7, 100, 228, 228, 500, 501], 90000
-    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", nc=3, N=N, K=K, ro=ro, unit_base=1000, pinned=pinned)],
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_GEMM_FP8, nc=3, N=N, K=K, ro=ro, unit_base=1000, pinned=pinned)],
                      env_extra={"COAST_HOST_CHUNK_BYTES": str(budget)})
     r = res["ops"][0]
     assert r["rc"] == 0 and r["path"] == "groups", r
@@ -265,32 +217,6 @@ def test_host_call_groups_per_chunk(mock_dir, tmp_path, pinned):
 
 
 # ------------------------------------------------------------------------------------------ the cubin's FP8 functions
-def fp8_functions():
-    elf = subprocess.run(["cuobjdump", "-elf", CUBIN], capture_output=True, text=True).stdout
-    return {f for f in re.findall(r"\.text\.(xmr_\w+)", elf) if f.startswith("xmr_gemm_fp8")}
-
-
-def test_every_fp8_function_is_reached_and_no_name_is_missing(mock_dir, tmp_path):
-    """one product, a batch and groups, B and B^T, NC 1-3, with and without a fault plan, on shapes that reach every path and
-    under each pair setting: the names launched are exactly the cubin's 20 xmr_gemm_fp8 functions (a missing name is a mock
-    error, which run() refuses)"""
-    ops = []
-    for bt in (False, True):
-        for nc in (1, 2, 3):
-            for p in (0, 0.3):
-                base = dict(op="launch", nc=nc, bt=bt, p=p, unit_base=(1 << 32) - 5)
-                for M, N, K in ((512, 512, 128), (384, 512, 128), (512, 384, 128), (384, 384, 256)):
-                    ops += [dict(base, M=M, N=N, K=K), dict(base, M=M, N=N, K=K, batch=2)]
-                ops += [dict(base, N=N, K=K, ro=RO) for N, K in ((256, 128), (128, 256))]
-    launched = set()
-    for env in ({}, {"COAST_GEMM_PAIR": "0"}, {"COAST_GEMM_PAIR": "1"}):
-        res, ev, _ = run(mock_dir, tmp_path, ops, env_extra=env)
-        assert [r["err"] for r in res["ops"] if r["rc"]] == []
-        launched |= {e["name"] for e in ev if e["op"] == "launch" and e["name"].startswith("xmr_gemm_fp8")}
-    have = fp8_functions()
-    assert len(have) == 20 and launched == have, (sorted(have - launched), sorted(launched - have))
-
-
 def sass_by_function():
     sass = subprocess.run(["cuobjdump", "-sass", CUBIN], capture_output=True, text=True).stdout
     parts = re.split(r"\n\s*Function : (\S+)\n", sass)

@@ -10,15 +10,13 @@ operands (exact in fp32 whatever the order of the additions) against a float64 b
 every persistent CTA run at least 3 tiles, with tiles of different products in one wave."""
 import pytest
 
+from mm_gpu import POISON, env as _env
 from test_gpu_stream_exact import GiB, _free, _room
 
 pytestmark = pytest.mark.gpu
 
-POISON = 0x5A5A5A5A
 M32 = 0xFFFFFFFF
 SMS = 132
-GEMM_KNOBS = ("COAST_GEMM_PAIR", "COAST_GEMM_GROUP_M", "COAST_GEMM_L2_HINTS", "COAST_GEMM_TAIL_SPLIT", "COAST_MM_PATH",
-              "COAST_HOST_CHUNK_BYTES", "COAST_HOST_PATH")
 
 
 # ------------------------------------------------------------------------------------------ references (on the device)
@@ -140,13 +138,6 @@ PATHS = [
     ("tf32_narrow", 4, 128, 128, 32, 400, None, "xmr_gemm_tf32n_nc{nc}"),
 ]
 PLANS = ["none", "bernoulli", "table", "majority"]
-
-
-def _env(monkeypatch, **env):
-    for k in GEMM_KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
 
 
 def _expected_name(path, nc):

@@ -10,21 +10,12 @@ zero-padded to 128 rows.  Row tables start past row 0 (the TF32 A map is rebased
 products and one large product, and the output buffers start poisoned: rows outside [ro[0], ro[G]) must keep the poison."""
 import pytest
 
+from mm_gpu import POISON, env as _env
 from test_gpu_stream_exact import GiB, _free, _room
 
 pytestmark = pytest.mark.gpu
 
-POISON = 0x5A5A5A5A
 M32 = 0xFFFFFFFF
-KNOBS = ("COAST_GEMM_PAIR", "COAST_GEMM_GROUP_M", "COAST_GEMM_L2_HINTS", "COAST_GEMM_TAIL_SPLIT", "COAST_MM_PATH",
-         "COAST_HOST_CHUNK_BYTES", "COAST_HOST_PATH")
-
-
-def _env(monkeypatch, **env):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
 
 
 def row_table(G, total, seed, first=5):

@@ -8,22 +8,13 @@ whose entries encode their own position shows a mis-strided or mis-swizzled K-ma
 import numpy as np
 import pytest
 
+from mm_gpu import POISON, add_stats, env
+
 pytestmark = pytest.mark.gpu
 
-KNOBS = ("COAST_GEMM_PAIR", "COAST_GEMM_GROUP_M", "COAST_GEMM_L2_HINTS", "COAST_GEMM_TAIL_SPLIT", "COAST_HOST_CHUNK_BYTES",
-         "COAST_HOST_PATH", "COAST_MM_PATH")
 MM_BATCHED, MM_GROUPED, BT = 0x20000, 0x40000, 0x80000
 K_MM_U32, K_GEMM_TF32, K_GEMM_BF16 = 3, 4, 8
-STAT_KEYS = ("errors_corrected", "dwc_detected", "syncs", "injected", "first_fault_unit")
-POISON = 0x7FC00BAD
 RO = [3, 3, 100, 101, 101, 500, 700, 828]          # from row 3: empty products, a one-row product, a 128-row product
-
-
-def env(monkeypatch, **kv):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in kv.items():
-        monkeypatch.setenv(k, v)
 
 
 def operands(kernel, rows, batch, N, K, seed, integer=True, amax=8):
@@ -275,11 +266,6 @@ def test_shards_sum_to_the_whole_launch(rt, monkeypatch, kernel):
     plan = cb.FaultPlan(mode=cb.PLAN_BERNOULLI, seed=2, p=0.1)
     ro = torch.tensor(RO, dtype=torch.int64, device="cuda")
     dt = torch.int32 if kernel == K_MM_U32 else torch.float32
-
-    def fold(tot, s):
-        for k in STAT_KEYS[:4]:
-            tot[k] += s[k]
-        tot["first_fault_unit"] = min(tot["first_fault_unit"], s["first_fault_unit"])
     whole, sw = rt.run(kernel, 3, A, R * N, M=G, N=N, K=K, aux=Bt, flags=3, mode=MM_GROUPED | BT, rows=ro, plan=plan, unit_base=50,
                        out=torch.zeros(RO[-1] * N, dtype=dt, device="cuda"))
     out = torch.zeros(RO[-1] * N, dtype=dt, device="cuda")
@@ -290,7 +276,7 @@ def test_shards_sum_to_the_whole_launch(rt, monkeypatch, kernel):
             continue
         _, s = rt.run(kernel, 3, A, (RO[hi] - RO[lo]) * N, M=hi - lo, N=N, K=K, aux=Bt[lo:], flags=3, mode=MM_GROUPED | BT,
                       rows=ro[lo:], plan=plan, unit_base=50 + (RO[lo] - RO[0]) * N, out=out)
-        fold(tot, s.as_dict())
+        add_stats(tot, s.as_dict())
     assert torch.equal(out, whole) and tot == sw.as_dict()
     # batched: whole matrices per shard
     M, batch = 128, 5
@@ -301,7 +287,7 @@ def test_shards_sum_to_the_whole_launch(rt, monkeypatch, kernel):
         o, s = rt.run(kernel, 2, A[lo * M:hi * M], (hi - lo) * M * N, M=M, N=N, K=K, aux=Bt[lo:hi], flags=3, mode=MM_BATCHED | BT,
                       plan=plan, unit_base=7 + lo * M * N)
         parts.append(o)
-        fold(tot, s.as_dict())
+        add_stats(tot, s.as_dict())
     assert torch.equal(torch.cat(parts), whole) and tot == sw.as_dict()
 
 

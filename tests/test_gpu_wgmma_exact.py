@@ -13,10 +13,8 @@ Every exact check here compares every element of the output."""
 import numpy as np
 import pytest
 
-from test_gpu_parity import STAT_KEYS, both, dev, host
-
-POISON = 0x5A5A5A5A                      # initial content of every matmul output buffer: a run that skips an element fails
-GEMM_KNOBS = ("COAST_GEMM_PAIR", "COAST_GEMM_GROUP_M", "COAST_GEMM_L2_HINTS", "COAST_GEMM_TAIL_SPLIT")
+from mm_gpu import POISON, STAT_KEYS, env as _gemm_env
+from test_gpu_parity import both, dev, host
 
 
 # ------------------------------------------------------------------------------------------ references (CPU)
@@ -120,13 +118,6 @@ GEMM_VARIANTS = [
     ("single_nc3", None, 3, 256, 128, "xmr_gemm_tf32_nc3"),
     ("pair_nc3", "1", 3, 256, 256, "xmr_gemm_tf32p_nc3"),
 ]
-
-
-def _gemm_env(monkeypatch, **env):
-    for k in GEMM_KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
 
 
 @pytest.mark.gpu

@@ -12,21 +12,11 @@ Chunk i runs on host stream i % 3.  The staging memory a call keeps may be small
 import numpy as np
 import pytest
 
-from test_host_logic import args_of, mock_dir, run_child  # noqa: F401  (mock_dir is a fixture)
-from test_ragged_host_logic import run as run_ragged
-from test_ragged_qsort_host_logic import run as run_qsort
-from test_batched_mm_host_logic import run as run_batched
+from mock_run import K_AES128, K_GEMM_TF32, K_MM_U32, K_SHA256, args_of, mock_dir, run  # noqa: F401  (mock_dir is a fixture)
 
-K_CRC16, K_SHA256, K_AES128, K_MM_U32, K_GEMM_TF32, K_QSORT = range(6)
-KEY_PER_UNIT, KEY_WRITEBACK, UNIT_OFFSETS, MM_BATCHED = 2, 4, 0x10000, 0x20000
+KEY_PER_UNIT, KEY_WRITEBACK = 2, 4
 HS = (0x1001, 0x1002, 0x1003)          # the mock numbers streams 0x1000 + k in creation order: the host call's three come first
 MIB = 1 << 20
-
-
-@pytest.fixture(autouse=True)
-def default_host_call(monkeypatch):
-    for k in ("COAST_HOST_CHUNK_BYTES", "COAST_HOST_PATH", "COAST_MM_PATH", "COAST_GEMM_PAIR"):
-        monkeypatch.delenv(k, raising=False)
 
 
 def trace(ev, bufs, in_place=False):
@@ -100,8 +90,8 @@ def uniform_expect(n, ib, ob, unit_base=0, ab=0, writeback=False, status=False, 
 def test_sha256_ramps_up_and_down(mock_dir, tmp_path, chunk_bytes):
     n = MIB + 123
     env = {"COAST_HOST_CHUNK_BYTES": str(chunk_bytes)} if chunk_bytes else None
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host", kernel=K_SHA256, nc=3, n=n, unit_bytes=64, in_bytes=64 * n,
-                                                  out_bytes=32 * n, unit_base=1000), dict(op="shutdown")], env_extra=env)
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_SHA256, nc=3, n=n, unit_bytes=64, in_bytes=64 * n,
+                                               out_bytes=32 * n, unit_base=1000), dict(op="shutdown")], "child.py", env_extra=env)
     r = res["ops"][0]
     assert r["rc"] == 0, r
     ops, slots = uniform_expect(n, 64, 32, unit_base=1000, chunk_bytes=chunk_bytes or 16 * MIB)
@@ -114,8 +104,8 @@ def test_sha256_ramps_up_and_down(mock_dir, tmp_path, chunk_bytes):
 
 def test_aes_per_unit_keys_with_write_back(mock_dir, tmp_path):
     n = 200000
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=K_AES128, nc=2, n=n, mode=KEY_PER_UNIT | KEY_WRITEBACK,
-                                                  in_bytes=16 * n, aux_bytes=16 * n, out_bytes=16 * n, unit_base=7), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=K_AES128, nc=2, n=n, mode=KEY_PER_UNIT | KEY_WRITEBACK,
+                                               in_bytes=16 * n, aux_bytes=16 * n, out_bytes=16 * n, unit_base=7), dict(op="shutdown")], "child.py")
     r = res["ops"][0]
     assert r["rc"] == 0, r
     ops, slots = uniform_expect(n, 16, 16, unit_base=7, ab=16, writeback=True)
@@ -125,8 +115,8 @@ def test_aes_per_unit_keys_with_write_back(mock_dir, tmp_path):
 
 def test_aes_status_bytes(mock_dir, tmp_path):
     n = 300001
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_status", kernel=K_AES128, nc=2, n=n, in_bytes=16 * n, out_bytes=16 * n),
-                                             dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_status", kernel=K_AES128, nc=2, n=n, in_bytes=16 * n, out_bytes=16 * n),
+                                          dict(op="shutdown")], "child.py")
     r = res["ops"][0]
     assert r["rc"] == 0, r
     ops, slots = uniform_expect(n, 16, 16, status=True)
@@ -136,9 +126,9 @@ def test_aes_status_bytes(mock_dir, tmp_path):
 
 def test_hybrid_sha256_reads_the_pinned_input_in_place(mock_dir, tmp_path):
     n = 300000
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_pinned", kernel=K_SHA256, nc=3, n=n, unit_bytes=64, in_bytes=64 * n,
-                                                  out_bytes=32 * n, unit_base=77, status=True), dict(op="shutdown")],
-                        env_extra={"COAST_HOST_PATH": "hybrid"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_pinned", kernel=K_SHA256, nc=3, n=n, unit_bytes=64, in_bytes=64 * n,
+                                               out_bytes=32 * n, unit_base=77, status=True), dict(op="shutdown")], "child.py",
+                     env_extra={"COAST_HOST_PATH": "hybrid"})
     r = res["ops"][0]
     assert r["rc"] == 0, r
     ops, slots = uniform_expect(n, 64, 32, unit_base=77, status=True, hybrid=True)
@@ -149,8 +139,8 @@ def test_hybrid_sha256_reads_the_pinned_input_in_place(mock_dir, tmp_path):
 
 def test_empty_sha256_input(mock_dir, tmp_path):
     n = 3
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host", kernel=K_SHA256, nc=3, n=n, unit_bytes=0, in_bytes=0, out_bytes=32 * n,
-                                                  unit_base=9), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_SHA256, nc=3, n=n, unit_bytes=0, in_bytes=0, out_bytes=32 * n,
+                                               unit_base=9), dict(op="shutdown")], "child.py")
     r = res["ops"][0]
     assert r["rc"] == 0, r
     ops, slots = uniform_expect(n, 0, 32, unit_base=9)
@@ -188,8 +178,8 @@ def test_ragged_sha256(mock_dir, tmp_path):
     lens[::37] = 0
     lens[100] = 50000                                        # longer than the chunk bytes: a chunk of its own
     off = [int(x) for x in 5 + np.concatenate([[0], np.cumsum(lens)])]
-    res, ev = run_ragged(mock_dir, tmp_path, [dict(op="run_host", kernel=K_SHA256, offsets=off, unit_bytes=50000, unit_base=1000)],
-                         env_extra={"COAST_HOST_CHUNK_BYTES": "20000"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_SHA256, offsets=off, unit_bytes=50000, unit_base=1000)], "ragged_child.py",
+                      env_extra={"COAST_HOST_CHUNK_BYTES": "20000"})
     r = res["ops"][0]
     assert r["rc"] == 0 and r["path"] == "staged", r
     ops, slots = ragged_expect(off, 32, False, 1000, 20000)
@@ -204,8 +194,8 @@ def test_ragged_quicksort(mock_dir, tmp_path):
     elems = rng.integers(0, 1025, 200)
     elems[::17] = 0
     off = [int(x) for x in 12 + 4 * np.concatenate([[0], np.cumsum(elems)])]
-    res, ev = run_qsort(mock_dir, tmp_path, [dict(op="run_host", offsets=off, unit_bytes=4096, unit_base=3)],
-                        env_extra={"COAST_HOST_CHUNK_BYTES": "30000"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", offsets=off, unit_bytes=4096, unit_base=3)], "ragged_qsort_child.py",
+                     env_extra={"COAST_HOST_CHUNK_BYTES": "30000"})
     r = res["ops"][0]
     assert r["rc"] == 0 and r["path"] == "staged", r
     ops, slots = ragged_expect(off, 0, True, 3, 30000)
@@ -218,8 +208,8 @@ def test_ragged_quicksort(mock_dir, tmp_path):
 # ---------------------------------------------------------------- matmuls
 @pytest.mark.parametrize("kernel,M,N,K,blocks", [(K_GEMM_TF32, 1024, 256, 128, 8), (K_MM_U32, 128, 128, 128, 1)])
 def test_matmul_row_blocks_share_one_upload_of_b(mock_dir, tmp_path, kernel, M, N, K, blocks):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=kernel, nc=3, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4,
-                                                  aux_bytes=K * N * 4, out_bytes=M * N * 4, unit_base=5), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=kernel, nc=3, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4,
+                                               aux_bytes=K * N * 4, out_bytes=M * N * 4, unit_base=5), dict(op="shutdown")], "child.py")
     r = res["ops"][0]
     assert r["rc"] == 0, r
     rows = M // blocks
@@ -240,8 +230,8 @@ def test_matmul_row_blocks_share_one_upload_of_b(mock_dir, tmp_path, kernel, M, 
     (K_GEMM_TF32, 128, 128, 32, 9, 200000, 2),
 ])
 def test_batched_chunks_of_whole_products(mock_dir, tmp_path, kernel, M, N, K, batch, budget, per):
-    res, ev = run_batched(mock_dir, tmp_path, [dict(op="run_host", kernel=kernel, nc=3, M=M, N=N, K=K, batch=batch, unit_base=1000)],
-                          env_extra={"COAST_HOST_CHUNK_BYTES": str(budget)})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=kernel, nc=3, M=M, N=N, K=K, batch=batch, unit_base=1000)],
+                       env_extra={"COAST_HOST_CHUNK_BYTES": str(budget)})
     r = res["ops"][0]
     assert r["rc"] == 0 and r["path"] == "staged", r
     ab, bb, cb, mn = 4 * M * K, 4 * K * N, 4 * M * N, M * N

@@ -12,51 +12,13 @@ import sys
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-K_CRC16, K_SHA256, K_AES128, K_MM_U32, K_GEMM_TF32, K_QSORT, K_CHSTONE_SHA = range(7)
-
-
-class XmrArgs(C.Structure):                     # coast_b200/csrc/xmr_args.h
-    _fields_ = [("inp", C.c_uint64), ("out", C.c_uint64), ("aux", C.c_uint64), ("n_units", C.c_uint64), ("unit_base", C.c_uint64),
-                ("counters", C.c_uint64), ("plan_table", C.c_uint64), ("status", C.c_uint64),
-                ("unit_bytes", C.c_uint32), ("flags", C.c_uint32), ("mode", C.c_uint32), ("M", C.c_uint32), ("N", C.c_uint32),
-                ("K", C.c_uint32), ("plan_mode", C.c_uint32), ("seed_lo", C.c_uint32), ("seed_hi", C.c_uint32),
-                ("threshold", C.c_uint32), ("n_sites", C.c_uint32), ("n_tiles", C.c_uint32), ("key", C.c_uint8 * 16)]
-
-
-@pytest.fixture(scope="session")
-def mock_dir(tmp_path_factory, built_lib):
-    d = tmp_path_factory.mktemp("mockcuda")
-    subprocess.run(["gcc", "-O1", "-shared", "-fPIC", "-Wall", "-I/usr/local/cuda/include", "-o", str(d / "libcuda.so.1"),
-                    os.path.join(ROOT, "tests", "mock_cuda", "mock_cuda.c")], check=True)
-    return d
-
-
-def run_child(mock_dir, tmp_path, ops, env_extra=None):
-    log = tmp_path / "mock.log"
-    if log.exists():
-        log.unlink()                                        # one log per child run
-    env = dict(os.environ, LD_LIBRARY_PATH=f"{mock_dir}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=str(log))
-    env.update(env_extra or {})
-    res = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mock_cuda", "child.py"), json.dumps({"ops": ops})],
-                         capture_output=True, text=True, env=env, timeout=300)
-    assert res.returncode == 0, res.stdout + res.stderr
-    events = [json.loads(ln) for ln in open(log)] if log.exists() else []
-    return json.loads(res.stdout.strip().splitlines()[-1]), events
-
-
-def args_of(ev):
-    assert sizeof_args() == 128
-    return XmrArgs.from_buffer_copy(bytes.fromhex(ev["arg0"]))
-
-
-def sizeof_args():
-    return C.sizeof(XmrArgs)
+from mock_run import (ROOT, XmrArgs, K_AES128, K_CHSTONE_SHA, K_CRC16, K_GEMM_TF32, K_MM_U32, K_QSORT, K_SHA256, args_of,  # noqa: F401
+                      mock_dir, run)
 
 
 def test_argument_block_mirror_matches_the_header():
     src = open(os.path.join(ROOT, "coast_b200", "csrc", "xmr_args.h")).read()
-    assert sizeof_args() == 128 and "unsigned char key[16];" in src and src.index("n_tiles") < src.index("key[16]")
+    assert C.sizeof(XmrArgs) == 128 and "unsigned char key[16];" in src and src.index("n_tiles") < src.index("key[16]")
 
 
 @pytest.mark.parametrize("kernel,nc,n,ub,in_b,out_b,want", [
@@ -71,8 +33,8 @@ def test_argument_block_mirror_matches_the_header():
     (K_CHSTONE_SHA, 3, 300, 16384, 300 * 16384, 300 * 20, ("xmr_chsha_nc3_inj0", 256, None)),
 ])
 def test_launch_geometry_and_argument_block(mock_dir, tmp_path, kernel, nc, n, ub, in_b, out_b, want):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=nc, n=n, unit_bytes=ub, in_bytes=in_b, out_bytes=out_b,
-                                                  flags=3), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=nc, n=n, unit_bytes=ub, in_bytes=in_b, out_bytes=out_b,
+                                               flags=3), dict(op="shutdown")], "child.py")
     assert res["init"] == 0 and res["ops"][0]["rc"] == 0, res
     assert not [e for e in ev if e["op"] == "error"], ev
     launches = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
@@ -96,7 +58,7 @@ def test_launch_geometry_and_argument_block(mock_dir, tmp_path, kernel, nc, n, u
 
 
 def test_injector_variant_and_plan_fields(mock_dir, tmp_path):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_AES128, nc=2, n=4096, in_bytes=65536, out_bytes=65536, p=2 ** -10)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_AES128, nc=2, n=4096, in_bytes=65536, out_bytes=65536, p=2 ** -10)], "child.py")
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]][0]
     a = args_of(la)
     assert la["name"] == "xmr_aes128_enc_nc2_inj1" and a.plan_mode == 1 and a.threshold == 1 << 22 and a.n_sites == 176
@@ -105,8 +67,8 @@ def test_injector_variant_and_plan_fields(mock_dir, tmp_path):
 @pytest.mark.parametrize("kernel,ub,ob,n", [(K_SHA256, 64, 32, 1), (K_SHA256, 64, 32, 1000), (K_SHA256, 64, 32, (1 << 20) + 123),
                                             (K_CRC16, 13, 2, 7), (K_AES128, 16, 16, 300001), (K_CHSTONE_SHA, 16384, 20, 3)])
 def test_run_host_chunk_schedule_copies_every_byte_once(mock_dir, tmp_path, kernel, ub, ob, n):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host", kernel=kernel, nc=3 if kernel != K_AES128 else 2, n=n, unit_bytes=ub if kernel != K_AES128 else 0,
-                                                  in_bytes=n * ub, out_bytes=n * ob, unit_base=1000), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=kernel, nc=3 if kernel != K_AES128 else 2, n=n, unit_bytes=ub if kernel != K_AES128 else 0,
+                                               in_bytes=n * ub, out_bytes=n * ob, unit_base=1000), dict(op="shutdown")], "child.py")
     r = res["ops"][0]
     assert r["rc"] == 0, r
     assert not [e for e in ev if e["op"] == "error"], [e for e in ev if e["op"] == "error"]
@@ -138,21 +100,21 @@ def test_run_host_chunk_schedule_copies_every_byte_once(mock_dir, tmp_path, kern
     (dict(op="launch", kernel=K_AES128, nc=2, n=4, in_bytes=80, out_bytes=64, misalign=4), "16-byte aligned"),
 ])
 def test_bad_arguments_fail_loudly(mock_dir, tmp_path, op, needle):
-    res, ev = run_child(mock_dir, tmp_path, [op])
+    res, ev, _ = run(mock_dir, tmp_path, [op], "child.py")
     r = res["ops"][0]
     assert r["rc"] != 0 and needle in r["err"], r
     assert not [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
 
 
 def test_unaligned_sha_input_takes_the_general_kernel(mock_dir, tmp_path):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_SHA256, nc=3, n=100, unit_bytes=64, in_bytes=6500, out_bytes=3200, misalign=4)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_SHA256, nc=3, n=100, unit_bytes=64, in_bytes=6500, out_bytes=3200, misalign=4)], "child.py")
     assert res["ops"][0]["rc"] == 0
     assert [e["name"] for e in ev if e["op"] == "launch" and "_nc" in e["name"]] == ["xmr_sha256_gen_nc3_inj0"]
     assert not [e for e in ev if e["op"] == "tmap"]
 
 
 def test_a_device_that_is_not_sm90_is_refused(mock_dir, tmp_path):
-    res, ev = run_child(mock_dir, tmp_path, [], env_extra={"MOCK_CUDA_CC_MAJOR": "10"})
+    res, ev, _ = run(mock_dir, tmp_path, [], "child.py", env_extra={"MOCK_CUDA_CC_MAJOR": "10"})
     assert res["init"] != 0 and "sm_90a code only" in res["error"]
 
 
@@ -164,8 +126,8 @@ def test_a_device_that_is_not_sm90_is_refused(mock_dir, tmp_path):
     (9, 9, 9, 3, {}, ["xmr_mm_u32_nc3_inj0"]),                                                        # the reference's own size
 ])
 def test_exact_matmul_path_selection_and_tensor_maps(mock_dir, tmp_path, M, N, K, nc, env, want):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_MM_U32, nc=nc, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4,
-                                                  aux_bytes=K * N * 4, out_bytes=M * N * 4, flags=3), dict(op="shutdown")], env_extra=env)
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_MM_U32, nc=nc, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4,
+                                               aux_bytes=K * N * 4, out_bytes=M * N * 4, flags=3), dict(op="shutdown")], "child.py", env_extra=env)
     assert res["ops"][0]["rc"] == 0, res
     assert not [e for e in ev if e["op"] == "error"], [e for e in ev if e["op"] == "error"]
     names = [e["name"] for e in ev if e["op"] == "launch" and e["name"] not in ("xmr_counters_reset",)]
@@ -180,16 +142,16 @@ def test_exact_matmul_path_selection_and_tensor_maps(mock_dir, tmp_path, M, N, K
 
 def test_tf32_gemm_launch(mock_dir, tmp_path):
     s = 512
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=3, n=s * s, M=s, N=s, K=s, in_bytes=s * s * 4,
-                                                  aux_bytes=s * s * 4, out_bytes=s * s * 4, flags=3)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=3, n=s * s, M=s, N=s, K=s, in_bytes=s * s * 4,
+                                               aux_bytes=s * s * 4, out_bytes=s * s * 4, flags=3)], "child.py")
     assert res["ops"][0]["rc"] == 0 and not [e for e in ev if e["op"] == "error"]
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]][0]
     assert la["name"] == "xmr_gemm_tf32_nc3_inj0" and la["block"] == 384 and la["grid"] == 16 and la["smem"] <= 232448
     tm = [e for e in ev if e["op"] == "tmap"]
     assert [t["rank"] for t in tm] == [2, 2] and tm[1]["swizzle"] == tm[0]["swizzle"]      # A and B^T: both K-major, 128-byte swizzle
     assert [e["name"] for e in ev if e["op"] == "launch" and e["name"] != "xmr_counters_reset"][0] == "xmr_gemm_bt"   # B transposed first
-    bad, _ = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=3, n=100 * 128, M=100, N=128, K=64, in_bytes=100 * 64 * 4,
-                                                  aux_bytes=64 * 128 * 4, out_bytes=100 * 128 * 4)])
+    bad, _, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=3, n=100 * 128, M=100, N=128, K=64, in_bytes=100 * 64 * 4,
+                                              aux_bytes=64 * 128 * 4, out_bytes=100 * 128 * 4)], "child.py")
     assert bad["ops"][0]["rc"] != 0 and "multiples of 128" in bad["ops"][0]["err"]
 
 
@@ -207,8 +169,8 @@ def test_tf32_gemm_kernel_selection_pairs_and_single(mock_dir, tmp_path, nc, M, 
     """which TF32 GEMM kernel a shape gets (single CTA / CTA pair, wide / narrow), with an EVEN grid for the cluster kernels and the
     B box matching what each kernel loads per TMA (64 columns for pairs, 128 for single CTAs)"""
     env = {"COAST_GEMM_PAIR": pair_env} if pair_env is not None else None
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=nc, n=M * N, M=M, N=N, K=64, in_bytes=M * 64 * 4,
-                                                  aux_bytes=64 * N * 4, out_bytes=M * N * 4, flags=3)], env_extra=env)
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_GEMM_TF32, nc=nc, n=M * N, M=M, N=N, K=64, in_bytes=M * 64 * 4,
+                                               aux_bytes=64 * N * 4, out_bytes=M * N * 4, flags=3)], "child.py", env_extra=env)
     assert res["ops"][0]["rc"] == 0 and not [e for e in ev if e["op"] == "error"], res
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]][0]
     assert (la["name"], la["grid"], la["block"]) == (want_name, want_grid, 384) and la["smem"] <= 232448
@@ -253,7 +215,7 @@ def test_launches_use_the_kernels_declared_cta_size_and_whole_clusters(mock_dir,
         ops += [dict(op="launch", kernel=7, nc=nc, n=333, mode=mode, in_bytes=333 * 64, out_bytes=333 * 64) for mode in (0, 1)]
     seen = set()
     for env in ({}, {"COAST_GEMM_PAIR": "1", "COAST_QSORT_PATH": "nested"}, {"COAST_GEMM_PAIR": "0"}):
-        res, ev = run_child(mock_dir, tmp_path, ops, env_extra=env)
+        res, ev, _ = run(mock_dir, tmp_path, ops, "child.py", env_extra=env)
         assert all(r["rc"] == 0 for r in res["ops"]), res
         for la in (e for e in ev if e["op"] == "launch" and "_nc" in e["name"]):
             threads, cluster = bounds[la["name"]]
@@ -269,20 +231,20 @@ def test_gemm_tuning_switches_reach_the_kernel_as_mode_bits(mock_dir, tmp_path):
     s = 512
     gemm = dict(op="launch", kernel=K_GEMM_TF32, nc=3, n=s * s, M=s, N=s, K=64, in_bytes=s * 64 * 4, aux_bytes=64 * s * 4, out_bytes=s * s * 4, flags=3)
     mm = dict(op="launch", kernel=K_MM_U32, nc=3, n=s * s, M=s, N=s, K=128, in_bytes=s * 128 * 4, aux_bytes=128 * s * 4, out_bytes=s * s * 4, flags=3)
-    res, ev = run_child(mock_dir, tmp_path, [gemm, mm], env_extra={"COAST_MM_PATH": "tc"})
+    res, ev, _ = run(mock_dir, tmp_path, [gemm, mm], "child.py", env_extra={"COAST_MM_PATH": "tc"})
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert [x["name"] for x in la] == ["xmr_gemm_tf32_nc3_inj0", "xmr_mm_u32_tc_nc3_inj0"]
     assert args_of(la[0]).mode == 0x100 and args_of(la[1]).mode == 0
     env = {"COAST_GEMM_GROUP_M": "8", "COAST_GEMM_L2_HINTS": "0", "COAST_GEMM_TAIL_SPLIT": "0", "COAST_MM_PATH": "tc"}
-    res, ev = run_child(mock_dir, tmp_path, [gemm, mm], env_extra=env)
+    res, ev, _ = run(mock_dir, tmp_path, [gemm, mm], "child.py", env_extra=env)
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert args_of(la[0]).mode == 8 | 0x200 and args_of(la[1]).mode == 0
 
 
 def test_quicksort_through_the_host_call_uses_one_scratch_slot_per_chunk(mock_dir, tmp_path):
     n, L = 3000, 580
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host", kernel=K_QSORT, nc=3, n=n, unit_bytes=4 * L, in_bytes=n * 4 * L,
-                                                  out_bytes=n * 4 * L), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_QSORT, nc=3, n=n, unit_bytes=4 * L, in_bytes=n * 4 * L,
+                                               out_bytes=n * 4 * L), dict(op="shutdown")], "child.py")
     assert res["ops"][0]["rc"] == 0 and not [e for e in ev if e["op"] == "error"]
     launches = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert sum(args_of(la).n_units for la in launches) == n and all(args_of(la).aux for la in launches)
@@ -292,9 +254,9 @@ def test_quicksort_through_the_host_call_uses_one_scratch_slot_per_chunk(mock_di
 def test_host_call_staging_is_bounded_by_the_call_not_by_the_largest_chunk(mock_dir, tmp_path):
     """one 64 MiB CHStone stream, and a 1-unit crc16 call: the staging slots must not be sized for 1024 units"""
     big = 64 << 20
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CHSTONE_SHA, nc=3, n=1, unit_bytes=big, in_bytes=big, out_bytes=20),
-                                             dict(op="run_host", kernel=K_CRC16, nc=3, n=1, unit_bytes=13, in_bytes=13, out_bytes=2),
-                                             dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CHSTONE_SHA, nc=3, n=1, unit_bytes=big, in_bytes=big, out_bytes=20),
+                                          dict(op="run_host", kernel=K_CRC16, nc=3, n=1, unit_bytes=13, in_bytes=13, out_bytes=2),
+                                          dict(op="shutdown")], "child.py")
     assert [r["rc"] for r in res["ops"]] == [0, 0, 0], res
     assert max(e["bytes"] for e in ev if e["op"] == "alloc") <= big + 4096
     assert ev[-1] == {"op": "exit", "live_allocations": 0}
@@ -303,7 +265,7 @@ def test_host_call_staging_is_bounded_by_the_call_not_by_the_largest_chunk(mock_
 def test_reference_entry_points_drive_the_host_call(mock_dir, tmp_path):
     """crc16 / sha256_hash (10 bytes and empty) / aes_enc_dec both directions / matrix_multiply 9x9 / sha_stream: one protected
     launch each with the mode of OPT_PASSES, buffers staged and released"""
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="entries", passes="-TMR -countErrors"), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="entries", passes="-TMR -countErrors"), dict(op="shutdown")], "child.py")
     assert res["ops"][0]["rc"] == 0 and not [e for e in ev if e["op"] == "error"], [e for e in ev if e["op"] == "error"]
     names = [e["name"] for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert names == ["xmr_crc16_gen_nc3_inj0", "xmr_sha256_gen_nc3_inj0", "xmr_sha256_gen_nc3_inj0", "xmr_aes128_enck_nc3_inj0",
@@ -317,8 +279,8 @@ def test_reference_entry_points_drive_the_host_call(mock_dir, tmp_path):
 
 def test_aes_per_unit_keys_with_write_back_through_the_host_call(mock_dir, tmp_path):
     n = 200000
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=K_AES128, nc=2, n=n, mode=2 | 4, in_bytes=16 * n, aux_bytes=16 * n,
-                                                  out_bytes=16 * n), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=K_AES128, nc=2, n=n, mode=2 | 4, in_bytes=16 * n, aux_bytes=16 * n,
+                                               out_bytes=16 * n), dict(op="shutdown")], "child.py")
     r = res["ops"][0]
     assert r["rc"] == 0 and not [e for e in ev if e["op"] == "error"]
     for key, direction in (("host_in", "h2d"), ("host_aux", "h2d"), ("host_out", "d2h"), ("host_aux", "d2h")):
@@ -334,8 +296,8 @@ def test_aes_per_unit_keys_with_write_back_through_the_host_call(mock_dir, tmp_p
 def test_large_matmul_through_the_host_call_is_pipelined_by_row_blocks(mock_dir, tmp_path):
     """B once; A rows up / launch / C rows down per block on rotating streams; every block's launch is keyed by its global element index"""
     M, N, K = 1024, 256, 128
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=K_GEMM_TF32, nc=3, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4,
-                                                  aux_bytes=K * N * 4, out_bytes=M * N * 4, unit_base=5), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=K_GEMM_TF32, nc=3, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4,
+                                               aux_bytes=K * N * 4, out_bytes=M * N * 4, unit_base=5), dict(op="shutdown")], "child.py")
     r = res["ops"][0]
     assert r["rc"] == 0 and not [e for e in ev if e["op"] == "error"], (r, [e for e in ev if e["op"] == "error"])
     launches = [(e, args_of(e)) for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
@@ -350,8 +312,8 @@ def test_large_matmul_through_the_host_call_is_pipelined_by_row_blocks(mock_dir,
 
 def test_matmul_through_the_host_call_is_one_shot(mock_dir, tmp_path):
     M = N = K = 128
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=K_MM_U32, nc=3, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4,
-                                                  aux_bytes=K * N * 4, out_bytes=M * N * 4), dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_aux", kernel=K_MM_U32, nc=3, n=M * N, M=M, N=N, K=K, in_bytes=M * K * 4,
+                                               aux_bytes=K * N * 4, out_bytes=M * N * 4), dict(op="shutdown")], "child.py")
     assert res["ops"][0]["rc"] == 0 and not [e for e in ev if e["op"] == "error"]
     assert [e["bytes"] for e in ev if e["op"] == "h2d"] == [M * K * 4, K * N * 4]
     assert [e["bytes"] for e in ev if e["op"] == "d2h" and e["bytes"] > 64] == [M * N * 4]
@@ -383,15 +345,15 @@ def test_lifecycle_and_small_api_calls(mock_dir, tmp_path):
     (3, 0, 1, "xmr_sha256_b64_nc1_inj0"),
 ])
 def test_sha_layout_flags_select_the_kernel(mock_dir, tmp_path, flags, mode, nc, want):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_SHA256, nc=nc, n=5000, unit_bytes=64, in_bytes=320000, out_bytes=160000,
-                                                  flags=flags)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_SHA256, nc=nc, n=5000, unit_bytes=64, in_bytes=320000, out_bytes=160000,
+                                               flags=flags)], "child.py")
     assert [e["name"] for e in ev if e["op"] == "launch" and "_nc" in e["name"]] == [want]
 
 
 def test_aes_decrypt_and_per_unit_keys_select_the_table_kernels(mock_dir, tmp_path):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="launch", kernel=K_AES128, nc=2, n=1000, mode=1, in_bytes=16000, out_bytes=16000),
-                                             dict(op="launch", kernel=K_AES128, nc=2, n=1000, mode=2, in_bytes=16000, out_bytes=16000, aux_bytes=16000),
-                                             dict(op="launch", kernel=K_AES128, nc=2, n=1000, mode=2, in_bytes=16000, out_bytes=16000)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_AES128, nc=2, n=1000, mode=1, in_bytes=16000, out_bytes=16000),
+                                          dict(op="launch", kernel=K_AES128, nc=2, n=1000, mode=2, in_bytes=16000, out_bytes=16000, aux_bytes=16000),
+                                          dict(op="launch", kernel=K_AES128, nc=2, n=1000, mode=2, in_bytes=16000, out_bytes=16000)], "child.py")
     assert [r["rc"] == 0 for r in res["ops"]] == [True, True, False] and "per-unit keys need d_aux" in res["ops"][2]["err"]
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert [e["name"] for e in la] == ["xmr_aes128_dec_nc2_inj0", "xmr_aes128_enck_nc2_inj0"]
@@ -401,8 +363,8 @@ def test_aes_decrypt_and_per_unit_keys_select_the_table_kernels(mock_dir, tmp_pa
 def test_sync_folds_counters_into_the_reference_symbols(mock_dir, tmp_path):
     """coast_sync(): device counters -> coast_stats, TMR_ERROR_CNT (an i32 in the reference: wraps, synchronization.cpp:1428-1431),
     __SYNC_COUNT (i64), and the counters start from zero again"""
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="sync_fold"), dict(op="sync_fold"), dict(op="shutdown")],
-                        env_extra={"MOCK_CUDA_TALLY": f"{2 ** 32 + 5},0,3200,7,41"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="sync_fold"), dict(op="sync_fold"), dict(op="shutdown")], "child.py",
+                     env_extra={"MOCK_CUDA_TALLY": f"{2 ** 32 + 5},0,3200,7,41"})
     a, b = res["ops"][0], res["ops"][1]
     assert a["launch"] == 0 and a["sync"] == 0 and a["stats"] == [2 ** 32 + 5, 0, 3200, 7, 41]
     assert a["TMR_ERROR_CNT"] == 5 and a["SYNC_COUNT"] == 3200 and a["second"] == [0, 0, 0, 0, 2 ** 64 - 1]
@@ -413,7 +375,7 @@ def test_peer_counter_block_receives_the_tallies_of_an_attached_process(mock_dir
     """coast_counters_attach(): every later kernel's argument block points at the OWNER's counters (the multi-GPU fold over NVLink
     peer memory, no collective); the attached process's coast_sync() reports zeros and never resets the owner's block; detach
     restores the local block; no peer access -> a loud error, not a silent local tally"""
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="peer_counters"), dict(op="shutdown")], env_extra={"MOCK_CUDA_TALLY": "4,0,3200,7,41"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="peer_counters"), dict(op="shutdown")], "child.py", env_extra={"MOCK_CUDA_TALLY": "4,0,3200,7,41"})
     r = res["ops"][0]
     assert r["export"] == 0 and r["attach"] == 0 and r["attach_twice"] != 0 and r["launch"] == 0 and r["sync_attached"] == 0
     launches = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
@@ -425,14 +387,14 @@ def test_peer_counter_block_receives_the_tallies_of_an_attached_process(mock_dir
     opens = [e for e in ev if e["op"] == "ipc_open"]
     assert len(opens) == 1 and opens[0]["flags"] == 1                                # CU_IPC_MEM_LAZY_ENABLE_PEER_ACCESS
     assert [e for e in ev if e["op"] == "ipc_close"]
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="peer_counters")], env_extra={"MOCK_IPC_FAIL": "1"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="peer_counters")], "child.py", env_extra={"MOCK_IPC_FAIL": "1"})
     r = res["ops"][0]
     assert r["attach"] != 0 and "peer" in r["attach_err"]
 
 
 def test_dwc_detection_calls_the_handler_which_aborts_by_default(mock_dir, tmp_path):
     """FAULT_DETECTED_DWC() (synchronization.cpp:1251-1266: default = abort()) is called by coast_sync, not by coast_sync_noabort"""
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="sync_fold", nc=2)], env_extra={"MOCK_CUDA_TALLY": "0,3,0,3,17"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="sync_fold", nc=2)], "child.py", env_extra={"MOCK_CUDA_TALLY": "0,3,0,3,17"})
     assert res["ops"][0]["stats"][:2] == [0, 3] and res["ops"][0]["stats"][4] == 17
     log = tmp_path / "mock2.log"
     env = dict(os.environ, LD_LIBRARY_PATH=f"{mock_dir}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=str(log), MOCK_CUDA_TALLY="0,3,0,3,17")
@@ -454,7 +416,7 @@ def test_pinned_buffers_take_the_zero_copy_host_call(mock_dir, tmp_path):
     no staging allocations; COAST_HOST_PATH=staged forces the chunked pipeline on the same buffers"""
     n = 300000
     op = dict(op="run_host_pinned", kernel=K_SHA256, nc=3, n=n, unit_bytes=64, in_bytes=64 * n, out_bytes=32 * n, unit_base=77, status=True)
-    res, ev = run_child(mock_dir, tmp_path, [op, dict(op="shutdown")], env_extra={"COAST_HOST_PATH": "zerocopy"})
+    res, ev, _ = run(mock_dir, tmp_path, [op, dict(op="shutdown")], "child.py", env_extra={"COAST_HOST_PATH": "zerocopy"})
     r = res["ops"][0]
     assert r["rc"] == 0 and not [e for e in ev if e["op"] == "error"], (r, [e for e in ev if e["op"] == "error"])
     launches = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
@@ -464,12 +426,12 @@ def test_pinned_buffers_take_the_zero_copy_host_call(mock_dir, tmp_path):
     assert not [e for e in ev if e["op"] == "h2d"] and all(e["bytes"] <= 64 for e in ev if e["op"] == "d2h")     # only the counters come back by copy
     assert ev[-1] == {"op": "exit", "live_allocations": 0}
     for forced in ({"COAST_HOST_PATH": "staged"}, {}):                       # the default is the staged pipeline (r02 measurement)
-        res, ev = run_child(mock_dir, tmp_path / "..", [op, dict(op="shutdown")], env_extra=forced)
+        res, ev, _ = run(mock_dir, tmp_path / "..", [op, dict(op="shutdown")], "child.py", env_extra=forced)
         r = res["ops"][0]
         assert r["rc"] == 0 and len([e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]) > 1
         _contiguous([(e["host"] - r["host_in"], e["bytes"]) for e in ev if e["op"] == "h2d"], 64 * n)
     # hybrid: chunked launches read the pinned input in place (no upload copies), outputs and status bytes are staged per chunk
-    res, ev = run_child(mock_dir, tmp_path / "..", [op, dict(op="shutdown")], env_extra={"COAST_HOST_PATH": "hybrid"})
+    res, ev, _ = run(mock_dir, tmp_path / "..", [op, dict(op="shutdown")], "child.py", env_extra={"COAST_HOST_PATH": "hybrid"})
     r = res["ops"][0]
     launches = [args_of(e) for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert r["rc"] == 0 and len(launches) > 1 and not [e for e in ev if e["op"] == "h2d"]
@@ -485,21 +447,21 @@ def test_default_host_path_is_zero_copy_only_for_tiny_outputs(mock_dir, tmp_path
     """measured policy (profiles/r02_e2e_*.json): staged by default; pinned buffers + an output of at most 1/8 of the input (crc16: 2 of 64
     bytes) -> one zero-copy launch; the same call with pageable memory falls back to the staged pipeline"""
     n = 200000
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_pinned", kernel=K_CRC16, nc=3, n=n, unit_bytes=64, in_bytes=64 * n, out_bytes=2 * n),
-                                             dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_pinned", kernel=K_CRC16, nc=3, n=n, unit_bytes=64, in_bytes=64 * n, out_bytes=2 * n),
+                                          dict(op="shutdown")], "child.py")
     la = [e for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert res["ops"][0]["rc"] == 0 and len(la) == 1 and args_of(la[0]).inp == res["ops"][0]["host_in"] and not [e for e in ev if e["op"] == "h2d"]
-    res, ev = run_child(mock_dir, tmp_path / "..", [dict(op="run_host", kernel=K_CRC16, nc=3, n=n, unit_bytes=64, in_bytes=64 * n, out_bytes=2 * n)])
+    res, ev, _ = run(mock_dir, tmp_path / "..", [dict(op="run_host", kernel=K_CRC16, nc=3, n=n, unit_bytes=64, in_bytes=64 * n, out_bytes=2 * n)], "child.py")
     assert res["ops"][0]["rc"] == 0 and [e for e in ev if e["op"] == "h2d"]
 
 
 def test_zero_copy_is_refused_for_pageable_buffers_only_when_forced(mock_dir, tmp_path):
     op = dict(op="run_host", kernel=K_SHA256, nc=3, n=1000, unit_bytes=64, in_bytes=64000, out_bytes=32000)
-    res, ev = run_child(mock_dir, tmp_path, [op], env_extra={"COAST_HOST_PATH": "zerocopy"})
+    res, ev, _ = run(mock_dir, tmp_path, [op], "child.py", env_extra={"COAST_HOST_PATH": "zerocopy"})
     assert res["ops"][0]["rc"] != 0 and "pinned" in res["ops"][0]["err"]
-    res, ev = run_child(mock_dir, tmp_path / "..", [op], env_extra={"COAST_HOST_PATH": "hybrid"})
+    res, ev, _ = run(mock_dir, tmp_path / "..", [op], "child.py", env_extra={"COAST_HOST_PATH": "hybrid"})
     assert res["ops"][0]["rc"] != 0 and "pinned" in res["ops"][0]["err"]
-    res, ev = run_child(mock_dir, tmp_path / "..", [op])                       # default: the staged pipeline
+    res, ev, _ = run(mock_dir, tmp_path / "..", [op], "child.py")                       # default: the staged pipeline
     assert res["ops"][0]["rc"] == 0 and [e for e in ev if e["op"] == "h2d"]
 
 
@@ -507,8 +469,8 @@ def test_host_call_stages_the_status_bytes_per_chunk(mock_dir, tmp_path):
     """ADVICE r01: kernels index status[] chunk-locally, so the host call must give every chunk its own device status
     buffer and copy it back to (host status + units done)"""
     n = 300001
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host_status", kernel=K_AES128, nc=2, n=n, in_bytes=16 * n, out_bytes=16 * n),
-                                             dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host_status", kernel=K_AES128, nc=2, n=n, in_bytes=16 * n, out_bytes=16 * n),
+                                          dict(op="shutdown")], "child.py")
     r = res["ops"][0]
     assert r["rc"] == 0 and not [e for e in ev if e["op"] == "error"]
     launches = [args_of(e) for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
@@ -520,8 +482,8 @@ def test_host_call_stages_the_status_bytes_per_chunk(mock_dir, tmp_path):
 def test_host_call_chunks_are_bounded_in_bytes(mock_dir, tmp_path):
     """ADVICE r01: 1024-unit floor x 48 MiB streams used to ask for hundreds of GiB; a unit above the byte bound is its own chunk"""
     big, n = 48 << 20, 5
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CHSTONE_SHA, nc=3, n=n, unit_bytes=big, in_bytes=n * big, out_bytes=n * 20),
-                                             dict(op="shutdown")])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CHSTONE_SHA, nc=3, n=n, unit_bytes=big, in_bytes=n * big, out_bytes=n * 20),
+                                          dict(op="shutdown")], "child.py")
     assert res["ops"][0]["rc"] == 0, res
     launches = [args_of(e) for e in ev if e["op"] == "launch" and "_nc" in e["name"]]
     assert [a.n_units for a in launches] == [1] * n and max(e["bytes"] for e in ev if e["op"] == "alloc") <= big + 4096
@@ -532,8 +494,8 @@ def test_a_failing_chunk_drains_the_copies_already_queued(mock_dir, tmp_path):
     """the host call must not return while earlier chunks' copies are still in flight on the caller's buffers: after a driver failure
     in a later chunk (here: a staging allocation above the mock box's 6 GiB) the streams are synchronised before the error comes back"""
     big, n = 5 << 30, 2                                                         # first slot fits, the second does not
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CHSTONE_SHA, nc=3, n=n, unit_bytes=1 << 28, in_bytes=n << 28, out_bytes=n * 20)],
-                        env_extra={"COAST_HOST_CHUNK_BYTES": str(1 << 28), "MOCK_CUDA_FAIL_ALLOC_AFTER": "6"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CHSTONE_SHA, nc=3, n=n, unit_bytes=1 << 28, in_bytes=n << 28, out_bytes=n * 20)], "child.py",
+                     env_extra={"COAST_HOST_CHUNK_BYTES": str(1 << 28), "MOCK_CUDA_FAIL_ALLOC_AFTER": "6"})
     r = res["ops"][0]
     if r["rc"] != 0:                                                            # the injected failure fired mid-schedule
         syncs = [i for i, e in enumerate(ev) if e["op"] == "stream_sync"]
@@ -542,7 +504,7 @@ def test_a_failing_chunk_drains_the_copies_already_queued(mock_dir, tmp_path):
 
 
 def test_single_caller_guard(mock_dir, tmp_path):
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="two_threads", iters=20000)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="two_threads", iters=20000)], "child.py")
     r = res["ops"][0]
     assert set(r["codes"]) <= {0, -100005} and 0 in r["codes"] and r["after"] == 0
 
@@ -550,7 +512,7 @@ def test_single_caller_guard(mock_dir, tmp_path):
 def test_sha256_entry_point_writes_the_callers_ctx_scratch(mock_dir, tmp_path):
     """ADVICE r01: sha256_hash leaves ctx_state / ctx_bitlen / ctx_data behind (sha256_common_tmr.c:101-180); ctx_state must be
     the big-endian words of the digest the launch returned, bitlen = 8*len and ctx_data the last padded block"""
-    res, ev = run_child(mock_dir, tmp_path, [dict(op="sha_ctx", lens=[10, 55, 56, 64, 119, 200])])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="sha_ctx", lens=[10, 55, 56, 64, 119, 200])], "child.py")
     for rec in res["ops"][0]["recs"]:
         ln = rec["len"]
         assert rec["bitlen"] == [(8 * ln) & 0xFFFFFFFF, ln >> 29]

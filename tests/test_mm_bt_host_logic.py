@@ -1,80 +1,16 @@
-"""Host logic of COAST_MM_B_TRANSPOSED on a GPU-less box, against the mock driver (tests/mock_cuda/mock_cuda_bt.c: mock_cuda.c
-with 2-byte tensor-map elements and the start of every map logged).  Every launch form of every matmul path is run with and
+"""Host logic of COAST_MM_B_TRANSPOSED on a GPU-less box, against the mock driver (tests/mock_cuda/mock_cuda.c) through
+tests/mock_cuda/mm_child.py.  Every launch form of every matmul path is run with and
 without the bit and the two records are compared.  Pinned here: the kernel the bit selects, with the grid, block and shared
 memory of the B launch; that GEMM_TF32 runs no transposing pre-pass and allocates no B^T scratch (grouped: the group block and
 the scan alone); that the limb path splits B^T with the streaming split of A into the same planes; that B's map lies on the
 caller's d_aux as (batch N) or (G N) rows of K with the per-kernel box; every refusal; and the bytes a host call copies."""
-import json
-import os
-import subprocess
-import sys
-
 import pytest
 
-from test_host_logic import ROOT, args_of
+from mock_run import (BAD_ARG, GRP_BYTES, K_AES128, K_CHSTONE_AES, K_CHSTONE_SHA, K_CRC16, K_GEMM_BF16, K_GEMM_TF32,  # noqa: F401
+                      K_MM_U32, K_QSORT, K_SHA256, MM_B_TRANSPOSED as BT, MM_BATCHED, MM_ELEM_BYTES, MM_GROUPED, arg0_ptr, args_of,
+                      maps, mock_dir, run, scratch, spans, work)
 
-MM_GROUPED, MM_BATCHED, BT = 0x40000, 0x20000, 0x80000
-K_CRC16, K_SHA256, K_AES128, K_MM_U32, K_GEMM_TF32, K_QSORT, K_CHSTONE_SHA, K_CHSTONE_AES, K_GEMM_BF16 = range(9)
-BAD_ARG = -100003
 PREPASSES = ("xmr_gemm_bt", "xmr_mm_split_a", "xmr_mm_split_bt", "xmr_mm_grp_split_a", "xmr_mm_group_scan")
-GRP_BYTES = lambda G: 128 + 4 * (G + 1)                  # noqa: E731  (xmr_mm_grp_bytes)
-KNOBS = ("COAST_GEMM_PAIR", "COAST_GEMM_GROUP_M", "COAST_GEMM_L2_HINTS", "COAST_GEMM_TAIL_SPLIT", "COAST_HOST_CHUNK_BYTES",
-         "COAST_HOST_PATH", "COAST_STRICT_FLAGS", "COAST_MM_PATH")
-
-
-@pytest.fixture(scope="session")
-def mock_dir(tmp_path_factory, built_lib):
-    d = tmp_path_factory.mktemp("mockcuda_bt")
-    subprocess.run(["gcc", "-O1", "-shared", "-fPIC", "-Wall", "-I/usr/local/cuda/include", "-o", str(d / "libcuda.so.1"),
-                    os.path.join(ROOT, "tests", "mock_cuda", "mock_cuda_bt.c")], check=True)
-    return d
-
-
-def run(mock_dir, tmp_path, ops, env_extra=None, driver_errors=False):
-    log = tmp_path / "mock.log"
-    if log.exists():
-        log.unlink()
-    env = dict(os.environ, LD_LIBRARY_PATH=f"{mock_dir}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=str(log))
-    for k in KNOBS:
-        env.pop(k, None)
-    env.update(env_extra or {})
-    res = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mock_cuda", "mm_bt_child.py"), json.dumps({"ops": ops})],
-                         capture_output=True, text=True, env=env, timeout=300)
-    assert res.returncode == 0, res.stdout + res.stderr
-    events = [json.loads(ln) for ln in open(log)] if log.exists() else []
-    if not driver_errors:
-        assert not [e for e in events if e["op"] == "error"], [e for e in events if e["op"] == "error"]
-    assert events[-1] == {"op": "exit", "live_allocations": 0}
-    return json.loads(res.stdout.strip().splitlines()[-1]), events
-
-
-def work(ev):
-    return [e for e in ev if e["op"] == "launch" and e["name"] != "xmr_counters_reset"]
-
-
-def maps(ev):
-    """(start, element bytes, dim0, dim1, box0, box1) of every tensor map, in encoding order"""
-    out = []
-    for i, e in enumerate(ev):
-        if e["op"] == "tmap_at":
-            t = ev[i + 1]
-            assert t["op"] in ("tmap", "tmap16")
-            out.append((e["addr"], t["elem"], t["dim0"], t["dim1"], t["box0"], t["box1"]))
-    return out
-
-
-def scratch(ev, sizes):
-    """bytes of every allocation after the caller's buffers (sizes, in order) and before the matmul kernel"""
-    allocs = [(i, e["bytes"]) for i, e in enumerate(ev) if e["op"] == "alloc" and not e["host"]]
-    for j in range(len(allocs) - len(sizes) + 1):
-        if [b for _, b in allocs[j:j + len(sizes)]] == sizes:
-            k = ev.index(work(ev)[-1])
-            return [b for i, b in allocs[j + len(sizes):] if i < k]
-    raise AssertionError("the caller's buffers are not in the log")
-
-
-def arg0_ptr(launch):
-    return int.from_bytes(bytes.fromhex(launch["arg0"]), "little")
 
 
 RO = [3, 3, 100, 101, 101, 500, 700]
@@ -121,7 +57,7 @@ LAUNCHES = [
 def test_the_bit_keeps_the_launch_and_reads_b_transposed_in_place(mock_dir, tmp_path, case):
     _, op, e, name = case
     op = dict(op, op="launch", unit_base=(1 << 32) - 5)
-    (rb, evb), (rt_, evt) = [run(mock_dir, tmp_path, [dict(op, bt=bt)], env_extra=e) for bt in (False, True)]
+    (rb, evb, _), (rt_, evt, _) = [run(mock_dir, tmp_path, [dict(op, bt=bt)], env_extra=e) for bt in (False, True)]
     rb, rt_ = rb["ops"][0], rt_["ops"][0]
     assert rb["rc"] == 0 and rt_["rc"] == 0, (rb, rt_)
     lb, lt = work(evb), work(evt)
@@ -148,7 +84,7 @@ def test_the_bit_keeps_the_launch_and_reads_b_transposed_in_place(mock_dir, tmp_
         assert pre_t == pre_b == (["xmr_mm_group_scan"] if grouped and "_tiled_" in name else [])
         assert st == sb and not maps(evt)
     else:
-        es = 2 if kernel == K_GEMM_BF16 else 4
+        es = MM_ELEM_BYTES.get(kernel, 4)
         pair = "tf32p_" in name or "bf16p_" in name
         # no transposing pre-pass and no B^T scratch: the scan and the group block alone for groups, nothing otherwise
         assert pre_t == (["xmr_mm_group_scan"] if grouped else [])
@@ -178,7 +114,7 @@ REFUSALS = [
 @pytest.mark.parametrize("case", REFUSALS, ids=[c[0] for c in REFUSALS])
 def test_the_bit_on_any_other_kernel_is_refused(mock_dir, tmp_path, case, call):
     _, op = case
-    res, ev = run(mock_dir, tmp_path, [dict(op, op=call, bt=True, alloc=[4096, 4096, 4096])])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op, op=call, bt=True, alloc=[4096, 4096, 4096])])
     r = res["ops"][0]
     assert r["rc"] == BAD_ARG and "COAST_MM_B_TRANSPOSED" in r["err"] and "MM_U32, GEMM_TF32 and GEMM_BF16 only" in r["err"], r
     assert not work(ev) and not [e for e in ev if e["op"] == "h2d"]
@@ -198,39 +134,35 @@ def test_bf16_b_rows_bound_moves_from_k_to_n(mock_dir, tmp_path, form):
         needle = "G*%s must be below 2^31"
     for op, refused_with in ((wide_n, True), (wide_k, False)):
         for bt in (False, True):
-            res, ev = run(mock_dir, tmp_path, [dict(op, op="launch", kernel=K_GEMM_BF16, nc=3, bt=bt)], driver_errors=True)
+            res, ev, _ = run(mock_dir, tmp_path, [dict(op, op="launch", kernel=K_GEMM_BF16, nc=3, bt=bt)], driver_errors=True)
             r = res["ops"][0]
             refused = bt == refused_with
             if refused:
                 assert r["rc"] == BAD_ARG and needle % ("N" if bt else "K") in r["err"], (op, bt, r)
             else:                                                  # past the bound, as far as the maps: the mock's buffers are too small
-                assert "2^31" not in r["err"] and [e for e in ev if e["op"] == "tmap_at"], (op, bt, r)
+                assert "2^31" not in r["err"] and "cuTensorMapEncodeTiled" in r["err"], (op, bt, r)
                 assert {"op": "error", "what": "tensor map covers memory outside a live allocation"} in ev
             assert not work(ev)
 
 
 def test_bound_on_tf32_and_mm_u32_stays_on_n(mock_dir, tmp_path):
     for kernel in (K_GEMM_TF32, K_MM_U32):
-        res, ev = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=3, M=128, N=256, K=64, batch=1 << 23, bt=True, alloc=[16, 16, 16])])
+        res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=3, M=128, N=256, K=64, batch=1 << 23, bt=True, alloc=[16, 16, 16])])
         r = res["ops"][0]
         assert r["rc"] == BAD_ARG and "batch*M and batch*N must be below 2^31" in r["err"] and not work(ev)
 
 
 @pytest.mark.parametrize("kernel", [K_GEMM_TF32, K_GEMM_BF16])
 def test_misaligned_b_transposed_is_refused(mock_dir, tmp_path, kernel):
-    res, ev = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=3, M=128, N=128, K=64, bt=True, shift=[0, 4, 0])])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=kernel, nc=3, M=128, N=128, K=64, bt=True, shift=[0, 4, 0])])
     r = res["ops"][0]
     assert r["rc"] == BAD_ARG and "16-byte aligned" in r["err"] and not work(ev)
 
 
 def test_misaligned_b_transposed_takes_the_plain_mm_u32_kernel(mock_dir, tmp_path):
     """as without the bit: the tensor-core and tiled paths need 16-byte aligned buffers, the plain kernel takes any"""
-    res, ev = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_MM_U32, nc=2, M=128, N=128, K=128, bt=True, shift=[0, 4, 0])])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_MM_U32, nc=2, M=128, N=128, K=128, bt=True, shift=[0, 4, 0])])
     assert res["ops"][0]["rc"] == 0 and [e["name"] for e in work(ev)] == ["xmr_mm_u32_bt_inj0_nc2"]
-
-
-def spans(ev, op, base, size):
-    return [(e["host"] - base, e["bytes"], e["stream"]) for e in ev if e["op"] == op and base <= e["host"] < base + size]
 
 
 def copies(ev, r, sizes):
@@ -257,10 +189,10 @@ def test_host_call_copies_the_bytes_of_the_b_layout(mock_dir, tmp_path, case, pi
     _, op, e, path = case
     recs = []
     for bt in (False, True):
-        res, ev = run(mock_dir, tmp_path, [dict(op, op="run_host", bt=bt, pinned=pinned, unit_base=5)], env_extra=e)
+        res, ev, _ = run(mock_dir, tmp_path, [dict(op, op="run_host", bt=bt, pinned=pinned, unit_base=5)], env_extra=e)
         r = res["ops"][0]
         assert r["rc"] == 0 and r["path"] == path, r
-        es = 2 if op["kernel"] == K_GEMM_BF16 else 4
+        es = MM_ELEM_BYTES.get(op["kernel"], 4)
         ro = op.get("ro")
         rows, b = (ro[-1], len(ro) - 1) if ro else (op.get("batch", 1) * op["M"], op.get("batch", 1))
         sizes = (es * rows * op["K"], es * b * op["K"] * op["N"], 4 * rows * op["N"], 8 * len(ro) if ro else 0)

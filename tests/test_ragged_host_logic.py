@@ -2,34 +2,11 @@
 kernel selection and the stream-ordered cost-ordering pre-pass, the argument block, loud failures for bad arguments and bad
 host offsets, and the chunk schedule of the ragged host call (every byte copied once, each offset slice uploaded unchanged
 with the input pointer biased by its first offset, a long unit alone in its chunk, no zero-copy path)."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-from test_host_logic import ROOT, _declared_bounds, args_of, mock_dir  # noqa: F401  (mock_dir is a fixture)
-
-UNIT_OFFSETS = 0x10000
-K_CRC16, K_SHA256, K_AES128 = 0, 1, 2
-BAD_ARG, UNSUPPORTED = -100003, -100004
-
-
-def run(mock_dir, tmp_path, ops, env_extra=None):
-    log = tmp_path / "mock.log"
-    if log.exists():
-        log.unlink()
-    env = dict(os.environ, LD_LIBRARY_PATH=f"{mock_dir}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=str(log))
-    env.update(env_extra or {})
-    res = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mock_cuda", "ragged_child.py"), json.dumps({"ops": ops})],
-                         capture_output=True, text=True, env=env, timeout=300)
-    assert res.returncode == 0, res.stdout + res.stderr
-    events = [json.loads(ln) for ln in open(log)] if log.exists() else []
-    assert not [e for e in events if e["op"] == "error"], [e for e in events if e["op"] == "error"]
-    assert events[-1] == {"op": "exit", "live_allocations": 0}
-    return json.loads(res.stdout.strip().splitlines()[-1]), events
+from mock_run import BAD_ARG, K_AES128, K_CRC16, K_SHA256, UNSUPPORTED, UNIT_OFFSETS, args_of, mock_dir, run  # noqa: F401
+from test_host_logic import _declared_bounds
 
 
 def offsets(lens, first=3):
@@ -47,7 +24,7 @@ def test_ragged_launch_runs_the_prepass_then_the_var_kernel_and_frees_its_scratc
     op = dict(op="launch", kernel=kernel, nc=nc, offsets=off, unit_bytes=255, unit_base=1 << 32, flags=3)
     if p:
         op["p"] = p
-    res, ev = run(mock_dir, tmp_path, [op])
+    res, ev, _ = run(mock_dir, tmp_path, [op], "ragged_child.py")
     r = res["ops"][0]
     assert r["rc"] == 0, r["err"]
     launches = [e for e in ev if e["op"] == "launch" and e["name"] != "xmr_counters_reset"]
@@ -71,21 +48,21 @@ def test_bad_ragged_arguments_fail_loudly(mock_dir, tmp_path, case):
     op.update({"aes": dict(kernel=K_AES128), "crc_bound": dict(kernel=K_CRC16, unit_bytes=256),
                "sha_bound": dict(unit_bytes=(1 << 28) + 1), "null_aux": dict(null_aux=True),
                "misaligned_aux": dict(aux_misalign=4), "n_too_large": dict(n=1 << 32)}[case])
-    res, ev = run(mock_dir, tmp_path, [op])
+    res, ev, _ = run(mock_dir, tmp_path, [op], "ragged_child.py")
     r = res["ops"][0]
     assert r["rc"] == BAD_ARG and "COAST_UNIT_OFFSETS" in r["err"], r
     assert not [e for e in ev if e["op"] == "launch" and "ragged" in e["name"]]
 
 
 def test_the_bounds_themselves_are_accepted(mock_dir, tmp_path):
-    res, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_CRC16, offsets=offsets([255, 0, 7]), unit_bytes=255),
-                                      dict(op="launch", kernel=K_SHA256, offsets=offsets([9, 0]), unit_bytes=1 << 28)])
+    res, _, _ = run(mock_dir, tmp_path, [dict(op="launch", kernel=K_CRC16, offsets=offsets([255, 0, 7]), unit_bytes=255),
+                                         dict(op="launch", kernel=K_SHA256, offsets=offsets([9, 0]), unit_bytes=1 << 28)], "ragged_child.py")
     assert [r["rc"] for r in res["ops"]] == [0, 0]
 
 
 @pytest.mark.parametrize("offs", [[0, 10, 5, 20], [0, 10, 400, 401]])
 def test_bad_host_offsets_fail_before_any_copy(mock_dir, tmp_path, offs):
-    res, ev = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CRC16, offsets=offs, unit_bytes=255)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CRC16, offsets=offs, unit_bytes=255)], "ragged_child.py")
     r = res["ops"][0]
     assert r["rc"] == BAD_ARG and "offsets must not decrease" in r["err"]
     assert not [e for e in ev if e["op"] in ("h2d", "launch") and e.get("name", "") != "xmr_counters_reset"]
@@ -99,8 +76,8 @@ def test_host_chunk_schedule_copies_every_byte_once_and_each_offset_slice_unchan
     lens[100] = 50000                                          # longer than the chunk bytes: a chunk of its own
     off = offsets(lens, first=5)
     n = len(lens)
-    res, ev = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_SHA256, offsets=off, unit_bytes=50000, pinned=pinned,
-                                            unit_base=1000)], env_extra={"COAST_HOST_CHUNK_BYTES": "20000"})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_SHA256, offsets=off, unit_bytes=50000, pinned=pinned,
+                                               unit_base=1000)], "ragged_child.py", env_extra={"COAST_HOST_CHUNK_BYTES": "20000"})
     r = res["ops"][0]
     assert r["rc"] == 0 and r["path"] == "staged", r
     h2d = [e for e in ev if e["op"] == "h2d"]
@@ -131,9 +108,9 @@ def test_host_chunk_schedule_copies_every_byte_once_and_each_offset_slice_unchan
 
 @pytest.mark.parametrize("path", ["zerocopy", "hybrid"])
 def test_forced_zero_copy_or_hybrid_ragged_host_calls_are_unsupported(mock_dir, tmp_path, path):
-    res, ev = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CRC16, offsets=offsets([3, 9, 0]), unit_bytes=255, pinned=True)],
-                  env_extra={"COAST_HOST_PATH": path})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CRC16, offsets=offsets([3, 9, 0]), unit_bytes=255, pinned=True)], "ragged_child.py",
+                     env_extra={"COAST_HOST_PATH": path})
     r = res["ops"][0]
     assert r["rc"] == UNSUPPORTED and "staged only" in r["err"]
-    res, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CRC16, offsets=offsets([3, 9, 0]), unit_bytes=255, pinned=True)])
+    res, _, _ = run(mock_dir, tmp_path, [dict(op="run_host", kernel=K_CRC16, offsets=offsets([3, 9, 0]), unit_bytes=255, pinned=True)], "ragged_child.py")
     assert res["ops"][0]["rc"] == 0 and res["ops"][0]["path"] == "staged"

@@ -2,35 +2,13 @@
 (tests/mock_cuda/mock_cuda.c): kernel selection after the cost-ordering pre-pass, one scratch allocation holding the pre-pass
 part and the per-warp replica slots, loud failures for bad arguments, and the chunks of the ragged host call (each chunk
 uploads and downloads the same byte span at the same offsets, with both d_in and d_out biased by its first offset)."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-from test_host_logic import ROOT, _declared_bounds, args_of, mock_dir  # noqa: F401  (mock_dir is a fixture)
+from mock_run import BAD_ARG, K_QSORT, SMS, UNSUPPORTED, UNIT_OFFSETS, args_of, mock_dir, run  # noqa: F401
+from test_host_logic import _declared_bounds
 
-UNIT_OFFSETS = 0x10000
-K_QSORT = 5
-BAD_ARG, UNSUPPORTED = -100003, -100004
-QSORT_THREADS, SMS = 128, 132
-
-
-def run(mock_dir, tmp_path, ops, env_extra=None):
-    log = tmp_path / "mock.log"
-    if log.exists():
-        log.unlink()
-    env = dict(os.environ, LD_LIBRARY_PATH=f"{mock_dir}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=str(log))
-    env.update(env_extra or {})
-    res = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "mock_cuda", "ragged_qsort_child.py"),
-                          json.dumps({"ops": ops})], capture_output=True, text=True, env=env, timeout=300)
-    assert res.returncode == 0, res.stdout + res.stderr
-    events = [json.loads(ln) for ln in open(log)] if log.exists() else []
-    assert not [e for e in events if e["op"] == "error"], [e for e in events if e["op"] == "error"]
-    assert events[-1] == {"op": "exit", "live_allocations": 0}
-    return json.loads(res.stdout.strip().splitlines()[-1]), events
+QSORT_THREADS = 128
 
 
 def offsets(elems, first=12):
@@ -54,7 +32,7 @@ def test_ragged_qsort_launch_runs_the_prepass_then_the_var_kernel_in_one_scratch
               unit_base=1 << 32, flags=3)
     if p:
         op["p"] = p
-    res, ev = run(mock_dir, tmp_path, [op])
+    res, ev, _ = run(mock_dir, tmp_path, [op], "ragged_qsort_child.py")
     r = res["ops"][0]
     assert r["rc"] == 0, r["err"]
     launches = [e for e in ev if e["op"] == "launch" and e["name"] != "xmr_counters_reset"]
@@ -86,23 +64,23 @@ def test_bad_ragged_qsort_arguments_fail_loudly(mock_dir, tmp_path, case):
     op = dict(op="launch", offsets=offsets([3, 4, 5]), unit_bytes=64)
     op.update({"bound_zero": dict(unit_bytes=0), "bound_odd": dict(unit_bytes=62), "bound_big": dict(unit_bytes=4100),
                "in_misaligned": dict(in_misalign=2), "out_misaligned": dict(out_misalign=1)}[case])
-    res, ev = run(mock_dir, tmp_path, [op])
+    res, ev, _ = run(mock_dir, tmp_path, [op], "ragged_qsort_child.py")
     r = res["ops"][0]
     assert r["rc"] == BAD_ARG and "COAST_UNIT_OFFSETS" in r["err"], r
     assert not [e for e in ev if e["op"] == "launch" and e["name"] != "xmr_counters_reset"]
 
 
 def test_the_bounds_themselves_are_accepted_and_aes_still_refused(mock_dir, tmp_path):
-    res, _ = run(mock_dir, tmp_path, [dict(op="launch", offsets=offsets([1024, 0, 7]), unit_bytes=4096),
-                                      dict(op="launch", offsets=offsets([1, 0, 1]), unit_bytes=4),
-                                      dict(op="launch", kernel=2, offsets=offsets([4, 4]), unit_bytes=64)])
+    res, _, _ = run(mock_dir, tmp_path, [dict(op="launch", offsets=offsets([1024, 0, 7]), unit_bytes=4096),
+                                         dict(op="launch", offsets=offsets([1, 0, 1]), unit_bytes=4),
+                                         dict(op="launch", kernel=2, offsets=offsets([4, 4]), unit_bytes=64)], "ragged_qsort_child.py")
     assert [r["rc"] for r in res["ops"]] == [0, 0, BAD_ARG]
     assert "COAST_UNIT_OFFSETS" in res["ops"][2]["err"]
 
 
 def test_nested_scheduling_of_a_ragged_batch_is_unsupported(mock_dir, tmp_path):
     op = dict(op="launch", offsets=offsets([3, 4, 5]), unit_bytes=64)
-    res, ev = run(mock_dir, tmp_path, [op], env_extra={"COAST_QSORT_PATH": "nested"})
+    res, ev, _ = run(mock_dir, tmp_path, [op], "ragged_qsort_child.py", env_extra={"COAST_QSORT_PATH": "nested"})
     r = res["ops"][0]
     assert r["rc"] == UNSUPPORTED and "COAST_QSORT_PATH=nested" in r["err"], r
     assert not [e for e in ev if e["op"] == "launch" and "qsort" in e["name"]]
@@ -110,7 +88,7 @@ def test_nested_scheduling_of_a_ragged_batch_is_unsupported(mock_dir, tmp_path):
 
 @pytest.mark.parametrize("offs", [[0, 12, 8, 20], [0, 12, 400, 404], [0, 12, 18, 24]])
 def test_bad_host_offsets_fail_before_any_copy(mock_dir, tmp_path, offs):
-    res, ev = run(mock_dir, tmp_path, [dict(op="run_host", offsets=offs, unit_bytes=64)])
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", offsets=offs, unit_bytes=64)], "ragged_qsort_child.py")
     r = res["ops"][0]
     assert r["rc"] == BAD_ARG and "COAST_UNIT_OFFSETS" in r["err"], r
     assert not [e for e in ev if e["op"] in ("h2d", "launch") and e.get("name", "") != "xmr_counters_reset"]
@@ -124,8 +102,8 @@ def test_host_chunks_upload_and_download_the_same_spans_with_both_pointers_biase
     off = offsets(elems, first=20)
     n = len(elems)
     budget = 40000
-    res, ev = run(mock_dir, tmp_path, [dict(op="run_host", offsets=off, unit_bytes=4096, pinned=pinned, unit_base=1000)],
-                  env_extra={"COAST_HOST_CHUNK_BYTES": str(budget)})
+    res, ev, _ = run(mock_dir, tmp_path, [dict(op="run_host", offsets=off, unit_bytes=4096, pinned=pinned, unit_base=1000)], "ragged_qsort_child.py",
+                     env_extra={"COAST_HOST_CHUNK_BYTES": str(budget)})
     r = res["ops"][0]
     assert r["rc"] == 0 and r["path"] == "staged", r
     h2d = [e for e in ev if e["op"] == "h2d" and r["host_in"] <= e["host"] < r["host_in"] + off[-1] + 16]
@@ -155,7 +133,7 @@ def test_host_chunks_upload_and_download_the_same_spans_with_both_pointers_biase
 
 @pytest.mark.parametrize("path", ["zerocopy", "hybrid"])
 def test_forced_zero_copy_or_hybrid_ragged_qsort_host_calls_are_unsupported(mock_dir, tmp_path, path):
-    res, _ = run(mock_dir, tmp_path, [dict(op="run_host", offsets=offsets([3, 9, 0]), unit_bytes=64, pinned=True)],
-                 env_extra={"COAST_HOST_PATH": path})
+    res, _, _ = run(mock_dir, tmp_path, [dict(op="run_host", offsets=offsets([3, 9, 0]), unit_bytes=64, pinned=True)], "ragged_qsort_child.py",
+                   env_extra={"COAST_HOST_PATH": path})
     r = res["ops"][0]
     assert r["rc"] == UNSUPPORTED and "staged only" in r["err"]

@@ -6,7 +6,7 @@ so that two builds of libcoast_rt.so can be compared with diff:
 The sweep is tests/test_mm_plan_sweep.py's, plus refusals (zero dimensions, n_units off the shape, the 2^31 row bounds,
 misaligned or null buffers and row offsets, too many groups, combined mode bits, store votes) and host calls (pageable and
 pinned buffers, several chunks, COAST_HOST_PATH=one-shot).  It runs <checkout>/coast_b200/libcoast_rt.so against this tree's
-mock driver (tests/mock_cuda/mock_cuda_bt.c), one op per init, with a marker in the log between ops.  Pointers are made
+mock driver (tests/mock_cuda/mock_cuda.c) through tests/mock_cuda/mm_child.py, one op per init, with a marker in the log between ops.  Pointers are made
 comparable across processes: an 8-byte word of an argument block, a tensor-map base or a copy's device side that points into
 a live allocation becomes a<id>+<offset>, a host-call chunk's biased d_in / d_out an offset from the slot buffer it is copied
 through, and a pageable host address an offset into the op's buffers.  After each op its rc, error text and coast_last_host_path()."""
@@ -22,10 +22,10 @@ import tempfile
 HERE = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(HERE, "tests"))
 import test_mm_plan_sweep as S  # noqa: E402
+from mock_run import (KNOBS, K_CRC16, K_GEMM_BF16, K_GEMM_FP8, K_GEMM_TF32, K_MM_U32, K_SHA256, MM_B_TRANSPOSED as BT,  # noqa: E402
+                      MM_BATCHED as BATCHED, MM_GROUPED as GROUPED, UNIT_OFFSETS)
 
-K_CRC16, K_SHA256 = 0, 1
-BATCHED, GROUPED, BT, UNIT_OFFSETS = 0x20000, 0x40000, 0x80000, 0x10000
-MM = (S.K_MM_U32, S.K_GEMM_TF32, S.K_GEMM_BF16)
+MM = (K_MM_U32, K_GEMM_TF32, K_GEMM_BF16, K_GEMM_FP8)
 
 
 def edge_ops():
@@ -73,16 +73,16 @@ def edge_ops():
 def child(root, ops):
     """runs each op as its own init .. shutdown of root's library, a marker line in the mock's log before it"""
     sys.path.insert(0, os.path.join(HERE, "tests", "mock_cuda"))
-    import mm_bt_child
-    mm_bt_child.R.lib_path = lambda: os.path.join(root, "coast_b200", "libcoast_rt.so")
+    import mm_child
+    mm_child.R.lib_path = lambda: os.path.join(root, "coast_b200", "libcoast_rt.so")
     results = []
     for i, op in enumerate(ops):
         with open(os.environ["MOCK_CUDA_LOG"], "a") as f:
             f.write(json.dumps({"op": "begin", "index": i}) + "\n")
-        sys.argv = ["mm_bt_child.py", json.dumps({"ops": [op]})]
+        sys.argv = ["mm_child.py", json.dumps({"ops": [op]})]
         buf = io.StringIO()
         with contextlib.redirect_stdout(buf):
-            mm_bt_child.main()
+            mm_child.main()
         results.append(json.loads(buf.getvalue().strip().splitlines()[-1])["ops"][0])
     print(json.dumps(results))
 
@@ -140,8 +140,8 @@ def normalise(events, results):
             lines.append(f"launch {e['name']} grid={e['grid']} block={e['block']} smem={e['smem']} stream={e['stream']} " + " ".join(words))
         elif kind in ("h2d", "d2h"):
             lines.append(f"{kind} a{e['alloc']}+{e['offset']} {e['bytes']} {host(e['host'])} stream={e['stream']}")
-        elif kind == "tmap_at":
-            lines.append(f"tmap_at {dev(e['addr'])}")
+        elif kind == "tmap":
+            lines.append(json.dumps(dict(e, addr=dev(e["addr"])), sort_keys=True))
         else:
             lines.append(json.dumps(e, sort_keys=True))
     if op >= 0:
@@ -160,13 +160,13 @@ def main():
     n_ops = n_events = 0
     with tempfile.TemporaryDirectory() as tmp:
         subprocess.run(["gcc", "-O1", "-shared", "-fPIC", "-Wall", "-I/usr/local/cuda/include", "-o", os.path.join(tmp, "libcuda.so.1"),
-                        os.path.join(HERE, "tests", "mock_cuda", "mock_cuda_bt.c")], check=True)
+                        os.path.join(HERE, "tests", "mock_cuda", "mock_cuda.c")], check=True)
         log = os.path.join(tmp, "mock.log")
         for env_extra, ops in S.SWEEP + edge_ops():
             if os.path.exists(log):
                 os.unlink(log)
             env = dict(os.environ, LD_LIBRARY_PATH=f"{tmp}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=log)
-            for k in S.KNOBS:
+            for k in KNOBS:
                 env.pop(k, None)
             env.update(env_extra)
             res = subprocess.run([sys.executable, os.path.abspath(__file__), "--root", root, "--child", json.dumps(ops)],
