@@ -106,7 +106,7 @@ _Static_assert(sizeof(map_desc) == 80, "map_desc has no padding");
 
 /* coast_run_host staging: a device buffer and its capacity; a slot is one host-call stream and the buffers its chunks use */
 typedef struct { CUdeviceptr p; size_t cap; } dev_buf;
-typedef struct { CUstream s; dev_buf in, out, aux, stat, rows; } host_slot;
+typedef struct { CUstream s; dev_buf in, out, aux, stat, rows, sc; } host_slot;   /* sc: a chunk's scales, A's then B's */
 
 #define MAX_FN 128
 static struct {
@@ -126,7 +126,7 @@ static struct {
     /* protection mode of the four reference entry points (coast_set_opt_passes / COAST_OPT_PASSES) */
     uint32_t def_nc, def_flags; int def_set;
     host_slot slot[3];               /* coast_run_host: chunk i runs on slot i % 3 */
-    dev_buf h_b; CUevent ev_b;       /* matmul host call: the replicated operand B and "B has landed" */
+    dev_buf h_b; CUevent ev_b;       /* matmul host call: the replicated operand B (and the scales every chunk shares) and "B has landed" */
     /* stream-ordered scratch (the replicas' private arrays of xmr_qsort.cuh): any number of streams may launch at once */
     CUmemoryPool pool;
     int numa_node;                   /* NUMA node the process was bound to by coast_init (-1: not bound) */
@@ -331,9 +331,9 @@ int coast_init(int device) { ENTER(); LEAVE(init_impl(device)); }
 static int shutdown_impl(void) {
     if (!G.inited) return COAST_OK;
     ensure_ctx();
-    dev_buf* bufs[] = { &G.h_b, &G.slot[0].in, &G.slot[0].out, &G.slot[0].aux, &G.slot[0].stat, &G.slot[0].rows, &G.slot[1].in,
-                        &G.slot[1].out, &G.slot[1].aux, &G.slot[1].stat, &G.slot[1].rows, &G.slot[2].in, &G.slot[2].out,
-                        &G.slot[2].aux, &G.slot[2].stat, &G.slot[2].rows };
+    dev_buf* bufs[] = { &G.h_b, &G.slot[0].in, &G.slot[0].out, &G.slot[0].aux, &G.slot[0].stat, &G.slot[0].rows, &G.slot[0].sc,
+                        &G.slot[1].in, &G.slot[1].out, &G.slot[1].aux, &G.slot[1].stat, &G.slot[1].rows, &G.slot[1].sc,
+                        &G.slot[2].in, &G.slot[2].out, &G.slot[2].aux, &G.slot[2].stat, &G.slot[2].rows, &G.slot[2].sc };
     for (size_t i = 0; i < sizeof bufs / sizeof bufs[0]; ++i) if (bufs[i]->p) p_cuMemFree_v2(bufs[i]->p);
     for (int i = 0; i < 3; ++i) if (G.slot[i].s) p_cuStreamDestroy_v2(G.slot[i].s);
     if (G.ev_b) p_cuEventDestroy_v2(G.ev_b);
@@ -512,6 +512,7 @@ typedef struct {
     int b_rows_k;                 /* B's map has K rows per product (GEMM_BF16 reading B in place); every B^T map has N (GEMM_FP8's
                                      always: a B^T map over the pre-pass's scratch or the caller's B^T) */
     uint32_t b_rows;              /* rows per product of B's map */
+    int scaled, rowwise;          /* GEMM_FP8 with COAST_MM_SCALE_TENSOR or COAST_MM_SCALE_ROWWISE; the latter */
 } mm_shape;
 
 /* What kernel selection decides about a launch; run_plan() does the rest. */
@@ -572,15 +573,35 @@ static int mm_bit_refused(const coast_launch_desc* d, uint32_t bit) {
                      : bit == COAST_MM_GROUPED ? "COAST_MM_GROUPED: grouped products exist" : "COAST_MM_B_TRANSPOSED: a transposed B exists";
     return fail(COAST_ERR_BAD_ARG, "%s for MM_U32, GEMM_TF32 and GEMM_BF16 only, plus GEMM_FP8 (kernel %u)", what, d->kernel);
 }
-/* The checks shared by coast_launch and coast_run_host: a matmul mode bit on another kernel, then the shape of a batch or of
- * groups.  Fills *m for the matmul kernels. */
+/* The scale bits (GEMM_FP8 only): one of the two, both scale pointers, d_scale_a 4-byte aligned and, row-wise, d_scale_b
+ * 8-byte aligned (the kernels read a thread's two column scales as one float2) */
+static int mm_scale_check(const coast_launch_desc* d) {
+    const uint32_t bits = d->mode & (COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE);
+    if (!bits) return COAST_OK;
+    const char* what = bits == COAST_MM_SCALE_TENSOR ? "COAST_MM_SCALE_TENSOR" : "COAST_MM_SCALE_ROWWISE";
+    if (d->kernel != COAST_K_GEMM_FP8)
+        return fail(COAST_ERR_BAD_ARG, "%s: scaled products exist for GEMM_FP8 only (kernel %u)",
+                    bits == (COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE) ? "COAST_MM_SCALE_TENSOR / COAST_MM_SCALE_ROWWISE" : what, d->kernel);
+    if (bits == (COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_SCALE_TENSOR and COAST_MM_SCALE_ROWWISE cannot be combined: one scale layout per launch");
+    if (!d->d_scale_a || !d->d_scale_b)
+        return fail(COAST_ERR_BAD_ARG, "%s: d_scale_a and d_scale_b must point to the scales of A and B", what);
+    if (((uintptr_t)d->d_scale_a) & 3u) return fail(COAST_ERR_BAD_ARG, "%s: d_scale_a must be 4-byte aligned", what);
+    if (bits == COAST_MM_SCALE_ROWWISE && (((uintptr_t)d->d_scale_b) & 7u))
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_SCALE_ROWWISE: d_scale_b must be 8-byte aligned (column scales are read in pairs)");
+    return COAST_OK;
+}
+/* The checks shared by coast_launch and coast_run_host: a matmul mode bit on another kernel, the scale bits, then the shape of
+ * a batch or of groups.  Fills *m for the matmul kernels. */
 static int mm_check(const coast_launch_desc* d, mm_shape* m) {
     int rc;
     memset(m, 0, sizeof *m);
     if ((rc = mm_bit_refused(d, COAST_MM_BATCHED)) || (rc = mm_bit_refused(d, COAST_MM_GROUPED)) ||
-        (rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)))
+        (rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)) || (rc = mm_scale_check(d)))
         return rc;
     if (!is_matmul(d->kernel)) return COAST_OK;
+    m->scaled = (d->mode & (COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE)) != 0;
+    m->rowwise = (d->mode & COAST_MM_SCALE_ROWWISE) != 0;
     m->es = KINFO[d->kernel].mm_elem;
     m->batched = (d->mode & COAST_MM_BATCHED) != 0;
     m->grouped = (d->mode & COAST_MM_GROUPED) != 0;
@@ -623,8 +644,15 @@ static uint64_t mm_row_tiles(const mm_shape* m, unsigned bm) { return m->rows / 
 
 /* A matmul kernel's name: stem, path variant, [_bt], [_grp], then _nc<n>_inj<i> for the kernels that came before batched,
  * grouped, BF16 and transposed-B launches and _inj<i>_nc<n> for the others.  GEMM_FP8's names are whole formats: one set of
- * kernels serves B and B^T, the narrow kernel exists at NC 1 only, and the grouped ones (always 128 x 128 tiles) carry no variant. */
-static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, uint32_t nc, int inj) {
+ * kernels serves B and B^T, the narrow kernel exists at NC 1 only, and the grouped ones (always 128 x 128 tiles) carry no variant;
+ * scaled GEMM_FP8 (xmr_scaled_fp8*) has the same set. */
+static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, int scaled, uint32_t nc, int inj) {
+    if (kernel == COAST_K_GEMM_FP8 && scaled) {
+        const char* f = grouped ? "xmr_scaled_fp8_grp_inj%d_nc%u" : *variant == 'p' ? "xmr_scaled_fp8p_inj%d_nc%u"
+                      : *variant == 'n' ? "xmr_scaled_fp8n_inj%d_nc1" : "xmr_scaled_fp8_inj%d_nc%u";
+        snprintf(name, 64, f, inj, nc);
+        return;
+    }
     if (kernel == COAST_K_GEMM_FP8) {
         const char* f = grouped ? "xmr_gemm_fp8_grp_inj%d_nc%u" : *variant == 'p' ? "xmr_gemm_fp8p_inj%d_nc%u"
                       : *variant == 'n' ? "xmr_gemm_fp8n_inj%d_nc1" : "xmr_gemm_fp8_inj%d_nc%u";
@@ -733,16 +761,18 @@ static int run_plan(const launch_plan* L, const coast_launch_desc* d, xmr_args* 
     CUtensorMap maps[2];
     rc = L->prepass ? L->prepass(L, d, scratch, stream) : COAST_OK;
     for (int i = 0; i < L->n_maps && !rc; ++i) rc = encode_map(&L->map[i], scratch, L->cache_maps, &maps[i]);
-    /* grouped: the tile table (and the GEMMs' rebased A map) after the other pre-passes; the kernel takes ro and the group block */
-    const void* ro = d->d_rows;
+    /* grouped: the tile table (and the GEMMs' rebased A map) after the other pre-passes; the kernel takes ro and the group block,
+     * then a scaled kernel the scales */
+    const void* ro = d->d_rows; const void* sa = d->d_scale_a; const void* sb = d->d_scale_b;
     CUdeviceptr grp = scratch + L->grp_off;
     if (!rc && L->mm.grouped && L->grp_tm)
         rc = prepass_group_scan(L, d, grp, d->kernel != COAST_K_MM_U32 ? &maps[0] : NULL, stream);
     if (!rc) {
-        void* params[5] = { a };
+        void* params[7] = { a };
         int n_params = 1;
         for (int i = 0; i < L->n_maps; ++i) params[n_params++] = &maps[i];
         if (L->mm.grouped) { params[n_params++] = &ro; params[n_params++] = &grp; }
+        if (L->mm.scaled) { params[n_params++] = &sa; params[n_params++] = &sb; }
         if (d->flags & COAST_F_VERBOSE)
             fprintf(stderr, "coast_rt: %s grid=%u block=%u smem=%u units=%llu\n", L->name, grid, L->block, L->smem,
                     (unsigned long long)d->n_units);
@@ -775,7 +805,9 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     a.status = (unsigned char*)d->d_status;
     /* the kernels find a batch from n_units / N (rows of the stacked problem) and a.M (rows per product): a batch of one is
      * an unbatched launch, argument block included */
-    a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~(COAST_MM_BATCHED | COAST_MM_GROUPED | COAST_MM_B_TRANSPOSED);
+    a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~(COAST_MM_BATCHED | COAST_MM_GROUPED | COAST_MM_B_TRANSPOSED |
+                                                                      COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE);
+    if (m.rowwise) a.mode |= XMR_MODE_SCALE_ROWWISE;
     a.M = d->M; a.N = d->N; a.K = d->K;
     memcpy(a.key, d->key, 16);
     if (inj) {
@@ -893,7 +925,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
             L.ctas = mm_row_tiles(&m, XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;   /* grouped: surplus CTAs exit */
             L.grp_tm = XMR_MMT_BM; L.grp_tiles_n = d->N / XMR_MMT_BN;
         }
-        mm_kernel_name(L.name, d->kernel, variant, bt_name, m.grouped, nc, inj);
+        mm_kernel_name(L.name, d->kernel, variant, bt_name, m.grouped, 0, nc, inj);
         break;
     }
     case COAST_K_QSORT:
@@ -958,7 +990,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
         const int pair = !m.grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
         /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it, TF32 and FP8 only skip the transposing pre-pass */
-        mm_kernel_name(L.name, d->kernel, pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt, m.grouped, nc, inj);
+        mm_kernel_name(L.name, d->kernel, pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt, m.grouped, m.scaled, nc, inj);
         { const char* g = getenv("COAST_GEMM_GROUP_M");
           if (g && atoi(g) > 0 && atoi(g) <= (int)XMR_MODE_GROUP_M_MASK) a.mode = (a.mode & ~XMR_MODE_GROUP_M_MASK) | (unsigned)atoi(g); }
         /* L2 eviction priorities: A evict_last, B and C evict_first; COAST_GEMM_L2_HINTS=0 loads and stores with the normal policy */
@@ -1178,9 +1210,11 @@ typedef struct { uint64_t off, len; } byte_range;           /* bytes [off, off +
 typedef struct {
     uint64_t items;                                          /* items the chunk takes */
     byte_range in, aux, out, stat, rows;                     /* of d_in, d_aux, d_out, d_status and d_rows */
+    byte_range sa, sb;                                       /* of d_scale_a and d_scale_b (row-wise scales) */
     uint64_t n_units, unit_base;                             /* of the chunk's launch; unit_base is added to the call's */
     uint32_t M;                                              /* rows of a matmul row block (0: the call's M) */
     uint64_t in_bias, out_bias;                              /* the launch's d_in / d_out are the slot's buffers minus these */
+    uint64_t sa_bias;                                        /* ... and its d_scale_a (groups: biased like d_in) */
 } host_chunk;
 
 typedef struct host_sched host_sched;
@@ -1193,6 +1227,8 @@ struct host_sched {
     uint64_t min_items, max_items, max_bytes;                /* chunk bounds */
     uint64_t min_in;                                         /* least input slot: an empty input still launches on an address */
     uint64_t shared_b;                                       /* bytes of the matmul's B: uploaded once, every chunk waits for it */
+    uint64_t sab, sbb;                                       /* scaled matmuls, per item: bytes of row-wise A and B scales */
+    uint64_t shared_sa, shared_sb;                           /* bytes of A and B scales uploaded once with B (tensorwise: 4 and 4) */
     CUdeviceptr zin;                                         /* hybrid: the input's mapped alias, which the kernels read in place */
     int qs, aux_back;                                        /* ragged quicksort (output in place of the input); AES key write-back */
     const char* path;                                        /* what coast_last_host_path() reports */
@@ -1206,6 +1242,8 @@ static void item_chunk(const host_sched* s, uint64_t first, uint64_t n, host_chu
     c->aux = (byte_range){ first * s->ab, n * s->ab };
     c->out = (byte_range){ first * s->ob, n * s->ob };
     c->stat = (byte_range){ c->unit_base, c->n_units };     /* one status byte per unit */
+    c->sa = (byte_range){ first * s->sab, n * s->sab };
+    c->sb = (byte_range){ first * s->sbb, n * s->sbb };
 }
 
 /* Uniform units.  Large chunks amortise the driver work of each chunk, but a fixed size leaves the copy engines idle while the
@@ -1268,6 +1306,8 @@ static void next_groups(const host_sched* s, uint64_t first, uint64_t* budget, h
     c->aux = (byte_range){ first * s->ab, (e - first) * s->ab };
     c->out = (byte_range){ ro[first] * s->ob, rows * s->ob }; c->out_bias = ro[first] * s->ob;
     c->rows = (byte_range){ first * 8u, (e - first + 1) * 8u };
+    c->sa = (byte_range){ ro[first] * s->sab, rows * s->sab }; c->sa_bias = ro[first] * s->sab;
+    c->sb = (byte_range){ first * s->sbb, (e - first) * s->sbb };
 }
 
 /* Matmul row blocks: max_items rows of A up and of C down per chunk; B is the schedule's shared operand. */
@@ -1277,19 +1317,20 @@ static void next_row_block(const host_sched* s, uint64_t done, uint64_t* budget,
 }
 
 static void grow(uint64_t* need, uint64_t len) { if (len > *need) *need = len; }
+static uint64_t align16(uint64_t x) { return (x + 15u) & ~(uint64_t)15u; }
 
 /* Runs a call's chunks.  The schedule is walked twice: once to size each slot for the largest chunk it gets -- every slot is
  * reserved before the first copy, so a failed allocation never leaves a partly written output -- and once to run. */
 static int run_chunks(const host_sched* s, coast_stats* out, int* dwc_fired) {
     const coast_launch_desc* d = s->d;
-    struct { uint64_t in, aux, out, stat, rows; } need[3];
+    struct { uint64_t in, aux, out, stat, rows, sc; } need[3];
     memset(need, 0, sizeof need);
     uint64_t n_chunks = 0;
     for (uint64_t done = 0, budget = s->budget; done < s->total; ++n_chunks) {
         host_chunk c; s->next(s, done, &budget, &c);
         const int i = (int)(n_chunks % 3);
         grow(&need[i].in, c.in.len); grow(&need[i].aux, c.aux.len); grow(&need[i].out, c.out.len); grow(&need[i].stat, c.stat.len);
-        grow(&need[i].rows, c.rows.len);
+        grow(&need[i].rows, c.rows.len); grow(&need[i].sc, align16(c.sa.len) + c.sb.len);
         done += c.items;
     }
     int rc;
@@ -1301,9 +1342,13 @@ static int run_chunks(const host_sched* s, coast_stats* out, int* dwc_fired) {
         if ((rc = slot_reserve(&sl->aux.p, &sl->aux.cap, need[i].aux))) return rc;
         if (d->d_status && (rc = slot_reserve(&sl->stat.p, &sl->stat.cap, need[i].stat))) return rc;
         if (need[i].rows && (rc = slot_reserve(&sl->rows.p, &sl->rows.cap, need[i].rows))) return rc;
+        if (need[i].sc && (rc = slot_reserve(&sl->sc.p, &sl->sc.cap, need[i].sc))) return rc;
     }
-    if (s->shared_b) {
-        if ((rc = slot_reserve(&G.h_b.p, &G.h_b.cap, s->shared_b))) return rc;
+    /* what every chunk shares goes up once: [B][A's scales][B's scales], each part 16-byte aligned */
+    const uint64_t sa_at = align16(s->shared_b), sb_at = sa_at + align16(s->shared_sa);
+    const int shared = s->shared_b || s->shared_sa || s->shared_sb;
+    if (shared) {
+        if ((rc = slot_reserve(&G.h_b.p, &G.h_b.cap, s->shared_sa || s->shared_sb ? sb_at + s->shared_sb : s->shared_b))) return rc;
         if (!G.ev_b) DRV(p_cuEventCreate(&G.ev_b, CU_EVENT_DISABLE_TIMING));
     }
 #define STEP(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) { rc = drv_fail(r_, #call); goto fail; } } while (0)
@@ -1326,13 +1371,24 @@ static int run_chunks(const host_sched* s, coast_stats* out, int* dwc_fired) {
             STEP(p_cuMemcpyHtoDAsync_v2(sl->rows.p, (const uint8_t*)d->d_rows + k.rows.off, (size_t)k.rows.len, sl->s));
             c.d_rows = (const void*)sl->rows.p;
         }
-        if (s->shared_b) {                                   /* B follows the first chunk's input, on stream 1 */
+        if (k.sa.len || k.sb.len) {                          /* row-wise scales of the chunk's rows and products */
+            const CUdeviceptr sbp = sl->sc.p + align16(k.sa.len);
+            if (k.sa.len) STEP(p_cuMemcpyHtoDAsync_v2(sl->sc.p, (const uint8_t*)d->d_scale_a + k.sa.off, (size_t)k.sa.len, sl->s));
+            if (k.sb.len) STEP(p_cuMemcpyHtoDAsync_v2(sbp, (const uint8_t*)d->d_scale_b + k.sb.off, (size_t)k.sb.len, sl->s));
+            if (k.sa.len) c.d_scale_a = (const void*)(uintptr_t)(sl->sc.p - k.sa_bias);
+            if (k.sb.len) c.d_scale_b = (const void*)(uintptr_t)sbp;
+        }
+        if (shared) {                                        /* B (and shared scales) follow the first chunk's input, on stream 1 */
             if (i == 0) {
-                STEP(p_cuMemcpyHtoDAsync_v2(G.h_b.p, d->d_aux, (size_t)s->shared_b, G.slot[1].s));
+                if (s->shared_b) STEP(p_cuMemcpyHtoDAsync_v2(G.h_b.p, d->d_aux, (size_t)s->shared_b, G.slot[1].s));
+                if (s->shared_sa) STEP(p_cuMemcpyHtoDAsync_v2(G.h_b.p + sa_at, d->d_scale_a, (size_t)s->shared_sa, G.slot[1].s));
+                if (s->shared_sb) STEP(p_cuMemcpyHtoDAsync_v2(G.h_b.p + sb_at, d->d_scale_b, (size_t)s->shared_sb, G.slot[1].s));
                 STEP(p_cuEventRecord(G.ev_b, G.slot[1].s));
             }
             STEP(p_cuStreamWaitEvent(sl->s, G.ev_b, 0));
-            c.d_aux = (const void*)G.h_b.p;
+            if (s->shared_b) c.d_aux = (const void*)G.h_b.p;
+            if (s->shared_sa) c.d_scale_a = (const void*)(uintptr_t)(G.h_b.p + sa_at);
+            if (s->shared_sb) c.d_scale_b = (const void*)(uintptr_t)(G.h_b.p + sb_at);
         }
         c.d_out = (void*)(uintptr_t)(sl->out.p - k.out_bias);
         if (d->d_status) c.d_status = (void*)sl->stat.p;    /* kernels index status[] chunk-locally */
@@ -1365,7 +1421,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
     { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) chunk_bytes = (uint64_t)atoll(e); }
     host_sched s; memset(&s, 0, sizeof s);
     s.d = d; s.upi = 1; s.path = "staged";
-    if ((rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED))) return rc;
+    if ((rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)) || (rc = mm_scale_check(d))) return rc;
 
     if (d->mode & COAST_UNIT_OFFSETS) {                      /* ragged: staged only */
         if ((rc = ragged_check(d))) return rc;
@@ -1422,6 +1478,14 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
             s.next = next_row_block; s.total = d->M; s.upi = d->N; s.ib = a_row; s.ob = c_row;
             s.max_items = rows; s.shared_b = bb;
             s.path = rows < d->M ? "row-blocks" : "one-shot";
+        }
+        /* scales: tensorwise, the two floats go up once; row-wise, each chunk takes the A scales of its rows and the B scales of its
+         * products, except that row blocks share B and so share its scales.  The chunks are those of the unscaled call. */
+        if (m.scaled && !m.rowwise) { s.shared_sa = 4; s.shared_sb = 4; }
+        if (m.rowwise) {
+            s.sab = 4u * (m.batched ? d->M : 1u);
+            if (m.grouped || m.batched) s.sbb = 4ull * d->N;
+            else s.shared_sb = 4ull * d->N;
         }
         return run_chunks(&s, out, dwc_fired);
     }

@@ -35,6 +35,9 @@ typedef struct xmr_args {
 #define XMR_MODE_GROUP_M_MASK  0xFFu
 #define XMR_MODE_L2_HINTS      0x100u
 #define XMR_MODE_NO_TAIL_SPLIT 0x200u
+/* scaled FP8 GEMM (xmr_scaled_fp8*; the host sets it for COAST_MM_SCALE_ROWWISE): one A scale per row and one B scale per
+ * column of each product, instead of one of each */
+#define XMR_MODE_SCALE_ROWWISE 0x400u
 
 /* counter slots (mirror coast_stats) */
 #define XMR_CTR_ERRORS   0

@@ -228,18 +228,38 @@ __device__ __forceinline__ void wgmma_u8_m64n64k32(uint32_t (&d)[32], uint64_t d
 // Epilogue of one consumer thread: vote the NC accumulators of its fragment element by element with the reference's select
 // voter / `fcmp oeq`, count, ONE store of the voted value.  Columns [n0 + 128 sub, ...) for sub < nsub_t.
 // GROUPED: C starts at row ro[0] (c_grp) and rows from row_end on belong to the next product: no vote, tally, flip or store.
-template <int NC, int NSUB, bool INJECT, bool GROUPED = false>
+// SCALED (xmr_scaled_fp8*): each replica's value, after the fault hook, becomes (acc x sa) x sb, two fp32 multiplies rounded to
+// nearest, and the vote is on those.  sa: the A scale of row `row` is sa[row] (ROWWISE) or sa[0]; sb: the B scale of column
+// `col` is sb[col] or sb[0] (the caller offsets both to the tile's product).  The two layouts are two instances, so neither
+// carries the other's loads and branches next to the accumulators.  Every replica reads the one copy
+// of a scale (-noMemReplication's load rule), after the main loop, so nothing of it is live next to the accumulators.
+template <int NC, int NSUB, bool INJECT, bool GROUPED = false, bool SCALED = false, bool ROWWISE = false>
 __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float (&acc)[NC][NSUB][64], uint32_t row0, uint32_t n0, uint32_t nsub_t,
-                                         bool hints, uint64_t pol_c, float* c_grp = nullptr, uint32_t row_end = 0) {
+                                         bool hints, uint64_t pol_c, float* c_grp = nullptr, uint32_t row_end = 0,
+                                         const float* sa = nullptr, const float* sb = nullptr) {
     const uint32_t flags = a.flags;
     const bool majority = flags & COAST_F_MAJORITY_VOTER;
     float* C = GROUPED ? c_grp : static_cast<float*>(a.out);
     const uint32_t lane = threadIdx.x & 31;
+    constexpr bool rowwise = SCALED && ROWWISE;
+    float s_row[2] = {1.f, 1.f}, s_col = 1.f;
+    if constexpr (SCALED) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {                       // a masked row of a grouped tile loads nothing
+            const uint32_t row = row0 + 8 * h;
+            if (!GROUPED || row < row_end) s_row[h] = __ldg(sa + (rowwise ? row : 0u));
+        }
+        if (!rowwise) s_col = __ldg(sb);
+    }
 #pragma unroll
     for (int sub = 0; sub < NSUB; ++sub) {
         if ((uint32_t)sub >= nsub_t) break;
 #pragma unroll
         for (int j = 0; j < WG_N / 8; ++j) {
+            float2 s_pair = make_float2(s_col, s_col);       // the B scales of this thread's two columns (an even first column)
+            if constexpr (SCALED) {
+                if constexpr (rowwise) s_pair = __ldg(reinterpret_cast<const float2*>(sb + n0 + sub * WG_N + 8 * j + 2 * (lane & 3)));
+            }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const uint32_t row = row0 + 8 * h, col = n0 + sub * WG_N + 8 * j + 2 * (lane & 3);
@@ -259,6 +279,12 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float 
                             uint32_t mk = 1u << f.bit;
                             if (f.replica == 0) r0 ^= mk; else if (f.replica == 1) r1 ^= mk; else r2 ^= mk;
                         }
+                    }
+                    if constexpr (SCALED) {                      // every replica scales its own value; explicit _rn: no contraction
+                        const float sr = s_row[h], sc = e ? s_pair.y : s_pair.x;
+                        r0 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r0), sr), sc));
+                        if (NC > 1) r1 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r1), sr), sc));
+                        if (NC > 2) r2 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r2), sr), sc));
                     }
                     const float f0 = __uint_as_float(r0), f1 = __uint_as_float(r1), f2 = __uint_as_float(r2);
                     uint32_t vote = r0, bad = 0;
@@ -283,9 +309,11 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float 
 // of the tile's B^T rows and multicasts them to both, so a stage is released only when the consumers of BOTH CTAs are done with it.
 // GROUPED (single CTAs with 128 x 128 tiles, xmr_mm_grp.cuh): a.M products of their own row counts, `ro` their row offsets and
 // `grp` the group block: the tiles come from its tile_start table, A through its rebased map, B^T rows from g N (Bf16: B rows from g K).
-template <class OP, int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false>
+// SCALED (xmr_scaled_fp8*): sa and sb are the caller's scales (see epilogue); a row-wise B scale vector holds N entries per product.
+template <class OP, int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false, bool SCALED = false>
 __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b,
-                                          const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr) {
+                                          const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr,
+                                          const float* sa = nullptr, const float* sb = nullptr) {
     static_assert(!(GROUPED && (PAIR || WIDE)), "grouped launches run on single CTAs with 128 x 128 tiles");
     using G = Geom<NC, WIDE>;
     constexpr int BN = G::BN, NSUB = G::NSUB, STAGES = G::STAGES;
@@ -436,10 +464,28 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
                 const unsigned long long r0 = __ldg(ro);
                 const grp::Tile x = grp::tile_of(ro, r0, R, ts, n_grp, tiles_n, group_m, tile);
                 const uint32_t row0 = x.start + x.tm * TM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
-                epilogue<NC, NSUB, INJECT, true>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c, static_cast<float*>(a.out) + r0 * a.N, x.end);
+                if constexpr (SCALED) {                         // row-wise: rows are d_in's (from ro[0]), columns product x.g's
+                    if (a.mode & XMR_MODE_SCALE_ROWWISE)
+                        epilogue<NC, NSUB, INJECT, true, true, true>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
+                                                                     static_cast<float*>(a.out) + r0 * a.N, x.end, sa + r0,
+                                                                     sb + (unsigned long long)x.g * a.N);
+                    else
+                        epilogue<NC, NSUB, INJECT, true, true>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
+                                                               static_cast<float*>(a.out) + r0 * a.N, x.end, sa, sb);
+                } else {
+                    epilogue<NC, NSUB, INJECT, true>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c, static_cast<float*>(a.out) + r0 * a.N, x.end);
+                }
             } else {
                 const uint32_t row0 = tm * TM + rank * BM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
-                epilogue<NC, NSUB, INJECT>(a, tally, acc, row0, n0, nsub_t, hints, pol_c);
+                if constexpr (SCALED) {                         // row-wise: the stacked rows index sa, the tile's product sb
+                    if (a.mode & XMR_MODE_SCALE_ROWWISE)
+                        epilogue<NC, NSUB, INJECT, false, true, true>(a, tally, acc, row0, n0, nsub_t, hints, pol_c, nullptr, 0u, sa,
+                                                                      sb + (unsigned long long)((tm * TM) / a.M) * a.N);
+                    else
+                        epilogue<NC, NSUB, INJECT, false, true>(a, tally, acc, row0, n0, nsub_t, hints, pol_c, nullptr, 0u, sa, sb);
+                } else {
+                    epilogue<NC, NSUB, INJECT>(a, tally, acc, row0, n0, nsub_t, hints, pol_c);
+                }
             }
         }
         tally.flush(a.counters);
@@ -598,3 +644,38 @@ XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj0_nc3, 3, 0, false)
 XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc1, 1, 1, false)
 XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc2, 2, 1, false)
 XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc3, 3, 1, false)
+
+// Scaled FP8 (COAST_MM_SCALE_TENSOR / COAST_MM_SCALE_ROWWISE): the GEMM_FP8 variants with the scale pointers after the maps
+// (grouped: after ro and the group block); every replica multiplies its accumulator by the A and B scales before the vote
+#define XMR_SCALED_KERNEL(NAME, NC, INJ, WIDE, PAIR, CLUSTER)                                                \
+    extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                      \
+    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, \
+         const float* sa, const float* sb) {                                                             \
+        xmr::gemm::gemm_body<xmr::gemm::Fp8, NC, INJ != 0, WIDE, PAIR, false, true>(a, &map_a, &map_b, nullptr, nullptr, sa, sb); \
+    }
+#define XMR_SCALED_GRP_KERNEL(NAME, NC, INJ)                                                                 \
+    extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
+    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, \
+         const unsigned long long* ro, const uint8_t* grp, const float* sa, const float* sb) {           \
+        xmr::gemm::gemm_body<xmr::gemm::Fp8, NC, INJ != 0, false, false, true, true>(a, &map_a, &map_b, ro, grp, sa, sb); \
+    }
+XMR_SCALED_KERNEL(xmr_scaled_fp8_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj0_nc1, 1, 0)
+XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj0_nc2, 2, 0)
+XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj0_nc3, 3, 0)
+XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc1, 1, 1)
+XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc2, 2, 1)
+XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc3, 3, 1)

@@ -23,6 +23,8 @@ UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 / QSORT bat
 MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8: n_units = batch*M*N, inp / aux / out hold batch A / B / C
 MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
 MM_B_TRANSPOSED = COAST_MM_B_TRANSPOSED = 0x80000  # MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8: aux holds B^T, N x K per product (nn.Linear.weight)
+MM_SCALE_TENSOR = COAST_MM_SCALE_TENSOR = 0x100000    # GEMM_FP8: one fp32 scale of A and one of B, applied by every replica before the vote
+MM_SCALE_ROWWISE = COAST_MM_SCALE_ROWWISE = 0x200000  # GEMM_FP8: one fp32 scale per row of the stacked A and per column of each product's B
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 
@@ -51,7 +53,8 @@ class LaunchDesc(C.Structure):
                 ("n_units", C.c_uint64), ("unit_base", C.c_uint64),
                 ("unit_bytes", C.c_uint32), ("M", C.c_uint32), ("N", C.c_uint32), ("K", C.c_uint32),
                 ("d_in", C.c_void_p), ("d_out", C.c_void_p), ("d_aux", C.c_void_p),
-                ("key", C.c_uint8 * 16), ("plan", C.POINTER(_Plan)), ("d_status", C.c_void_p), ("d_rows", C.c_void_p)]
+                ("key", C.c_uint8 * 16), ("plan", C.POINTER(_Plan)), ("d_status", C.c_void_p), ("d_rows", C.c_void_p),
+                ("d_scale_a", C.c_void_p), ("d_scale_b", C.c_void_p)]
 
 
 class _Stats(C.Structure):
@@ -188,7 +191,8 @@ class Runtime:
         return s.cuda_stream
 
     def make_desc(self, kernel, num_clones, d_in, d_out, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0,
-                  d_aux=None, key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, d_status=None, d_rows=None):
+                  d_aux=None, key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, d_status=None, d_rows=None,
+                  scale_a=None, scale_b=None):
         d = LaunchDesc()
         d.kernel, d.num_clones, d.flags, d.mode = kernel, num_clones, flags, mode
         d.n_units, d.unit_base, d.unit_bytes = n_units, unit_base, unit_bytes
@@ -203,11 +207,15 @@ class Runtime:
             d.d_status = d_status.data_ptr() if hasattr(d_status, "data_ptr") else d_status
         if d_rows is not None:
             d.d_rows = d_rows.data_ptr() if hasattr(d_rows, "data_ptr") else d_rows
+        if scale_a is not None:
+            d.d_scale_a = scale_a.data_ptr() if hasattr(scale_a, "data_ptr") else scale_a
+        if scale_b is not None:
+            d.d_scale_b = scale_b.data_ptr() if hasattr(scale_b, "data_ptr") else scale_b
         keep = None
         if plan is not None and plan.mode != PLAN_NONE:
             keep = plan.to_c()
             d.plan = C.pointer(keep)
-        d._keep = (keep, d_in, d_out, d_aux, d_rows)
+        d._keep = (keep, d_in, d_out, d_aux, d_rows, scale_a, scale_b)
         return d
 
     def launch(self, desc: LaunchDesc, stream=None):
@@ -275,13 +283,18 @@ class Runtime:
 
     # -- convenience: device tensors in, device tensor + Stats out ----------------------------
     def run(self, kernel, num_clones, inp, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0, aux=None,
-            key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, out=None, stream=None, status=None, rows=None):
+            key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0, out=None, stream=None, status=None, rows=None,
+            scale_a=None, scale_b=None):
         """rows: with MM_GROUPED, the CUDA int64/uint64 tensor of M + 1 row offsets (M = the product count).
         K_GEMM_BF16: inp and aux are torch.bfloat16 tensors (or their uint16 / int16 views); the result is fp32 like K_GEMM_TF32's.
-        K_GEMM_FP8: inp and aux are torch.float8_e4m3fn tensors (or their uint8 views); the result is fp32."""
+        K_GEMM_FP8: inp and aux are torch.float8_e4m3fn tensors (or their uint8 views); the result is fp32.  With MM_SCALE_TENSOR
+        scale_a and scale_b are one-element float32 CUDA tensors; with MM_SCALE_ROWWISE scale_a holds one per stacked row of A and
+        scale_b one per column of each product's B."""
         torch = self.torch
         if mode & MM_GROUPED:
             self._check_rows(rows, M, N, n_units, inp, K, out, MM_ELEM_BYTES.get(kernel, 4))
+        if mode & (MM_SCALE_TENSOR | MM_SCALE_ROWWISE):
+            self._check_scales(scale_a, scale_b, mode, M, N, n_units, rows)
         ragged_qsort = bool(mode & UNIT_OFFSETS) and kernel == K_QSORT
         if out is None and ragged_qsort:       # the arrays are sorted into the bytes they came from: out mirrors inp
             out = torch.zeros(inp.numel() * inp.element_size(), dtype=torch.uint8, device=f"cuda:{self.device}")
@@ -293,7 +306,8 @@ class Runtime:
         if out is None:
             out = torch.empty(n_units * out_bytes(kernel, unit_bytes), dtype=torch.uint8, device=f"cuda:{self.device}")
         d = self.make_desc(kernel, num_clones, inp, out, n_units, flags=flags, mode=mode, unit_bytes=unit_bytes,
-                           M=M, N=N, K=K, d_aux=aux, key=key, plan=plan, unit_base=unit_base, d_status=status, d_rows=rows)
+                           M=M, N=N, K=K, d_aux=aux, key=key, plan=plan, unit_base=unit_base, d_status=status, d_rows=rows,
+                           scale_a=scale_a, scale_b=scale_b)
         self.launch(d, stream)
         return out, self.sync(stream)
 
@@ -316,6 +330,32 @@ class Runtime:
         if any(bad) or (out_rows is not None and int(ro[-1]) > out_rows):
             raise CoastError(ERR_BAD_ARG, f"MM_GROUPED: row offsets must not decrease, must span n_units / N = {R} rows and end "
                                           "within inp and out")
+
+    def _check_scales(self, scale_a, scale_b, mode, M, N, n_units, rows):
+        """A scaled launch's scales: contiguous float32 CUDA tensors, one element each (MM_SCALE_TENSOR), or (MM_SCALE_ROWWISE) one
+        per stacked row of A -- M, batch*M, or for groups at least ro[G] since row r of inp uses scale_a[r] -- and one per column
+        of each product's B, P*N.  The library reads what the shape says; this catches a short vector before it runs."""
+        torch = self.torch
+        for name, s in (("scale_a", scale_a), ("scale_b", scale_b)):
+            if s is None or not hasattr(s, "data_ptr") or s.dtype != torch.float32 or not s.is_cuda or not s.is_contiguous():
+                raise CoastError(ERR_BAD_ARG, f"MM_SCALE: {name} must be a contiguous float32 CUDA tensor")
+        if not mode & MM_SCALE_ROWWISE:
+            if scale_a.numel() != 1 or scale_b.numel() != 1:
+                raise CoastError(ERR_BAD_ARG, "MM_SCALE_TENSOR: scale_a and scale_b hold one float each")
+            return
+        if N < 1 or n_units % N:
+            raise CoastError(ERR_BAD_ARG, f"MM_SCALE_ROWWISE: n_units ({n_units}) must be a multiple of N ({N})")
+        if mode & MM_GROUPED:
+            P, need_a = M, int(rows[: M + 1].view(torch.int64)[-1])
+            ok_a = scale_a.numel() >= need_a
+        else:
+            P = n_units // (M * N) if M else 0
+            need_a = n_units // N
+            ok_a = scale_a.numel() == need_a
+        if not ok_a or scale_b.numel() != P * N:
+            raise CoastError(ERR_BAD_ARG, f"MM_SCALE_ROWWISE: scale_a holds {scale_a.numel()} floats and scale_b {scale_b.numel()}; "
+                                          f"one per row of A ({'at least ' if mode & MM_GROUPED else ''}{need_a}) and one per "
+                                          f"column of each B ({P * N}) are needed")
 
     def _check_offsets(self, inp, aux, n_units, unit_bytes, *, kernel=None, out=None):
         """A ragged batch's device offsets (int64 or uint64 tensor, n_units + 1 entries): they never decrease, no length
@@ -345,16 +385,17 @@ class Runtime:
     # -- the reference-facing host call: HOST buffers, H2D + kernel + D2H inside ---------------
     def run_host(self, kernel, num_clones, h_in, h_out, n_units, *, flags=0, mode=0, unit_bytes=0, M=0, N=0, K=0,
                  h_aux=None, key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0,
-                 abort_on_dwc: bool = False, h_rows=None) -> Stats:
-        """h_in/h_out/h_aux: CPU torch tensors or numpy arrays (pinned memory makes the copies async)."""
+                 abort_on_dwc: bool = False, h_rows=None, scale_a=None, scale_b=None) -> Stats:
+        """h_in/h_out/h_aux: CPU torch tensors or numpy arrays (pinned memory makes the copies async); scale_a / scale_b: the
+        host float32 scales of a MM_SCALE_TENSOR or MM_SCALE_ROWWISE call."""
         def ptr(x):
             if x is None:
                 return None
             return x.data_ptr() if hasattr(x, "data_ptr") else x.ctypes.data
         d = self.make_desc(kernel, num_clones, ptr(h_in), ptr(h_out), n_units, flags=flags, mode=mode,
                            unit_bytes=unit_bytes, M=M, N=N, K=K, d_aux=ptr(h_aux), key=key, plan=plan,
-                           unit_base=unit_base, d_rows=ptr(h_rows))
-        d._keep2 = (h_in, h_out, h_aux, h_rows)
+                           unit_base=unit_base, d_rows=ptr(h_rows), scale_a=ptr(scale_a), scale_b=ptr(scale_b))
+        d._keep2 = (h_in, h_out, h_aux, h_rows, scale_a, scale_b)
         st = _Stats()
         fn = self.L.coast_run_host if abort_on_dwc else self.L.coast_run_host_noabort
         self._check(fn(C.byref(d), C.byref(st)))

@@ -176,7 +176,8 @@ typedef struct coast_fault_plan {
  *            fault site of width 32 and one fp32 vote, as GEMM_TF32.  The 8-bit wgmma reads B K-major only, so B is
  *            transposed into P*K*N bytes of scratch first; with COAST_MM_B_TRANSPOSED the caller's B^T is read in place.
  *            COAST_MM_BATCHED and COAST_MM_GROUPED as below; the element offsets count 1-byte elements in d_in and d_aux,
- *            4-byte ones in d_out.
+ *            4-byte ones in d_out.  With COAST_MM_SCALE_TENSOR or COAST_MM_SCALE_ROWWISE every replica multiplies its value
+ *            by the scales of A and B before the vote (see below).
  *   MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 with COAST_MM_B_TRANSPOSED: aux: B^T, N x K row-major per product (see below).
  *   QSORT    in : n_units x unit_bytes, arrays of L = unit_bytes/4 int32 (L <= 1024)   out: the sorted arrays
  *   CHSTONE_SHA in : n_units x unit_bytes stream bytes (unit_bytes a multiple of 64, 64 <= unit_bytes < 2^29)
@@ -246,6 +247,28 @@ typedef struct coast_fault_plan {
  * rules are unchanged; the 2^31 bound on B's stacked rows is on batch*N (grouped: G*N) for every kernel with the bit.
  * COAST_ERR_BAD_ARG for the bit on any other kernel. */
 #define COAST_MM_B_TRANSPOSED   0x80000u
+/* Scaled FP8 matmuls (GEMM_FP8 only), what torch._scaled_mm(a, b, scale_a, scale_b) computes with fp32 output.  One of two
+ * bits; each combines with COAST_MM_BATCHED, COAST_MM_GROUPED and COAST_MM_B_TRANSPOSED:
+ *   COAST_MM_SCALE_TENSOR : d_scale_a and d_scale_b each point to ONE float, applied to every element of every product;
+ *   COAST_MM_SCALE_ROWWISE: d_scale_a holds one float per row of the stacked A, indexed like d_in's rows: M entries for one
+ *     product, batch*M for a batch (product b row i at b*M + i), and for groups row r of d_in uses d_scale_a[r], so entries
+ *     [ro[0], ro[G]) are read.  d_scale_b holds one float per column of each product's B, P*N entries (product p column n at
+ *     p*N + n); with COAST_MM_B_TRANSPOSED column n of B is row n of B^T, so the indexing is the same.
+ * Element (i, j) of replica r is v_r = (acc_r * sa_i) * sb_j, two fp32 multiplies rounded to nearest (tensorwise: sa_i = sa[0],
+ * sb_j = sb[0], so a tensorwise launch equals a row-wise one with constant vectors, bit for bit).  The vote, the counters and
+ * d_status work on v_0 .. v_{NC-1} as they do without scales on acc_r: the scale multiply is part of the protected function,
+ * and what is voted is what is stored.  Every replica reads the one copy of a scale (-noMemReplication's load rule).
+ * The fault site is unchanged: site 0 is the replica's final accumulator, 32 bits, flipped BEFORE the scale.  So a zero scale
+ * hides a flip that leaves the accumulator finite (the unit counts as injected and no vote disagrees; inf or NaN times 0 is NaN,
+ * which disagrees), a NaN scale makes every vote of its row or column disagree, and a multiply that rounds two different
+ * accumulators to one value hides the flip as well.
+ * d_scale_a and d_scale_b are device pointers for coast_launch and host pointers for coast_run_host, read only with a scale
+ * bit.  COAST_ERR_BAD_ARG for a scale bit on any other kernel, for both bits together, for a null scale pointer, for d_scale_a
+ * not 4-byte aligned and, row-wise, for d_scale_b not 8-byte aligned.  Shards: a row or product shard passes d_scale_a + its
+ * first row and d_scale_b + p_lo*N; a grouped shard passes d_scale_a unchanged (its rows are absolute, like d_in's) and
+ * d_scale_b + g_lo*N.  Tensorwise scales are passed unchanged. */
+#define COAST_MM_SCALE_TENSOR   0x100000u
+#define COAST_MM_SCALE_ROWWISE  0x200000u
 #define COAST_AES_DECRYPT       0x1u
 #define COAST_AES_KEY_PER_UNIT  0x2u
 #define COAST_AES_KEY_WRITEBACK 0x4u   /* with KEY_PER_UNIT: store what aes_enc_dec() leaves in key[] (TI_aes_128.c:214-221 mutates
@@ -272,6 +295,8 @@ typedef struct coast_launch_desc {
                               field of the board report line (decoder.py:66) for campaign tooling.  A device
                               pointer for coast_launch, a host pointer for coast_run_host (not for the matmuls). */
     const void* d_rows;    /* COAST_MM_GROUPED only (read only with the bit): G + 1 u64 row offsets, see above */
+    const void* d_scale_a; /* COAST_MM_SCALE_TENSOR / _ROWWISE only (read only with a bit): float scales of A's rows, see above */
+    const void* d_scale_b; /* ... and of B's columns */
 } coast_launch_desc;
 
 /* Counters of everything launched since the last coast_sync(). */
@@ -394,7 +419,10 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  * chunk uploads its A and B matrices, launches with its unit_base and downloads its C matrices.  Grouped matmuls
  * (COAST_MM_GROUPED) are staged in chunks of whole products whose A rows, B matrices, C rows and offsets fit COAST_HOST_CHUNK_BYTES
  * (a larger product is a chunk of its own): each uploads its slice of the offsets unchanged and launches with d_in and d_out
- * biased by ro[first] rows.  On any failure every copy already queued on
+ * biased by ro[first] rows.  Scaled GEMM_FP8 (COAST_MM_SCALE_*) keeps the chunks of the unscaled call: tensorwise, the two
+ * floats go up once; row-wise, row blocks send B's column scales once with B and each block its rows' A scales, batched chunks
+ * the A rows and B columns of their products, grouped chunks A scales [ro[first], ro[end]) biased like d_in and B scales
+ * [first*N, end*N).  On any failure every copy already queued on
  * the caller's buffers is drained before the call returns. */
 int  coast_run_host(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
 /* What the last host call did: "staged", "hybrid" or "zerocopy"; unbatched matmuls: "row-blocks" or "one-shot"; grouped: "groups". */
