@@ -505,7 +505,8 @@ static int encode_map(const map_desc* want, CUdeviceptr scratch, int cached, CUt
  * (batch*M)-row matrix and only B changes from one product to the next.  Grouped (COAST_MM_GROUPED): M is the product count G,
  * the stacked A and C are one R-row matrix from row ro[0] (R = n_units / N) and B is G matrices end to end. */
 typedef struct {
-    unsigned es;                  /* bytes per element of A and B; C elements are 4 bytes */
+    unsigned es;                  /* bytes per element of A and B */
+    unsigned ces;                 /* bytes per element of C: 4, or 2 with COAST_MM_OUT_BF16 (bfloat16) */
     int batched, grouped, bt;     /* the mode bits */
     uint64_t P;                   /* products: 1, the batch or G */
     uint64_t rows;                /* stacked rows of A and C: batch*M or R */
@@ -591,15 +592,25 @@ static int mm_scale_check(const coast_launch_desc* d) {
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_SCALE_ROWWISE: d_scale_b must be 8-byte aligned (column scales are read in pairs)");
     return COAST_OK;
 }
-/* The checks shared by coast_launch and coast_run_host: a matmul mode bit on another kernel, the scale bits, then the shape of
- * a batch or of groups.  Fills *m for the matmul kernels. */
+/* BF16 output (GEMM_BF16 and GEMM_FP8 only; not with a scale bit) */
+static int mm_out_check(const coast_launch_desc* d) {
+    if (!(d->mode & COAST_MM_OUT_BF16)) return COAST_OK;
+    if (d->kernel != COAST_K_GEMM_BF16 && d->kernel != COAST_K_GEMM_FP8)
+        return fail(COAST_ERR_BAD_ARG, "COAST_MM_OUT_BF16: bfloat16 output exists for GEMM_BF16 and GEMM_FP8 only (kernel %u)", d->kernel);
+    if (d->mode & (COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE))
+        return fail(COAST_ERR_UNSUPPORTED, "COAST_MM_OUT_BF16: scaled GEMM_FP8 has no bfloat16-output kernels yet; its C is fp32");
+    return COAST_OK;
+}
+/* The checks shared by coast_launch and coast_run_host: a matmul mode bit on another kernel, the scale and output bits, then the
+ * shape of a batch or of groups.  Fills *m for the matmul kernels; m->ces is the one place that knows C's element size. */
 static int mm_check(const coast_launch_desc* d, mm_shape* m) {
     int rc;
     memset(m, 0, sizeof *m);
     if ((rc = mm_bit_refused(d, COAST_MM_BATCHED)) || (rc = mm_bit_refused(d, COAST_MM_GROUPED)) ||
-        (rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)) || (rc = mm_scale_check(d)))
+        (rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)) || (rc = mm_scale_check(d)) || (rc = mm_out_check(d)))
         return rc;
     if (!is_matmul(d->kernel)) return COAST_OK;
+    m->ces = (d->mode & COAST_MM_OUT_BF16) ? 2u : KINFO[d->kernel].out_bytes;
     m->scaled = (d->mode & (COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE)) != 0;
     m->rowwise = (d->mode & COAST_MM_SCALE_ROWWISE) != 0;
     m->es = KINFO[d->kernel].mm_elem;
@@ -645,8 +656,15 @@ static uint64_t mm_row_tiles(const mm_shape* m, unsigned bm) { return m->rows / 
 /* A matmul kernel's name: stem, path variant, [_bt], [_grp], then _nc<n>_inj<i> for the kernels that came before batched,
  * grouped, BF16 and transposed-B launches and _inj<i>_nc<n> for the others.  GEMM_FP8's names are whole formats: one set of
  * kernels serves B and B^T, the narrow kernel exists at NC 1 only, and the grouped ones (always 128 x 128 tiles) carry no variant;
- * scaled GEMM_FP8 (xmr_scaled_fp8*) has the same set. */
-static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, int scaled, uint32_t nc, int inj) {
+ * scaled GEMM_FP8 (xmr_scaled_fp8*) has the same set.  BF16 output (o16: 2-byte C elements) has a twin of each GEMM_BF16 and
+ * GEMM_FP8 kernel, named xmr_o16_ + the name after its xmr_gemm_ prefix. */
+static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, int scaled, int o16, uint32_t nc, int inj) {
+    if (o16) {
+        char twin[64];
+        mm_kernel_name(twin, kernel, variant, bt, grouped, scaled, 0, nc, inj);
+        snprintf(name, 64, "%.4so16_%s", twin, strchr(twin + 4, '_') + 1);    /* xmr_gemm_<rest> -> xmr_o16_<rest> */
+        return;
+    }
     if (kernel == COAST_K_GEMM_FP8 && scaled) {
         const char* f = grouped ? "xmr_scaled_fp8_grp_inj%d_nc%u" : *variant == 'p' ? "xmr_scaled_fp8p_inj%d_nc%u"
                       : *variant == 'n' ? "xmr_scaled_fp8n_inj%d_nc1" : "xmr_scaled_fp8_inj%d_nc%u";
@@ -806,7 +824,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     /* the kernels find a batch from n_units / N (rows of the stacked problem) and a.M (rows per product): a batch of one is
      * an unbatched launch, argument block included */
     a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~(COAST_MM_BATCHED | COAST_MM_GROUPED | COAST_MM_B_TRANSPOSED |
-                                                                      COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE);
+                                                                      COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE | COAST_MM_OUT_BF16);
     if (m.rowwise) a.mode |= XMR_MODE_SCALE_ROWWISE;
     a.M = d->M; a.N = d->N; a.K = d->K;
     memcpy(a.key, d->key, 16);
@@ -925,7 +943,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
             L.ctas = mm_row_tiles(&m, XMR_MMT_BM) * (d->N / XMR_MMT_BN); L.waves = 0;   /* grouped: surplus CTAs exit */
             L.grp_tm = XMR_MMT_BM; L.grp_tiles_n = d->N / XMR_MMT_BN;
         }
-        mm_kernel_name(L.name, d->kernel, variant, bt_name, m.grouped, 0, nc, inj);
+        mm_kernel_name(L.name, d->kernel, variant, bt_name, m.grouped, 0, 0, nc, inj);
         break;
     }
     case COAST_K_QSORT:
@@ -990,7 +1008,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
         const int pair = !m.grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
         /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it, TF32 and FP8 only skip the transposing pre-pass */
-        mm_kernel_name(L.name, d->kernel, pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt, m.grouped, m.scaled, nc, inj);
+        mm_kernel_name(L.name, d->kernel, pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt, m.grouped, m.scaled, m.ces == 2, nc, inj);
         { const char* g = getenv("COAST_GEMM_GROUP_M");
           if (g && atoi(g) > 0 && atoi(g) <= (int)XMR_MODE_GROUP_M_MASK) a.mode = (a.mode & ~XMR_MODE_GROUP_M_MASK) | (unsigned)atoi(g); }
         /* L2 eviction priorities: A evict_last, B and C evict_first; COAST_GEMM_L2_HINTS=0 loads and stores with the normal policy */
@@ -1421,7 +1439,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
     { const char* e = getenv("COAST_HOST_CHUNK_BYTES"); if (e && atoll(e) > 0) chunk_bytes = (uint64_t)atoll(e); }
     host_sched s; memset(&s, 0, sizeof s);
     s.d = d; s.upi = 1; s.path = "staged";
-    if ((rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)) || (rc = mm_scale_check(d))) return rc;
+    if ((rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)) || (rc = mm_scale_check(d)) || (rc = mm_out_check(d))) return rc;
 
     if (d->mode & COAST_UNIT_OFFSETS) {                      /* ragged: staged only */
         if ((rc = ragged_check(d))) return rc;
@@ -1449,7 +1467,7 @@ static int run_host_impl(const coast_launch_desc* d, coast_stats* out, int* dwc_
     if ((rc = mm_check(d, &m))) return rc;
     if (is_matmul(d->kernel)) {
         if (d->d_status) return fail(COAST_ERR_UNSUPPORTED, "coast_run_host: d_status is not staged for the matmul kernels; use coast_launch");
-        const uint64_t a_row = (uint64_t)d->K * m.es, c_row = (uint64_t)d->N * 4u, bb = (uint64_t)d->K * d->N * m.es;
+        const uint64_t a_row = (uint64_t)d->K * m.es, c_row = (uint64_t)d->N * m.ces, bb = (uint64_t)d->K * d->N * m.es;
         if (m.grouped) {                                     /* whole products per chunk, the offsets checked first */
             const uint64_t* ro = (const uint64_t*)d->d_rows;
             for (uint32_t g = 0; g < d->M; ++g)

@@ -89,6 +89,15 @@ __device__ __forceinline__ void tma_load_2d_mcast(void* smem_dst, const CUtensor
 __device__ __forceinline__ void st_v2_hint(void* p, uint32_t x, uint32_t y, uint64_t pol) {
     asm volatile("st.global.L2::cache_hint.v2.b32 [%0], {%1, %2}, %3;" ::"l"(p), "r"(x), "r"(y), "l"(pol) : "memory");
 }
+__device__ __forceinline__ void st_b32_hint(void* p, uint32_t x, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(p), "r"(x), "l"(pol) : "memory");
+}
+// two fp32 values (bit patterns) rounded to bfloat16, to nearest even, into one bf16x2: lo in bits [0,16), hi in [16,32)
+__device__ __forceinline__ uint32_t pack_bf16x2_rn(uint32_t lo, uint32_t hi) {
+    uint32_t d;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "r"(hi), "r"(lo));
+    return d;
+}
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -233,13 +242,21 @@ __device__ __forceinline__ void wgmma_u8_m64n64k32(uint32_t (&d)[32], uint64_t d
 // `col` is sb[col] or sb[0] (the caller offsets both to the tile's product).  The two layouts are two instances, so neither
 // carries the other's loads and branches next to the accumulators.  Every replica reads the one copy
 // of a scale (-noMemReplication's load rule), after the main loop, so nothing of it is live next to the accumulators.
-template <int NC, int NSUB, bool INJECT, bool GROUPED = false, bool SCALED = false, bool ROWWISE = false>
+// OUT_BF16 (xmr_o16_*, COAST_MM_OUT_BF16; not with SCALED): C holds bfloat16.  Each replica rounds its thread's two values
+// (after the fault hook) into one bf16x2 with cvt.rn, the vote and the tally run on the 16-bit halves (`fcmp oeq` on the widened
+// values, the majority voter bitwise on the pair), and one 4-byte store writes the voted pair.  Its own branch, so that the fp32
+// epilogue's code is not touched.
+template <bool OUT_BF16> struct CElem { using T = float; };
+template <> struct CElem<true> { using T = uint16_t; };
+template <int NC, int NSUB, bool INJECT, bool GROUPED = false, bool SCALED = false, bool ROWWISE = false, bool OUT_BF16 = false>
 __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float (&acc)[NC][NSUB][64], uint32_t row0, uint32_t n0, uint32_t nsub_t,
-                                         bool hints, uint64_t pol_c, float* c_grp = nullptr, uint32_t row_end = 0,
+                                         bool hints, uint64_t pol_c, typename CElem<OUT_BF16>::T* c_grp = nullptr, uint32_t row_end = 0,
                                          const float* sa = nullptr, const float* sb = nullptr) {
+    static_assert(!(SCALED && OUT_BF16), "scaled GEMM_FP8 has no bfloat16-output epilogue");
+    using CT = typename CElem<OUT_BF16>::T;
     const uint32_t flags = a.flags;
     const bool majority = flags & COAST_F_MAJORITY_VOTER;
-    float* C = GROUPED ? c_grp : static_cast<float*>(a.out);
+    CT* C = GROUPED ? c_grp : static_cast<CT*>(a.out);
     const uint32_t lane = threadIdx.x & 31;
     constexpr bool rowwise = SCALED && ROWWISE;
     float s_row[2] = {1.f, 1.f}, s_col = 1.f;
@@ -265,41 +282,82 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float 
                 const uint32_t row = row0 + 8 * h, col = n0 + sub * WG_N + 8 * j + 2 * (lane & 3);
                 if constexpr (GROUPED) { if (row >= row_end) continue; }
                 const unsigned long long local0 = (unsigned long long)row * a.N + col;
-                uint32_t o[2];
+                if constexpr (OUT_BF16) {
+                    uint32_t x[3][2];                            // [replica][element]: the accumulators after the fault hook
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int i = 4 * j + 2 * h + e;
-                    uint32_t r0 = __float_as_uint(acc[0][sub][i]);
-                    uint32_t r1 = NC > 1 ? __float_as_uint(acc[NC > 1 ? 1 : 0][sub][i]) : r0;
-                    uint32_t r2 = NC > 2 ? __float_as_uint(acc[NC > 2 ? 2 : 0][sub][i]) : r0;
-                    if (INJECT) {
-                        Fault f = fault_for_unit(a, NC, local0 + e, [](uint32_t) { return 32u; });
-                        if (f.active) {
-                            tally.injected++;
-                            uint32_t mk = 1u << f.bit;
-                            if (f.replica == 0) r0 ^= mk; else if (f.replica == 1) r1 ^= mk; else r2 ^= mk;
+                    for (int e = 0; e < 2; ++e) {
+                        const int i = 4 * j + 2 * h + e;
+                        x[0][e] = __float_as_uint(acc[0][sub][i]);
+                        x[1][e] = NC > 1 ? __float_as_uint(acc[NC > 1 ? 1 : 0][sub][i]) : x[0][e];
+                        x[2][e] = NC > 2 ? __float_as_uint(acc[NC > 2 ? 2 : 0][sub][i]) : x[0][e];
+                        if (INJECT) {
+                            Fault f = fault_for_unit(a, NC, local0 + e, [](uint32_t) { return 32u; });
+                            if (f.active) {
+                                tally.injected++;
+                                const uint32_t mk = 1u << f.bit;
+                                if (f.replica == 0) x[0][e] ^= mk; else if (f.replica == 1) x[1][e] ^= mk; else x[2][e] ^= mk;
+                            }
                         }
                     }
-                    if constexpr (SCALED) {                      // every replica scales its own value; explicit _rn: no contraction
-                        const float sr = s_row[h], sc = e ? s_pair.y : s_pair.x;
-                        r0 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r0), sr), sc));
-                        if (NC > 1) r1 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r1), sr), sc));
-                        if (NC > 2) r2 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r2), sr), sc));
+                    const uint32_t p0 = pack_bf16x2_rn(x[0][0], x[0][1]);         // every replica rounds its own pair
+                    const uint32_t p1 = NC > 1 ? pack_bf16x2_rn(x[1][0], x[1][1]) : p0;
+                    const uint32_t p2 = NC > 2 ? pack_bf16x2_rn(x[2][0], x[2][1]) : p0;
+                    uint32_t o = p0;
+                    if (NC == 3 && majority) o = (p0 & p1) | (p0 & p2) | (p1 & p2);
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const uint32_t half = e ? 0xFFFF0000u : 0x0000FFFFu;       // element e's bfloat16
+                        const float f0 = __uint_as_float(e ? p0 & half : p0 << 16), f1 = __uint_as_float(e ? p1 & half : p1 << 16),
+                                    f2 = __uint_as_float(e ? p2 & half : p2 << 16);
+                        uint32_t bad = 0;
+                        if (NC == 2) bad = (f0 == f1) ? 0u : 1u;
+                        if (NC == 3) {
+                            const bool c01 = (f0 == f1), c02 = (f0 == f2);       // fcmp oeq on the widened values
+                            if (!majority && !c01) o = (o & ~half) | (p2 & half);
+                            bad = (c01 && c02) ? 0u : 1u;
+                        }
+                        tally.unit_exit<NC>(bad, 1u, flags, a.unit_base + local0 + e);
                     }
-                    const float f0 = __uint_as_float(r0), f1 = __uint_as_float(r1), f2 = __uint_as_float(r2);
-                    uint32_t vote = r0, bad = 0;
-                    if (NC == 2) bad = (f0 == f1) ? 0u : 1u;
-                    if (NC == 3) {
-                        const bool c01 = (f0 == f1), c02 = (f0 == f2);       // fcmp oeq
-                        vote = majority ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
-                        bad = (c01 && c02) ? 0u : 1u;
+                    CT* dst = C + local0;
+                    if (hints) st_b32_hint(dst, o, pol_c);
+                    else *reinterpret_cast<uint32_t*>(dst) = o;
+                } else {
+                    uint32_t o[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int i = 4 * j + 2 * h + e;
+                        uint32_t r0 = __float_as_uint(acc[0][sub][i]);
+                        uint32_t r1 = NC > 1 ? __float_as_uint(acc[NC > 1 ? 1 : 0][sub][i]) : r0;
+                        uint32_t r2 = NC > 2 ? __float_as_uint(acc[NC > 2 ? 2 : 0][sub][i]) : r0;
+                        if (INJECT) {
+                            Fault f = fault_for_unit(a, NC, local0 + e, [](uint32_t) { return 32u; });
+                            if (f.active) {
+                                tally.injected++;
+                                uint32_t mk = 1u << f.bit;
+                                if (f.replica == 0) r0 ^= mk; else if (f.replica == 1) r1 ^= mk; else r2 ^= mk;
+                            }
+                        }
+                        if constexpr (SCALED) {                      // every replica scales its own value; explicit _rn: no contraction
+                            const float sr = s_row[h], sc = e ? s_pair.y : s_pair.x;
+                            r0 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r0), sr), sc));
+                            if (NC > 1) r1 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r1), sr), sc));
+                            if (NC > 2) r2 = __float_as_uint(__fmul_rn(__fmul_rn(__uint_as_float(r2), sr), sc));
+                        }
+                        const float f0 = __uint_as_float(r0), f1 = __uint_as_float(r1), f2 = __uint_as_float(r2);
+                        uint32_t vote = r0, bad = 0;
+                        if (NC == 2) bad = (f0 == f1) ? 0u : 1u;
+                        if (NC == 3) {
+                            const bool c01 = (f0 == f1), c02 = (f0 == f2);       // fcmp oeq
+                            vote = majority ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
+                            bad = (c01 && c02) ? 0u : 1u;
+                        }
+                        o[e] = vote;
+                        tally.unit_exit<NC>(bad, 1u, flags, a.unit_base + local0 + e);
                     }
-                    o[e] = vote;
-                    tally.unit_exit<NC>(bad, 1u, flags, a.unit_base + local0 + e);
+                    float* dst = C + local0;
+                    if (hints) st_v2_hint(dst, o[0], o[1], pol_c);
+                    else *reinterpret_cast<uint2*>(dst) = make_uint2(o[0], o[1]);
                 }
-                float* dst = C + local0;
-                if (hints) st_v2_hint(dst, o[0], o[1], pol_c);
-                else *reinterpret_cast<uint2*>(dst) = make_uint2(o[0], o[1]);
             }
         }
     }
@@ -310,7 +368,8 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float 
 // GROUPED (single CTAs with 128 x 128 tiles, xmr_mm_grp.cuh): a.M products of their own row counts, `ro` their row offsets and
 // `grp` the group block: the tiles come from its tile_start table, A through its rebased map, B^T rows from g N (Bf16: B rows from g K).
 // SCALED (xmr_scaled_fp8*): sa and sb are the caller's scales (see epilogue); a row-wise B scale vector holds N entries per product.
-template <class OP, int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false, bool SCALED = false>
+// OUT_BF16 (xmr_o16_*): C holds bfloat16 at the same element offsets (see epilogue).
+template <class OP, int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false, bool SCALED = false, bool OUT_BF16 = false>
 __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b,
                                           const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr,
                                           const float* sa = nullptr, const float* sb = nullptr) {
@@ -464,27 +523,29 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
                 const unsigned long long r0 = __ldg(ro);
                 const grp::Tile x = grp::tile_of(ro, r0, R, ts, n_grp, tiles_n, group_m, tile);
                 const uint32_t row0 = x.start + x.tm * TM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
+                using CT = typename CElem<OUT_BF16>::T;
                 if constexpr (SCALED) {                         // row-wise: rows are d_in's (from ro[0]), columns product x.g's
                     if (a.mode & XMR_MODE_SCALE_ROWWISE)
-                        epilogue<NC, NSUB, INJECT, true, true, true>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
-                                                                     static_cast<float*>(a.out) + r0 * a.N, x.end, sa + r0,
+                        epilogue<NC, NSUB, INJECT, true, true, true, OUT_BF16>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
+                                                                     static_cast<CT*>(a.out) + r0 * a.N, x.end, sa + r0,
                                                                      sb + (unsigned long long)x.g * a.N);
                     else
-                        epilogue<NC, NSUB, INJECT, true, true>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
-                                                               static_cast<float*>(a.out) + r0 * a.N, x.end, sa, sb);
+                        epilogue<NC, NSUB, INJECT, true, true, false, OUT_BF16>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
+                                                               static_cast<CT*>(a.out) + r0 * a.N, x.end, sa, sb);
                 } else {
-                    epilogue<NC, NSUB, INJECT, true>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c, static_cast<float*>(a.out) + r0 * a.N, x.end);
+                    epilogue<NC, NSUB, INJECT, true, false, false, OUT_BF16>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
+                                                                             static_cast<CT*>(a.out) + r0 * a.N, x.end);
                 }
             } else {
                 const uint32_t row0 = tm * TM + rank * BM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
                 if constexpr (SCALED) {                         // row-wise: the stacked rows index sa, the tile's product sb
                     if (a.mode & XMR_MODE_SCALE_ROWWISE)
-                        epilogue<NC, NSUB, INJECT, false, true, true>(a, tally, acc, row0, n0, nsub_t, hints, pol_c, nullptr, 0u, sa,
+                        epilogue<NC, NSUB, INJECT, false, true, true, OUT_BF16>(a, tally, acc, row0, n0, nsub_t, hints, pol_c, nullptr, 0u, sa,
                                                                       sb + (unsigned long long)((tm * TM) / a.M) * a.N);
                     else
-                        epilogue<NC, NSUB, INJECT, false, true>(a, tally, acc, row0, n0, nsub_t, hints, pol_c, nullptr, 0u, sa, sb);
+                        epilogue<NC, NSUB, INJECT, false, true, false, OUT_BF16>(a, tally, acc, row0, n0, nsub_t, hints, pol_c, nullptr, 0u, sa, sb);
                 } else {
-                    epilogue<NC, NSUB, INJECT>(a, tally, acc, row0, n0, nsub_t, hints, pol_c);
+                    epilogue<NC, NSUB, INJECT, false, false, false, OUT_BF16>(a, tally, acc, row0, n0, nsub_t, hints, pol_c);
                 }
             }
         }
@@ -541,10 +602,11 @@ xmr_gemm_bt_u8(const uint8_t* __restrict__ B, uint8_t* __restrict__ Bt, unsigned
     }
 }
 
-#define XMR_GEMM_KERNEL(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER)                                            \
+#define XMR_GEMM_KERNEL(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER) XMR_GEMM_KERNEL_C(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER, false)
+#define XMR_GEMM_KERNEL_C(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER, O16)                                    \
     extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                      \
     NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b) { \
-        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, PAIR>(a, &map_a, &map_b);                        \
+        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, PAIR, false, false, O16>(a, &map_a, &map_b);     \
     }
 #define XMR_NO_CLUSTER
 #define XMR_PAIR_CLUSTER __cluster_dims__(2, 1, 1)
@@ -567,11 +629,12 @@ XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc3_inj1, 3, 1, false, true, XMR_PAIR_CLUST
 
 // grouped (COAST_MM_GROUPED): single CTAs and 128 x 128 tiles (tf32n unprotected); `ro` = the caller's row offsets, `grp` = the
 // group block the pre-pass wrote (xmr_mm_grp.cuh)
-#define XMR_GEMM_GRP_KERNEL(OP, NAME, NC, INJ, WIDE)                                                       \
+#define XMR_GEMM_GRP_KERNEL(OP, NAME, NC, INJ, WIDE) XMR_GEMM_GRP_KERNEL_C(OP, NAME, NC, INJ, WIDE, false)
+#define XMR_GEMM_GRP_KERNEL_C(OP, NAME, NC, INJ, WIDE, O16)                                                \
     extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
     NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, \
          const unsigned long long* ro, const uint8_t* grp) {                                             \
-        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, false, true>(a, &map_a, &map_b, ro, grp);        \
+        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, false, true, false, O16>(a, &map_a, &map_b, ro, grp); \
     }
 XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj0_nc2, 2, 0, false)
 XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj0_nc3, 3, 0, false)
@@ -679,3 +742,67 @@ XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj0_nc3, 3, 0)
 XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc1, 1, 1)
 XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc2, 2, 1)
 XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc3, 3, 1)
+
+// BF16 output (COAST_MM_OUT_BF16): every GEMM_BF16 and GEMM_FP8 variant once more, named xmr_o16_ + the name without its
+// xmr_gemm_ prefix; C holds bfloat16, each replica rounds its values before the vote (see epilogue).  Scaled GEMM_FP8 has no
+// BF16-output set: its TMR and DWC kernels spilled 104-296 bytes with it (DESIGN.md §10 item 12)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16_grp_inj0_nc2, 2, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16_grp_inj0_nc3, 3, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16_grp_inj1_nc2, 2, 1, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16_grp_inj1_nc3, 3, 1, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16n_grp_inj0_nc1, 1, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16n_grp_inj1_nc1, 1, 1, false, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16n_bt_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16n_bt_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16_bt_grp_inj0_nc2, 2, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16_bt_grp_inj0_nc3, 3, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16_bt_grp_inj1_nc2, 2, 1, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16_bt_grp_inj1_nc3, 3, 1, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16n_bt_grp_inj0_nc1, 1, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16n_bt_grp_inj1_nc1, 1, 1, false, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER, true)
+XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj0_nc1, 1, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj0_nc2, 2, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj0_nc3, 3, 0, false, true)
+XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj1_nc1, 1, 1, false, true)
+XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj1_nc2, 2, 1, false, true)
+XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj1_nc3, 3, 1, false, true)

@@ -25,6 +25,7 @@ MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32 / GEMM
 MM_B_TRANSPOSED = COAST_MM_B_TRANSPOSED = 0x80000  # MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8: aux holds B^T, N x K per product (nn.Linear.weight)
 MM_SCALE_TENSOR = COAST_MM_SCALE_TENSOR = 0x100000    # GEMM_FP8: one fp32 scale of A and one of B, applied by every replica before the vote
 MM_SCALE_ROWWISE = COAST_MM_SCALE_ROWWISE = 0x200000  # GEMM_FP8: one fp32 scale per row of the stacked A and per column of each product's B
+MM_OUT_BF16 = COAST_MM_OUT_BF16 = 0x400000            # GEMM_BF16 / GEMM_FP8: C is bfloat16, every replica rounds before the vote
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 
@@ -33,7 +34,10 @@ OUT_BYTES = {K_CRC16: 2, K_SHA256: 32, K_AES128: 16, K_MM_U32: 4, K_GEMM_TF32: 4
 MM_ELEM_BYTES = {K_GEMM_BF16: 2, K_GEMM_FP8: 1}   # bytes per A and B element of the matmuls; 4 for MM_U32 and GEMM_TF32
 
 
-def out_bytes(kernel: int, unit_bytes: int = 0) -> int:
+def out_bytes(kernel: int, unit_bytes: int = 0, mode: int = 0) -> int:
+    """bytes of output per unit; with MM_OUT_BF16, GEMM_BF16 and GEMM_FP8 write 2-byte bfloat16 C elements"""
+    if mode & MM_OUT_BF16 and kernel in (K_GEMM_BF16, K_GEMM_FP8):
+        return 2
     return unit_bytes if kernel == K_QSORT else OUT_BYTES[kernel]
 
 
@@ -289,10 +293,11 @@ class Runtime:
         K_GEMM_BF16: inp and aux are torch.bfloat16 tensors (or their uint16 / int16 views); the result is fp32 like K_GEMM_TF32's.
         K_GEMM_FP8: inp and aux are torch.float8_e4m3fn tensors (or their uint8 views); the result is fp32.  With MM_SCALE_TENSOR
         scale_a and scale_b are one-element float32 CUDA tensors; with MM_SCALE_ROWWISE scale_a holds one per stacked row of A and
-        scale_b one per column of each product's B."""
+        scale_b one per column of each product's B.  With MM_OUT_BF16 (K_GEMM_BF16, K_GEMM_FP8) the result is bfloat16 bytes, two
+        per element: view it as torch.bfloat16."""
         torch = self.torch
         if mode & MM_GROUPED:
-            self._check_rows(rows, M, N, n_units, inp, K, out, MM_ELEM_BYTES.get(kernel, 4))
+            self._check_rows(rows, M, N, n_units, inp, K, out, MM_ELEM_BYTES.get(kernel, 4), out_bytes(kernel, unit_bytes, mode))
         if mode & (MM_SCALE_TENSOR | MM_SCALE_ROWWISE):
             self._check_scales(scale_a, scale_b, mode, M, N, n_units, rows)
         ragged_qsort = bool(mode & UNIT_OFFSETS) and kernel == K_QSORT
@@ -302,18 +307,18 @@ class Runtime:
             self._check_offsets(inp, aux, n_units, unit_bytes, kernel=kernel, out=out)
         if out is None and mode & MM_GROUPED:   # C rows at ro[g]: out covers rows [0, ro[G]), like inp
             R_end = int(rows[: M + 1].view(torch.int64)[-1])
-            out = torch.empty(R_end * N * 4, dtype=torch.uint8, device=f"cuda:{self.device}")
+            out = torch.empty(R_end * N * out_bytes(kernel, unit_bytes, mode), dtype=torch.uint8, device=f"cuda:{self.device}")
         if out is None:
-            out = torch.empty(n_units * out_bytes(kernel, unit_bytes), dtype=torch.uint8, device=f"cuda:{self.device}")
+            out = torch.empty(n_units * out_bytes(kernel, unit_bytes, mode), dtype=torch.uint8, device=f"cuda:{self.device}")
         d = self.make_desc(kernel, num_clones, inp, out, n_units, flags=flags, mode=mode, unit_bytes=unit_bytes,
                            M=M, N=N, K=K, d_aux=aux, key=key, plan=plan, unit_base=unit_base, d_status=status, d_rows=rows,
                            scale_a=scale_a, scale_b=scale_b)
         self.launch(d, stream)
         return out, self.sync(stream)
 
-    def _check_rows(self, rows, G, N, n_units, inp, K, out, esize=4):
+    def _check_rows(self, rows, G, N, n_units, inp, K, out, esize=4, out_esize=4):
         """A grouped launch's device row offsets (int64 or uint64 tensor, G + 1 entries): they never decrease and span exactly
-        n_units / N rows, which lie within inp (K elements of esize bytes per row) and out (N per row).  The kernels only clamp; this catches a bad table
+        n_units / N rows, which lie within inp (K elements of esize bytes per row) and out (N elements of out_esize bytes per row).  The kernels only clamp; this catches a bad table
         before it runs."""
         torch = self.torch
         if rows is None or not hasattr(rows, "data_ptr") or rows.dtype not in (torch.int64, torch.uint64) or not rows.is_cuda:
@@ -325,7 +330,7 @@ class Runtime:
         ro = rows[: G + 1].view(torch.int64)
         R = n_units // N
         in_rows = inp.numel() * inp.element_size() // (esize * K) if K else 0
-        out_rows = out.numel() * out.element_size() // (4 * N) if out is not None else None
+        out_rows = out.numel() * out.element_size() // (out_esize * N) if out is not None else None
         bad = torch.stack([(ro < 0).any(), (ro[1:] < ro[:-1]).any(), ro[-1] - ro[0] != R, ro[-1] > in_rows]).tolist()
         if any(bad) or (out_rows is not None and int(ro[-1]) > out_rows):
             raise CoastError(ERR_BAD_ARG, f"MM_GROUPED: row offsets must not decrease, must span n_units / N = {R} rows and end "
@@ -387,7 +392,8 @@ class Runtime:
                  h_aux=None, key: bytes | None = None, plan: FaultPlan | None = None, unit_base=0,
                  abort_on_dwc: bool = False, h_rows=None, scale_a=None, scale_b=None) -> Stats:
         """h_in/h_out/h_aux: CPU torch tensors or numpy arrays (pinned memory makes the copies async); scale_a / scale_b: the
-        host float32 scales of a MM_SCALE_TENSOR or MM_SCALE_ROWWISE call."""
+        host float32 scales of a MM_SCALE_TENSOR or MM_SCALE_ROWWISE call.  With MM_OUT_BF16, h_out receives bfloat16 bytes, two
+        per element."""
         def ptr(x):
             if x is None:
                 return None

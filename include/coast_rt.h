@@ -168,7 +168,8 @@ typedef struct coast_fault_plan {
  *   GEMM_BF16 in : A, M x K bfloat16 row-major; aux: B, K x N bfloat16 row-major   out: C, M x N float: the fp32-accumulated
  *            sum of the exact bf16 x bf16 products.  M%128 == N%128 == K%64 == 0 (grouped: N and K only), buffers 16-byte
  *            aligned.  A unit is one C element with one fault site of width 32, as GEMM_TF32.  COAST_MM_BATCHED and
- *            COAST_MM_GROUPED as below; the element offsets there count 2-byte elements in d_in and d_aux, 4-byte ones in d_out.
+ *            COAST_MM_GROUPED as below; the element offsets there count 2-byte elements in d_in and d_aux, 4-byte ones in d_out
+ *            (2-byte ones with COAST_MM_OUT_BF16: C is then bfloat16, see below).
  *   GEMM_FP8 in : A, M x K FP8 E4M3 row-major; aux: B, K x N FP8 E4M3 row-major   out: C, M x N float.  E4M3 is the OCP
  *            encoding of torch.float8_e4m3fn: no infinities, S.1111.111 is NaN.  The products are exact; they are summed in
  *            the tensor core's accumulator, whose width for FP8 is not fp32's (DESIGN.md §6), then written as fp32.
@@ -176,7 +177,7 @@ typedef struct coast_fault_plan {
  *            fault site of width 32 and one fp32 vote, as GEMM_TF32.  The 8-bit wgmma reads B K-major only, so B is
  *            transposed into P*K*N bytes of scratch first; with COAST_MM_B_TRANSPOSED the caller's B^T is read in place.
  *            COAST_MM_BATCHED and COAST_MM_GROUPED as below; the element offsets count 1-byte elements in d_in and d_aux,
- *            4-byte ones in d_out.  With COAST_MM_SCALE_TENSOR or COAST_MM_SCALE_ROWWISE every replica multiplies its value
+ *            4-byte ones in d_out (2-byte ones with COAST_MM_OUT_BF16).  With COAST_MM_SCALE_TENSOR or COAST_MM_SCALE_ROWWISE every replica multiplies its value
  *            by the scales of A and B before the vote (see below).
  *   MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 with COAST_MM_B_TRANSPOSED: aux: B^T, N x K row-major per product (see below).
  *   QSORT    in : n_units x unit_bytes, arrays of L = unit_bytes/4 int32 (L <= 1024)   out: the sorted arrays
@@ -269,6 +270,23 @@ typedef struct coast_fault_plan {
  * d_scale_b + g_lo*N.  Tensorwise scales are passed unchanged. */
 #define COAST_MM_SCALE_TENSOR   0x100000u
 #define COAST_MM_SCALE_ROWWISE  0x200000u
+/* BF16 output (GEMM_BF16 and GEMM_FP8 only): with COAST_MM_OUT_BF16 in `mode`, C is bfloat16.  It
+ * combines with COAST_MM_BATCHED, COAST_MM_GROUPED and COAST_MM_B_TRANSPOSED.  C keeps its layout: row-major, the same element
+ * offsets as above (d_out + b*M*N, d_out + ro[g]*N, ...), now counting 2-byte elements.  Element (i, j) of replica r is
+ * x_r, the accumulator after the fault hook, rounded to bfloat16 to nearest even (cvt.rn; subnormals are kept, a NaN
+ * becomes 0x7FFF): v_r = bf16(x_r).  The vote, `fcmp oeq` on the
+ * widened values (+0 and -0 agree, NaN disagrees with everything), the select and majority voters (bitwise on the 16-bit
+ * patterns), the counters and d_status work on v_0 .. v_{NC-1} as they do on x_r without the bit: the rounding is part of the
+ * protected function, and what is voted is what is stored.  The fault sites are unchanged (one 32-bit site per element, on the
+ * accumulator), so a plan draws the same faults as for the fp32-output launch.  A flip that the rounding absorbs counts in
+ * `injected` but not in errors_corrected or dwc_detected, and leaves its d_status byte 0.  With at most one flip per unit (the
+ * plans above), the bf16 C of any launch equals the fp32 C of the same launch and plan rounded to nearest even, for every NC,
+ * voter and plan, except for the sign of a zero where TMR's select voter meets a sign flip on replica 0 of a value that rounds
+ * to zero (DESIGN.md §3.13).  COAST_ERR_BAD_ARG for the bit on any other kernel; COAST_ERR_UNSUPPORTED with a scale bit
+ * (scaled GEMM_FP8 writes fp32 C only, for now).  The alignment rules are unchanged.
+ * coast_run_host stages and downloads C at 2 bytes per element.  coast_out_bytes() does not see the mode and returns the fp32
+ * size (4); a caller sizes a bf16 C at 2 bytes per unit. */
+#define COAST_MM_OUT_BF16       0x400000u
 #define COAST_AES_DECRYPT       0x1u
 #define COAST_AES_KEY_PER_UNIT  0x2u
 #define COAST_AES_KEY_WRITEBACK 0x4u   /* with KEY_PER_UNIT: store what aes_enc_dec() leaves in key[] (TI_aes_128.c:214-221 mutates
@@ -376,7 +394,8 @@ int  coast_stats_reset(void* stream);
 uint32_t coast_fault_sites(uint32_t kernel, uint32_t unit_bytes, uint32_t K);
 uint32_t coast_fault_site_bits(uint32_t kernel, uint32_t unit_bytes, uint32_t K, uint32_t site);
 uint32_t coast_out_bytes_per_unit(uint32_t kernel);                      /* 0 for QSORT (variable) */
-uint32_t coast_out_bytes(uint32_t kernel, uint32_t unit_bytes);          /* QSORT: unit_bytes, the sorted array */
+uint32_t coast_out_bytes(uint32_t kernel, uint32_t unit_bytes);          /* QSORT: unit_bytes, the sorted array; the matmuls:
+                                                                            the fp32 C size, 4 (COAST_MM_OUT_BF16 C: 2) */
 uint32_t coast_votes_per_unit(uint32_t kernel);  /* sync points per unit at the SoR exit */
 
 /* --- thin memory helpers for pure-C callers (no torch) --------------- */
@@ -422,7 +441,7 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  * biased by ro[first] rows.  Scaled GEMM_FP8 (COAST_MM_SCALE_*) keeps the chunks of the unscaled call: tensorwise, the two
  * floats go up once; row-wise, row blocks send B's column scales once with B and each block its rows' A scales, batched chunks
  * the A rows and B columns of their products, grouped chunks A scales [ro[first], ro[end]) biased like d_in and B scales
- * [first*N, end*N).  On any failure every copy already queued on
+ * [first*N, end*N).  With COAST_MM_OUT_BF16 the same schedules move C at 2 bytes per element.  On any failure every copy already queued on
  * the caller's buffers is drained before the call returns. */
 int  coast_run_host(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
 /* What the last host call did: "staged", "hybrid" or "zerocopy"; unbatched matmuls: "row-blocks" or "one-shot"; grouped: "groups". */
