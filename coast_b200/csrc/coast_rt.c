@@ -409,8 +409,9 @@ static const struct kernel_info {
     [COAST_K_CHSTONE_AES] = { "chstone_aes", 64, 16, 64,            64, 0, 1 },
     [COAST_K_GEMM_BF16]   = { "gemm_bf16",   4,  1,  0,             0,  0, 0, 2 },
     [COAST_K_GEMM_FP8]    = { "gemm_fp8",    4,  1,  0,             0,  0, 0, 1 },
+    [COAST_K_GEMM_I8]     = { "gemm_i8",     4,  1,  0,             0,  0, 0, 1 },
 };
-/* an id with a row above; the ids between are unassigned (9) and unknown like those past the table */
+/* an id with a row above; the ids between are unassigned (9, 11) and unknown like those past the table */
 static int known_kernel(uint32_t kernel) { return kernel < COAST_K_COUNT_ && KINFO[kernel].name; }
 static int is_matmul(uint32_t kernel) { return known_kernel(kernel) && KINFO[kernel].mm_elem != 0; }
 
@@ -453,6 +454,7 @@ uint32_t coast_fault_sites(uint32_t kernel, uint32_t unit_bytes, uint32_t K) {
     case COAST_K_GEMM_TF32: return 1u;
     case COAST_K_GEMM_BF16: return 1u;
     case COAST_K_GEMM_FP8:  return 1u;
+    case COAST_K_GEMM_I8:   return 1u;
     case COAST_K_QSORT:     return 33u * (unit_bytes / 4u);
     case COAST_K_CHSTONE_SHA: return 421u * (unit_bytes / 64u + 1u);
     case COAST_K_CHSTONE_AES: return 176u;
@@ -511,7 +513,7 @@ typedef struct {
     uint64_t P;                   /* products: 1, the batch or G */
     uint64_t rows;                /* stacked rows of A and C: batch*M or R */
     int b_rows_k;                 /* B's map has K rows per product (GEMM_BF16 reading B in place); every B^T map has N (GEMM_FP8's
-                                     always: a B^T map over the pre-pass's scratch or the caller's B^T) */
+                                     and GEMM_I8's always: a B^T map over the pre-pass's scratch or the caller's B^T) */
     uint32_t b_rows;              /* rows per product of B's map */
     int scaled, rowwise;          /* GEMM_FP8 with COAST_MM_SCALE_TENSOR or COAST_MM_SCALE_ROWWISE; the latter */
 } mm_shape;
@@ -572,7 +574,7 @@ static int mm_bit_refused(const coast_launch_desc* d, uint32_t bit) {
     if (!(d->mode & bit) || is_matmul(d->kernel)) return COAST_OK;
     const char* what = bit == COAST_MM_BATCHED ? "COAST_MM_BATCHED: batched products exist"
                      : bit == COAST_MM_GROUPED ? "COAST_MM_GROUPED: grouped products exist" : "COAST_MM_B_TRANSPOSED: a transposed B exists";
-    return fail(COAST_ERR_BAD_ARG, "%s for MM_U32, GEMM_TF32 and GEMM_BF16 only, plus GEMM_FP8 (kernel %u)", what, d->kernel);
+    return fail(COAST_ERR_BAD_ARG, "%s for MM_U32, GEMM_TF32 and GEMM_BF16 only, plus GEMM_FP8 and GEMM_I8 (kernel %u)", what, d->kernel);
 }
 /* The scale bits (GEMM_FP8 only): one of the two, both scale pointers, d_scale_a 4-byte aligned and, row-wise, d_scale_b
  * 8-byte aligned (the kernels read a thread's two column scales as one float2) */
@@ -656,7 +658,7 @@ static uint64_t mm_row_tiles(const mm_shape* m, unsigned bm) { return m->rows / 
 /* A matmul kernel's name: stem, path variant, [_bt], [_grp], then _nc<n>_inj<i> for the kernels that came before batched,
  * grouped, BF16 and transposed-B launches and _inj<i>_nc<n> for the others.  GEMM_FP8's names are whole formats: one set of
  * kernels serves B and B^T, the narrow kernel exists at NC 1 only, and the grouped ones (always 128 x 128 tiles) carry no variant;
- * scaled GEMM_FP8 (xmr_scaled_fp8*) has the same set.  BF16 output (o16: 2-byte C elements) has a twin of each GEMM_BF16 and
+ * scaled GEMM_FP8 (xmr_scaled_fp8*) and GEMM_I8 (xmr_gemm_i8*) have the same set.  BF16 output (o16: 2-byte C elements) has a twin of each GEMM_BF16 and
  * GEMM_FP8 kernel, named xmr_o16_ + the name after its xmr_gemm_ prefix. */
 static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, int scaled, int o16, uint32_t nc, int inj) {
     if (o16) {
@@ -671,10 +673,11 @@ static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int
         snprintf(name, 64, f, inj, nc);
         return;
     }
-    if (kernel == COAST_K_GEMM_FP8) {
-        const char* f = grouped ? "xmr_gemm_fp8_grp_inj%d_nc%u" : *variant == 'p' ? "xmr_gemm_fp8p_inj%d_nc%u"
-                      : *variant == 'n' ? "xmr_gemm_fp8n_inj%d_nc1" : "xmr_gemm_fp8_inj%d_nc%u";
-        snprintf(name, 64, f, inj, nc);
+    if (kernel == COAST_K_GEMM_FP8 || kernel == COAST_K_GEMM_I8) {
+        static const char* const fmt[2][4] = {       /* [I8][grouped, pair, narrow, single] */
+            { "xmr_gemm_fp8_grp_inj%d_nc%u", "xmr_gemm_fp8p_inj%d_nc%u", "xmr_gemm_fp8n_inj%d_nc1", "xmr_gemm_fp8_inj%d_nc%u" },
+            { "xmr_gemm_i8_grp_inj%d_nc%u", "xmr_gemm_i8p_inj%d_nc%u", "xmr_gemm_i8n_inj%d_nc1", "xmr_gemm_i8_inj%d_nc%u" } };
+        snprintf(name, 64, fmt[kernel == COAST_K_GEMM_I8][grouped ? 0 : *variant == 'p' ? 1 : *variant == 'n' ? 2 : 3], inj, nc);
         return;
     }
     const char* stem = kernel == COAST_K_MM_U32 ? "xmr_mm_u32" : kernel == COAST_K_GEMM_BF16 ? "xmr_gemm_bf16" : "xmr_gemm_tf32";
@@ -683,7 +686,7 @@ static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int
     else snprintf(name, 64, "%s%s_nc%u_inj%d", stem, variant, nc, inj);
 }
 
-/* Pre-passes of the wgmma kernels: TF32 and FP8 wgmma read both operands K-major, so B (K x N, row-major) is transposed into
+/* Pre-passes of the wgmma kernels: TF32, FP8 and INT8 wgmma read both operands K-major, so B (K x N, row-major) is transposed into
  * scratch (4-byte or 1-byte elements);
  * the limb kernel splits A and B into u8 limb planes ([plane][rows][K] and, transposed, [plane][P N][K]).  The products' B
  * matrices become one stacked (P N) x K operand; their A matrices already are one matrix. */
@@ -982,15 +985,17 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     }
     case COAST_K_GEMM_TF32:
     case COAST_K_GEMM_BF16:
-    case COAST_K_GEMM_FP8: {
+    case COAST_K_GEMM_FP8:
+    case COAST_K_GEMM_I8: {
         /* one body for every operand type (xmr_gemm_tf32.cuh): fp32 operands read as TF32, B^T K-major from a transposing pre-pass
-         * into scratch; bfloat16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch); or E4M3 operands,
-         * 128-element k-blocks and, as for TF32, B^T K-major from a byte-transposing pre-pass */
-        const int bf16 = d->kernel == COAST_K_GEMM_BF16, fp8 = d->kernel == COAST_K_GEMM_FP8;
-        const char* TY = fp8 ? "FP8" : bf16 ? "BF16" : "TF32";
-        const unsigned bk = fp8 ? XMR_GEMM_FP8_BK : bf16 ? XMR_GEMM_BF16_BK : XMR_GEMM_BK;
-        const CUtensorMapDataType dt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                                                                 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+         * into scratch; bfloat16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch); or E4M3 or s8
+         * operands, 128-element k-blocks and, as for TF32, B^T K-major from a byte-transposing pre-pass */
+        const int bf16 = d->kernel == COAST_K_GEMM_BF16, i8 = d->kernel == COAST_K_GEMM_I8;
+        const int byte_ops = d->kernel == COAST_K_GEMM_FP8 || i8;          /* 1-byte operands: FP8 and I8 share their layout */
+        const char* TY = i8 ? "I8" : byte_ops ? "FP8" : bf16 ? "BF16" : "TF32";
+        const unsigned bk = byte_ops ? XMR_GEMM_FP8_BK : bf16 ? XMR_GEMM_BF16_BK : XMR_GEMM_BK;
+        const CUtensorMapDataType dt = byte_ops ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                                                      : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
         if (m.grouped && (d->N % xmr_gemm_bn(0) || d->K % bk))
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_%s grouped tiles are 128 x 128 x %u: N must be a multiple of 128 and K of %u "
                                                "(got %u, %u); the products' rows are free", TY, bk, bk, d->N, d->K);
@@ -1007,7 +1012,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         const char* e = getenv("COAST_GEMM_PAIR");
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
         const int pair = !m.grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
-        /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it, TF32 and FP8 only skip the transposing pre-pass */
+        /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it, TF32, FP8 and I8 only skip the transposing pre-pass */
         mm_kernel_name(L.name, d->kernel, pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt, m.grouped, m.scaled, m.ces == 2, nc, inj);
         { const char* g = getenv("COAST_GEMM_GROUP_M");
           if (g && atoi(g) > 0 && atoi(g) <= (int)XMR_MODE_GROUP_M_MASK) a.mode = (a.mode & ~XMR_MODE_GROUP_M_MASK) | (unsigned)atoi(g); }

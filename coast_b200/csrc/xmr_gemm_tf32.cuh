@@ -23,6 +23,8 @@
 // And FP8 operands (xmr_gemm_fp8*, operand type Fp8): E4M3 A and B, fp32 C, wgmma m64n128k32.  The 8-bit wgmma has no transpose
 // immediates, so B is read K-major only: as for TF32, a byte-transposing pre-pass (xmr_gemm_bt_u8) writes B^T into scratch, and
 // a caller's B^T (COAST_MM_B_TRANSPOSED) is read in place by the same kernels.
+// And INT8 operands (xmr_gemm_i8*, operand type I8): s8 A and B laid out as FP8's, wgmma m64n128k32 into s32 accumulators that
+// wrap, so C = A . B mod 2^32 exactly; the epilogue votes the int32 words with integer equality.
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, 64 rows of the 128-row tile each.
 // Persistent CTAs, one per SM.  Tiles: 128 x 256 unprotected (N % 256 == 0), 128 x 128 otherwise; the accumulators of a
 // replica are 64 x 128 wgmma fragments (64 fp32 registers per thread), so TMR holds 192 accumulator registers per thread.
@@ -177,6 +179,15 @@ __device__ __forceinline__ void wgmma_e4m3_m64n128k32(float (&d)[64], uint64_t d
         : "l"(da), "l"(db));
 }
 
+// D (+)= A . B^T with both operands K-major, s8 x s8 into s32 accumulators (no .satfinite: the sums wrap mod 2^32); D's fragment
+// layout as above
+__device__ __forceinline__ void wgmma_s8_m64n128k32(int32_t (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db));
+}
+
 // The operand types of gemm_body.  Both stage 128-byte k-blocks (BK elements) and step A's descriptor by 32 bytes (WG_K elements)
 // per wgmma; they differ in the instruction and in how B reaches shared memory:
 //   Tf32: B^T rows from the transposing pre-pass, K-major like A; TMA boxes of B_BOX rows of B^T at 128 bytes per row;
@@ -185,6 +196,7 @@ __device__ __forceinline__ void wgmma_e4m3_m64n128k32(float (&d)[64], uint64_t d
 //   Bf16T: the caller's B^T (COAST_MM_B_TRANSPOSED: N rows of K) read in place, K-major like A and like Tf32's B^T: the same
 //         boxes of B_BOX rows of 128 bytes (64 k), a k16 step is 32 bytes, and the wgmma's B transpose immediate is 0.
 struct Tf32 {
+    using Acc = float;
     static constexpr int BK = XMR_GEMM_BK, WG_K = 8;
     static constexpr bool B_IN_PLACE = false;
     static constexpr uint32_t B_KSTEP = 32 >> 4;                 // descriptor start field per wgmma k step
@@ -193,6 +205,7 @@ struct Tf32 {
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_tf32_m64n128k8(d, da, db); }
 };
 struct Bf16 {
+    using Acc = float;
     static constexpr int BK = XMR_GEMM_BF16_BK, WG_K = 16;
     static constexpr bool B_IN_PLACE = true;
     static constexpr uint32_t B_KSTEP = (WG_K * ROW_BYTES) >> 4;
@@ -201,6 +214,7 @@ struct Bf16 {
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_bf16_m64n128k16(d, da, db); }
 };
 struct Bf16T {
+    using Acc = float;
     static constexpr int BK = XMR_GEMM_BF16_BK, WG_K = 16;
     static constexpr bool B_IN_PLACE = false;
     static constexpr uint32_t B_KSTEP = 32 >> 4;
@@ -212,12 +226,24 @@ struct Bf16T {
 //        128-byte row, and a k32 step is 32 bytes, the same descriptor step as Tf32's.  The accumulator is the wgmma's own
 //        (DESIGN.md §6: for FP8 it is narrower than fp32), as with torch._scaled_mm(use_fast_accum=True).
 struct Fp8 {
+    using Acc = float;
     static constexpr int BK = XMR_GEMM_FP8_BK, WG_K = 32;
     static constexpr bool B_IN_PLACE = false;
     static constexpr uint32_t B_KSTEP = 32 >> 4;
     static constexpr __host__ __device__ int b_box(bool pair) { return (int)xmr_gemm_b_box(pair); }
     static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc(saddr); }
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_e4m3_m64n128k32(d, da, db); }
+};
+//   I8: s8 operands, laid out as Fp8's (the same k-blocks, descriptors, pre-pass and B^T boxes), into s32 accumulators that wrap:
+//       C = sum_k a_ik b_kj mod 2^32, exact for any K.  The epilogue votes them as integers (see epilogue).
+struct I8 {
+    using Acc = int32_t;
+    static constexpr int BK = XMR_GEMM_FP8_BK, WG_K = 32;
+    static constexpr bool B_IN_PLACE = false;
+    static constexpr uint32_t B_KSTEP = 32 >> 4;
+    static constexpr __host__ __device__ int b_box(bool pair) { return (int)xmr_gemm_b_box(pair); }
+    static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc(saddr); }
+    static __device__ __forceinline__ void mma(int32_t (&d)[64], uint64_t da, uint64_t db) { wgmma_s8_m64n128k32(d, da, db); }
 };
 
 __device__ __forceinline__ void wgmma_u8_m64n32k32(uint32_t (&d)[16], uint64_t da, uint64_t db) {
@@ -246,13 +272,22 @@ __device__ __forceinline__ void wgmma_u8_m64n64k32(uint32_t (&d)[32], uint64_t d
 // (after the fault hook) into one bf16x2 with cvt.rn, the vote and the tally run on the 16-bit halves (`fcmp oeq` on the widened
 // values, the majority voter bitwise on the pair), and one 4-byte store writes the voted pair.  Its own branch, so that the fp32
 // epilogue's code is not touched.
+// Integer accumulators (AccT int32_t, xmr_gemm_i8*; neither SCALED nor OUT_BF16): the vote is integer equality (`icmp eq`) on the
+// two's-complement words, with the select or the bitwise majority voter.  The fp32 vote would be wrong on them: `fcmp oeq` takes a
+// bit-31 flip of a zero C (0x80000000, -0.0) as equal to +0.0, and every C whose pattern is a NaN as a disagreement.  Its own
+// branch as well; C is written with the same 8-byte pair stores.
+template <class X, class Y> struct Same { static constexpr bool value = false; };
+template <class X> struct Same<X, X> { static constexpr bool value = true; };
 template <bool OUT_BF16> struct CElem { using T = float; };
 template <> struct CElem<true> { using T = uint16_t; };
-template <int NC, int NSUB, bool INJECT, bool GROUPED = false, bool SCALED = false, bool ROWWISE = false, bool OUT_BF16 = false>
-__device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float (&acc)[NC][NSUB][64], uint32_t row0, uint32_t n0, uint32_t nsub_t,
+template <int NC, int NSUB, bool INJECT, bool GROUPED = false, bool SCALED = false, bool ROWWISE = false, bool OUT_BF16 = false,
+          class AccT = float>
+__device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (&acc)[NC][NSUB][64], uint32_t row0, uint32_t n0, uint32_t nsub_t,
                                          bool hints, uint64_t pol_c, typename CElem<OUT_BF16>::T* c_grp = nullptr, uint32_t row_end = 0,
                                          const float* sa = nullptr, const float* sb = nullptr) {
     static_assert(!(SCALED && OUT_BF16), "scaled GEMM_FP8 has no bfloat16-output epilogue");
+    constexpr bool INT_ACC = !Same<AccT, float>::value;
+    static_assert(!INT_ACC || (Same<AccT, int32_t>::value && !SCALED && !OUT_BF16), "integer accumulators: s32, unscaled, 4-byte C");
     using CT = typename CElem<OUT_BF16>::T;
     const uint32_t flags = a.flags;
     const bool majority = flags & COAST_F_MAJORITY_VOTER;
@@ -282,7 +317,36 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, float 
                 const uint32_t row = row0 + 8 * h, col = n0 + sub * WG_N + 8 * j + 2 * (lane & 3);
                 if constexpr (GROUPED) { if (row >= row_end) continue; }
                 const unsigned long long local0 = (unsigned long long)row * a.N + col;
-                if constexpr (OUT_BF16) {
+                if constexpr (INT_ACC) {
+                    uint32_t o[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int i = 4 * j + 2 * h + e;
+                        uint32_t r0 = (uint32_t)acc[0][sub][i];
+                        uint32_t r1 = NC > 1 ? (uint32_t)acc[NC > 1 ? 1 : 0][sub][i] : r0;
+                        uint32_t r2 = NC > 2 ? (uint32_t)acc[NC > 2 ? 2 : 0][sub][i] : r0;
+                        if (INJECT) {
+                            Fault f = fault_for_unit(a, NC, local0 + e, [](uint32_t) { return 32u; });
+                            if (f.active) {
+                                tally.injected++;
+                                uint32_t mk = 1u << f.bit;
+                                if (f.replica == 0) r0 ^= mk; else if (f.replica == 1) r1 ^= mk; else r2 ^= mk;
+                            }
+                        }
+                        uint32_t vote = r0, bad = 0;
+                        if (NC == 2) bad = (r0 == r1) ? 0u : 1u;
+                        if (NC == 3) {
+                            const bool c01 = (r0 == r1), c02 = (r0 == r2);       // icmp eq
+                            vote = majority ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
+                            bad = (c01 && c02) ? 0u : 1u;
+                        }
+                        o[e] = vote;
+                        tally.unit_exit<NC>(bad, 1u, flags, a.unit_base + local0 + e);
+                    }
+                    CT* dst = C + local0;
+                    if (hints) st_v2_hint(dst, o[0], o[1], pol_c);
+                    else *reinterpret_cast<uint2*>(dst) = make_uint2(o[0], o[1]);
+                } else if constexpr (OUT_BF16) {
                     uint32_t x[3][2];                            // [replica][element]: the accumulators after the fault hook
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
@@ -471,7 +535,7 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
         const uint32_t a_off = (uint32_t)(wg - 1) * 64u * 128u;      // this warpgroup's 64 rows of the A tile
         const uint64_t pol_c = l2_policy_evict_first();
         Tally tally(a);
-        float acc[NC][NSUB][64];
+        typename OP::Acc acc[NC][NSUB][64];                 // fp32, or s32 for I8
         uint32_t it = 0;
         for (uint32_t tile = worker; tile < n_virtual; tile += n_workers) {
             uint32_t tm, n0, bn_t;
@@ -483,7 +547,7 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
 #pragma unroll
                 for (int sub = 0; sub < NSUB; ++sub)
 #pragma unroll
-                    for (int i = 0; i < 64; ++i) acc[r][sub][i] = 0.f;
+                    for (int i = 0; i < 64; ++i) acc[r][sub][i] = typename OP::Acc(0);
 #pragma unroll
             for (int r = 0; r < NC; ++r)
 #pragma unroll
@@ -707,6 +771,27 @@ XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj0_nc3, 3, 0, false)
 XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc1, 1, 1, false)
 XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc2, 2, 1, false)
 XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc3, 3, 1, false)
+// INT8 (s8) operands, s32 C: GEMM_FP8's variants and names, B^T K-major from the byte pre-pass or the caller; integer vote
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
+XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj0_nc1, 1, 0, false)
+XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj0_nc2, 2, 0, false)
+XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj0_nc3, 3, 0, false)
+XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj1_nc1, 1, 1, false)
+XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj1_nc2, 2, 1, false)
+XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj1_nc3, 3, 1, false)
 
 // Scaled FP8 (COAST_MM_SCALE_TENSOR / COAST_MM_SCALE_ROWWISE): the GEMM_FP8 variants with the scale pointers after the maps
 // (grouped: after ro and the group block); every replica multiplies its accumulator by the A and B scales before the vote

@@ -74,7 +74,9 @@ typedef enum coast_kernel_id {
     /* 9 is not assigned: coast_launch refuses it as an unknown kernel */
     COAST_K_GEMM_FP8  = 10, /* FP8 E4M3 in, fp32 out, wgmma e4m3; B^T read K-major (a byte-transposing pre-pass without
                                COAST_MM_B_TRANSPOSED) */
-    COAST_K_COUNT_    = 11
+    /* 11 is not assigned either */
+    COAST_K_GEMM_I8   = 12, /* int8 (s8) in, int32 out, exact mod 2^32, wgmma s8; B^T read K-major as for GEMM_FP8; integer vote */
+    COAST_K_COUNT_    = 13
 } coast_kernel_id;
 
 /* numClones of dataflowProtection::run: 3 = -TMR, 2 = -DWC, 1 = unprotected
@@ -179,7 +181,19 @@ typedef struct coast_fault_plan {
  *            COAST_MM_BATCHED and COAST_MM_GROUPED as below; the element offsets count 1-byte elements in d_in and d_aux,
  *            4-byte ones in d_out (2-byte ones with COAST_MM_OUT_BF16).  With COAST_MM_SCALE_TENSOR or COAST_MM_SCALE_ROWWISE every replica multiplies its value
  *            by the scales of A and B before the vote (see below).
- *   MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 with COAST_MM_B_TRANSPOSED: aux: B^T, N x K row-major per product (see below).
+ *   GEMM_I8  in : A, M x K int8 row-major; aux: B, K x N int8 row-major   out: C, M x N int32:
+ *            C[i][j] = sum_k a_ik * b_kj mod 2^32, as two's complement, for any K: the s32 accumulators have no .satfinite and
+ *            wrap.  This equals MM_U32 on the sign-extended operands, and torch._int_mm whenever no sum leaves int32 (always for
+ *            K < 2^17).  Shape and alignment rules, the B^T pre-pass and scratch, COAST_MM_BATCHED, COAST_MM_GROUPED and
+ *            COAST_MM_B_TRANSPOSED are GEMM_FP8's (element offsets: 1-byte elements in d_in and d_aux, 4-byte ones in d_out).
+ *            A unit is one C element with one fault site of width 32 (the s32 accumulator after the main loop) and one vote,
+ *            GEMM_TF32's geometry, so a plan draws the faults of a GEMM_FP8 launch of the same shape.  The vote is INTEGER
+ *            equality (`icmp eq`) with the select voter r0==r1 ? r0 : r2, or bitwise majority with COAST_F_MAJORITY_VOTER.
+ *            The fp32 vote would be wrong on these words: a bit-31 flip of a zero C gives 0x80000000, which `fcmp oeq` takes
+ *            for -0.0 == +0.0, so TMR's select voter would store INT_MIN silently and DWC would miss the flip; and every C in
+ *            [-8388607, -1] or [2139095041, 2147483647] is a NaN pattern, which `fcmp oeq` would count as a disagreement.
+ *            COAST_MM_SCALE_* and COAST_MM_OUT_BF16 are refused (COAST_ERR_BAD_ARG).
+ *   MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8 with COAST_MM_B_TRANSPOSED: aux: B^T, N x K row-major per product (see below).
  *   QSORT    in : n_units x unit_bytes, arrays of L = unit_bytes/4 int32 (L <= 1024)   out: the sorted arrays
  *   CHSTONE_SHA in : n_units x unit_bytes stream bytes (unit_bytes a multiple of 64, 64 <= unit_bytes < 2^29)
  *            out: n_units x 5 uint32 = sha_info_digest[5] (sha.h:38)
@@ -208,26 +222,26 @@ typedef struct coast_fault_plan {
  * SHA256, whose d_out is indexed by the shard's own units) and unit_base = lo.  COAST_QSORT_PATH=nested gives
  * COAST_ERR_UNSUPPORTED: a ragged batch runs the state-machine scheduling only. */
 #define COAST_UNIT_OFFSETS      0x10000u
-/* Batched matmuls (MM_U32, GEMM_TF32, GEMM_BF16 and GEMM_FP8 only): with COAST_MM_BATCHED in `mode`, M, N and K are the shape of ONE product and
+/* Batched matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8 and GEMM_I8 only): with COAST_MM_BATCHED in `mode`, M, N and K are the shape of ONE product and
  * n_units = batch x M x N.  d_in holds `batch` A matrices (M x K) end to end, d_aux `batch` B matrices (K x N) and d_out
  * receives `batch` C matrices (M x N), all dense and row-major.  The launch equals `batch` single launches, matrix b with
  * d_in + b*M*K, d_aux + b*K*N, d_out + b*M*N (elements) and unit_base + b*M*N: the same output bytes, summed counters and
  * minimum first_fault_unit.  Fault plans stay keyed by the global unit index (a TABLE plan has n_units entries), and the
  * in-loop store votes keep their meaning (K + 1 votes per unit on the plain kernel).  Each path's shape rules apply to the
- * per-matrix M, N and K; a TF32 / BF16 / FP8 CTA pair needs the per-matrix M to be a multiple of 256.  COAST_ERR_BAD_ARG for the bit on
+ * per-matrix M, N and K; a TF32 / BF16 / FP8 / I8 CTA pair needs the per-matrix M to be a multiple of 256.  COAST_ERR_BAD_ARG for the bit on
  * any other kernel, for n_units zero or not a multiple of M*N, and for batch*M or batch*N (GEMM_BF16 without COAST_MM_B_TRANSPOSED:
  * batch*K) at or above 2^31.  Without the
  * bit n_units must be M*N; with batch = 1 the launch is identical to an unbatched one.  A shard takes whole matrices
  * [b_lo, b_hi): the three pointers and unit_base offset as above, n_units = (b_hi - b_lo) x M x N. */
 #define COAST_MM_BATCHED        0x20000u
-/* Grouped matmuls (MM_U32, GEMM_TF32, GEMM_BF16 and GEMM_FP8 only): with COAST_MM_GROUPED in `mode`, M is the number of products G (at least 1) and N
+/* Grouped matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8 and GEMM_I8 only): with COAST_MM_GROUPED in `mode`, M is the number of products G (at least 1) and N
  * and K are shared by all of them.  d_rows points to G + 1 non-decreasing uint64_t row offsets ro[] (8-byte aligned; a device
  * pointer for coast_launch, a host pointer for coast_run_host): product g has M_g = ro[g+1] - ro[g] rows (zero is allowed),
  * its A at d_in + ro[g]*K, its B at d_aux + g*K*N and its C at d_out + ro[g]*N (elements); d_aux holds the G dense K x N
  * matrices end to end.  n_units = R*N with R = ro[G] - ro[0] the rows of all products.  The launch equals G single launches,
  * product g with M = M_g and unit_base + (ro[g] - ro[0])*N: the same output elements, summed counters, minimum
  * first_fault_unit and d_status bytes (coast_launch).  Fault plans stay keyed by the global unit index (a TABLE plan has n_units
- * entries); the sites are those of the kernel (K for MM_U32, 1 for GEMM_TF32, GEMM_BF16 and GEMM_FP8) and the in-loop store votes keep K + 1 votes per
+ * entries); the sites are those of the kernel (K for MM_U32, 1 for GEMM_TF32, GEMM_BF16, GEMM_FP8 and GEMM_I8) and the in-loop store votes keep K + 1 votes per
  * unit.  Each path's shape rules apply to N and K only: every M_g is allowed on every path.  The kernels clamp every offset to
  * [ro[0], ro[0] + R] and count a decreasing pair as zero rows, so a malformed table never reads or writes outside
  * [ro[0], ro[0] + R) rows of the buffers; coast_run_host (and Runtime.run) refuse a table that decreases or whose last offset is
@@ -237,13 +251,13 @@ typedef struct coast_fault_plan {
  * takes whole products [g_lo, g_hi): d_rows + g_lo with the same d_in and d_out, d_aux + g_lo*K*N, M = g_hi - g_lo,
  * n_units = (ro[g_hi] - ro[g_lo])*N and unit_base + (ro[g_lo] - ro[0])*N. */
 #define COAST_MM_GROUPED        0x40000u
-/* Transposed B (MM_U32, GEMM_TF32, GEMM_BF16 and GEMM_FP8 only), the layout of a linear layer's weight: with COAST_MM_B_TRANSPOSED in
+/* Transposed B (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8 and GEMM_I8 only), the layout of a linear layer's weight: with COAST_MM_B_TRANSPOSED in
  * `mode`, d_aux holds B^T, each product's B stored as N rows of K elements, row-major: element (k, n) of product p is at
  * d_aux[p*N*K + n*K + k].  It combines with COAST_MM_BATCHED and COAST_MM_GROUPED; the product offsets into d_aux (p*K*N
  * elements) and the shard rules stay as documented there.  The launch equals the same launch without the bit whose d_aux holds
  * every product's B = (B^T)^T: the same output bytes, summed counters, minimum first_fault_unit and d_status bytes.  Fault sites,
  * their widths, TABLE plans and the in-loop store votes are unchanged.  B^T is read in place: GEMM_TF32 runs no transposing
- * pre-pass and needs no B^T scratch, GEMM_BF16 reads B^T K-major, GEMM_FP8 runs no byte-transposing pre-pass and needs no
+ * pre-pass and needs no B^T scratch, GEMM_BF16 reads B^T K-major, GEMM_FP8 and GEMM_I8 run no byte-transposing pre-pass and need no
  * scratch (a grouped launch still allocates its group block), MM_U32's limb path splits B^T like A.  Each path's shape
  * rules are unchanged; the 2^31 bound on B's stacked rows is on batch*N (grouped: G*N) for every kernel with the bit.
  * COAST_ERR_BAD_ARG for the bit on any other kernel. */
@@ -302,7 +316,7 @@ typedef struct coast_launch_desc {
     uint64_t n_units;      /* units in THIS launch                                */
     uint64_t unit_base;    /* global index of this launch's unit 0 (fault plans)  */
     uint32_t unit_bytes;   /* CRC16/SHA256: message length of every unit          */
-    uint32_t M, N, K;      /* MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8           */
+    uint32_t M, N, K;      /* the matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8) */
     const void* d_in;
     void*       d_out;
     const void* d_aux;
@@ -427,7 +441,7 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  *     ONE launch reads the mapped host memory and writes the voted output straight back; the
  *     default when the output is at most 1/8 of the input (CRC16, CHSTONE_SHA);
  *   hybrid: the staged chunks' kernels read a pinned input in place, outputs are staged;
- *   matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8): B goes up once and C comes down in row blocks (one-shot: one
+ *   matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8): B goes up once and C comes down in row blocks (one-shot: one
  *     block for small or oddly shaped problems).
  * COAST_HOST_PATH=staged|hybrid|zerocopy forces a path, and for matmuls one-shot forces one block
  * (INTEGRATION.md §config).  Ragged calls (COAST_UNIT_OFFSETS, d_aux = host offsets, which must never
