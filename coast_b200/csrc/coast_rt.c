@@ -503,6 +503,24 @@ static int encode_map(const map_desc* want, CUdeviceptr scratch, int cached, CUt
     return COAST_OK;
 }
 
+/* One row per matmul operand type: what the GEMM launch and the kernel names need to know about it (MM_U32: its names only). */
+static const struct mm_op {
+    const char* ty;                         /* the type in messages: GEMM_<ty> */
+    const char* prefix, * stem;             /* kernel names: xmr_<prefix>_<stem>...; scaled and BF16-output GEMMs swap the prefix */
+    unsigned bk;                            /* elements per k-block (one 128-byte swizzle row) */
+    CUtensorMapDataType dt;                 /* A's and B's tensor-map element type */
+    int b_in_place;                         /* B (K x N) is read in place, MN-major: no transposing pre-pass, no scratch */
+    int bt_kernels;                         /* a caller's B^T has kernels of its own (_bt); else the same kernels read it */
+    int nc_first;                           /* _nc<n>_inj<i> on the kernels that are neither grouped nor _bt (they came first) */
+    int grp_variant;                        /* grouped kernels keep the path variant (the n of NC 1); else they carry none */
+} MM_OPS[COAST_K_COUNT_] = {
+    [COAST_K_MM_U32]    = { "U32",  "mm",   "u32",  0,                0,                                0, 1, 1, 1 },
+    [COAST_K_GEMM_TF32] = { "TF32", "gemm", "tf32", XMR_GEMM_BK,      CU_TENSOR_MAP_DATA_TYPE_FLOAT32,  0, 0, 1, 1 },
+    [COAST_K_GEMM_BF16] = { "BF16", "gemm", "bf16", XMR_GEMM_BF16_BK, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 1, 1, 0, 1 },
+    [COAST_K_GEMM_FP8]  = { "FP8",  "gemm", "fp8",  XMR_GEMM_FP8_BK,  CU_TENSOR_MAP_DATA_TYPE_UINT8,    0, 0, 0, 0 },
+    [COAST_K_GEMM_I8]   = { "I8",   "gemm", "i8",   XMR_GEMM_FP8_BK,  CU_TENSOR_MAP_DATA_TYPE_UINT8,    0, 0, 0, 0 },
+};
+
 /* The shape of a matmul launch, read off its descriptor once.  Batched (COAST_MM_BATCHED): the stacked A and C are one
  * (batch*M)-row matrix and only B changes from one product to the next.  Grouped (COAST_MM_GROUPED): M is the product count G,
  * the stacked A and C are one R-row matrix from row ro[0] (R = n_units / N) and B is G matrices end to end. */
@@ -619,7 +637,7 @@ static int mm_check(const coast_launch_desc* d, mm_shape* m) {
     m->batched = (d->mode & COAST_MM_BATCHED) != 0;
     m->grouped = (d->mode & COAST_MM_GROUPED) != 0;
     m->bt = (d->mode & COAST_MM_B_TRANSPOSED) != 0;
-    m->b_rows_k = d->kernel == COAST_K_GEMM_BF16 && !m->bt;
+    m->b_rows_k = MM_OPS[d->kernel].b_in_place && !m->bt;
     m->b_rows = m->b_rows_k ? d->K : d->N;
     const char bc = m->b_rows_k ? 'K' : 'N';
     m->P = 1; m->rows = d->M;
@@ -655,35 +673,16 @@ static int mm_check(const coast_launch_desc* d, mm_shape* m) {
 /* tiles of bm rows over the stacked rows; a grouped launch's products start anywhere, so it gets one more per product (a bound) */
 static uint64_t mm_row_tiles(const mm_shape* m, unsigned bm) { return m->rows / bm + (m->grouped ? m->P : 0); }
 
-/* A matmul kernel's name: stem, path variant, [_bt], [_grp], then _nc<n>_inj<i> for the kernels that came before batched,
- * grouped, BF16 and transposed-B launches and _inj<i>_nc<n> for the others.  GEMM_FP8's names are whole formats: one set of
- * kernels serves B and B^T, the narrow kernel exists at NC 1 only, and the grouped ones (always 128 x 128 tiles) carry no variant;
- * scaled GEMM_FP8 (xmr_scaled_fp8*) and GEMM_I8 (xmr_gemm_i8*) have the same set.  BF16 output (o16: 2-byte C elements) has a twin of each GEMM_BF16 and
- * GEMM_FP8 kernel, named xmr_o16_ + the name after its xmr_gemm_ prefix. */
+/* A matmul kernel's name: xmr_<prefix>_<stem><variant>[_bt][_grp], then _inj<i>_nc<n>, or _nc<n>_inj<i> where the row says so.
+ * The prefix is scaled for COAST_MM_SCALE_* and o16 for COAST_MM_OUT_BF16 (2-byte C elements); the variant is the path ("n",
+ * "p", "_tc", "_tiled" or ""). */
 static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, int scaled, int o16, uint32_t nc, int inj) {
-    if (o16) {
-        char twin[64];
-        mm_kernel_name(twin, kernel, variant, bt, grouped, scaled, 0, nc, inj);
-        snprintf(name, 64, "%.4so16_%s", twin, strchr(twin + 4, '_') + 1);    /* xmr_gemm_<rest> -> xmr_o16_<rest> */
-        return;
-    }
-    if (kernel == COAST_K_GEMM_FP8 && scaled) {
-        const char* f = grouped ? "xmr_scaled_fp8_grp_inj%d_nc%u" : *variant == 'p' ? "xmr_scaled_fp8p_inj%d_nc%u"
-                      : *variant == 'n' ? "xmr_scaled_fp8n_inj%d_nc1" : "xmr_scaled_fp8_inj%d_nc%u";
-        snprintf(name, 64, f, inj, nc);
-        return;
-    }
-    if (kernel == COAST_K_GEMM_FP8 || kernel == COAST_K_GEMM_I8) {
-        static const char* const fmt[2][4] = {       /* [I8][grouped, pair, narrow, single] */
-            { "xmr_gemm_fp8_grp_inj%d_nc%u", "xmr_gemm_fp8p_inj%d_nc%u", "xmr_gemm_fp8n_inj%d_nc1", "xmr_gemm_fp8_inj%d_nc%u" },
-            { "xmr_gemm_i8_grp_inj%d_nc%u", "xmr_gemm_i8p_inj%d_nc%u", "xmr_gemm_i8n_inj%d_nc1", "xmr_gemm_i8_inj%d_nc%u" } };
-        snprintf(name, 64, fmt[kernel == COAST_K_GEMM_I8][grouped ? 0 : *variant == 'p' ? 1 : *variant == 'n' ? 2 : 3], inj, nc);
-        return;
-    }
-    const char* stem = kernel == COAST_K_MM_U32 ? "xmr_mm_u32" : kernel == COAST_K_GEMM_BF16 ? "xmr_gemm_bf16" : "xmr_gemm_tf32";
-    if (bt || grouped || kernel == COAST_K_GEMM_BF16)
-        snprintf(name, 64, "%s%s%s%s_inj%d_nc%u", stem, variant, bt ? "_bt" : "", grouped ? "_grp" : "", inj, nc);
-    else snprintf(name, 64, "%s%s_nc%u_inj%d", stem, variant, nc, inj);
+    const struct mm_op* op = &MM_OPS[kernel];
+    bt = bt && op->bt_kernels;
+    const int ni = op->nc_first && !bt && !grouped;
+    snprintf(name, 64, "xmr_%s_%s%s%s%s_%s%u_%s%u", scaled ? "scaled" : o16 ? "o16" : op->prefix, op->stem,
+             grouped && !op->grp_variant ? "" : variant, bt ? "_bt" : "", grouped ? "_grp" : "", ni ? "nc" : "inj", ni ? nc : (unsigned)inj,
+             ni ? "inj" : "nc", ni ? (unsigned)inj : nc);
 }
 
 /* Pre-passes of the wgmma kernels: TF32, FP8 and INT8 wgmma read both operands K-major, so B (K x N, row-major) is transposed into
@@ -989,19 +988,15 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     case COAST_K_GEMM_I8: {
         /* one body for every operand type (xmr_gemm_tf32.cuh): fp32 operands read as TF32, B^T K-major from a transposing pre-pass
          * into scratch; bfloat16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch); or E4M3 or s8
-         * operands, 128-element k-blocks and, as for TF32, B^T K-major from a byte-transposing pre-pass */
-        const int bf16 = d->kernel == COAST_K_GEMM_BF16, i8 = d->kernel == COAST_K_GEMM_I8;
-        const int byte_ops = d->kernel == COAST_K_GEMM_FP8 || i8;          /* 1-byte operands: FP8 and I8 share their layout */
-        const char* TY = i8 ? "I8" : byte_ops ? "FP8" : bf16 ? "BF16" : "TF32";
-        const unsigned bk = byte_ops ? XMR_GEMM_FP8_BK : bf16 ? XMR_GEMM_BF16_BK : XMR_GEMM_BK;
-        const CUtensorMapDataType dt = byte_ops ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                                                                      : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+         * operands, 128-element k-blocks and, as for TF32, B^T K-major from a byte-transposing pre-pass (the type's MM_OPS row) */
+        const struct mm_op* op = &MM_OPS[d->kernel];
+        const unsigned bk = op->bk;
         if (m.grouped && (d->N % xmr_gemm_bn(0) || d->K % bk))
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_%s grouped tiles are 128 x 128 x %u: N must be a multiple of 128 and K of %u "
-                                               "(got %u, %u); the products' rows are free", TY, bk, bk, d->N, d->K);
+                                               "(got %u, %u); the products' rows are free", op->ty, bk, bk, d->N, d->K);
         if (!m.grouped && (d->M % XMR_WG_BM || d->N % xmr_gemm_bn(0) || d->K % bk))
             return fail(COAST_ERR_UNSUPPORTED, "GEMM_%s tiles are 128x128x%u: M,N must be multiples of 128 and K of %u (got %u,%u,%u)",
-                        TY, bk, bk, d->M, d->N, d->K);
+                        op->ty, bk, bk, d->M, d->N, d->K);
         if (!aligned16 || (((uintptr_t)d->d_aux) & 15u) || (((uintptr_t)d->d_out) & 15u)) return fail(COAST_ERR_BAD_ARG, "GEMM buffers must be 16-byte aligned");
         /* unprotected 128 x 256 tiles when N allows (wide), else 128 x 128.  CTA-pair kernels (cluster 2 x 1 x 1,
          * 256-row pair tiles, B multicast) are bit-identical to the single-CTA kernels.  Default: pairs for the unprotected and
@@ -1012,8 +1007,9 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         const char* e = getenv("COAST_GEMM_PAIR");
         const int want_pair = e && (!strcmp(e, "0") || !strcmp(e, "1")) ? e[0] == '1' : nc < 3;
         const int pair = !m.grouped && want_pair && d->M % (2u * XMR_WG_BM) == 0 && d->N % xmr_gemm_bn(nc == 1) == 0 && G.sm_count >= 2;
-        /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it, TF32, FP8 and I8 only skip the transposing pre-pass */
-        mm_kernel_name(L.name, d->kernel, pair ? "p" : nc == 1 && !wide ? "n" : "", bf16 && m.bt, m.grouped, m.scaled, m.ces == 2, nc, inj);
+        /* a caller's B^T is read in place, K-major: BF16 has kernels of its own for it (bt_kernels), TF32, FP8 and I8 only skip the
+         * transposing pre-pass */
+        mm_kernel_name(L.name, d->kernel, pair ? "p" : nc == 1 && !wide ? "n" : "", m.bt, m.grouped, m.scaled, m.ces == 2, nc, inj);
         { const char* g = getenv("COAST_GEMM_GROUP_M");
           if (g && atoi(g) > 0 && atoi(g) <= (int)XMR_MODE_GROUP_M_MASK) a.mode = (a.mode & ~XMR_MODE_GROUP_M_MASK) | (unsigned)atoi(g); }
         /* L2 eviction priorities: A evict_last, B and C evict_first; COAST_GEMM_L2_HINTS=0 loads and stores with the normal policy */
@@ -1025,7 +1021,7 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         L.ctas = mm_row_tiles(&m, XMR_WG_BM) * (d->N / xmr_gemm_bn(wide)); L.waves = 1; L.cluster = pair ? 2 : 1;
         L.grp_tm = XMR_WG_BM; L.grp_tiles_n = d->N / xmr_gemm_bn(wide);
         /* B^T of every product into scratch, unless the caller holds it (COAST_MM_B_TRANSPOSED) or BF16 reads B in place */
-        const int b_scratch = !bf16 && !m.bt;
+        const int b_scratch = !op->b_in_place && !m.bt;
         const uintptr_t b_base = b_scratch ? 0 : (uintptr_t)d->d_aux;
         if (b_scratch) {
             L.scratch = (size_t)m.P * d->K * d->N * m.es;
@@ -1035,11 +1031,11 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
         /* A: the stacked rows of d_in; for groups a placeholder of 128 rows that the scan rebases onto row ro[0] of d_in with R rows
          * (the host does not read the device table).  The placeholder is the B^T scratch, or without it d_aux: d_in of a host-call
          * chunk is biased by ro[first] rows and need not be an address of its own */
-        if (m.grouped) plan_wg_map(&L.map[0], dt, m.es, b_base, b_scratch, d->K, XMR_WG_BM, 1, XMR_WG_BM);
-        else plan_wg_map(&L.map[0], dt, m.es, (uintptr_t)d->d_in, 0, d->K, (uint32_t)m.rows, 1, XMR_WG_BM);
+        if (m.grouped) plan_wg_map(&L.map[0], op->dt, m.es, b_base, b_scratch, d->K, XMR_WG_BM, 1, XMR_WG_BM);
+        else plan_wg_map(&L.map[0], op->dt, m.es, (uintptr_t)d->d_in, 0, d->K, (uint32_t)m.rows, 1, XMR_WG_BM);
         /* B: the stacked B^T, (P N) rows of K, in scratch or the caller's; BF16 without COAST_MM_B_TRANSPOSED: the caller's B,
          * (P K) rows of N in boxes of 64 columns x 64 k-rows */
-        plan_wg_map(&L.map[1], dt, m.es, b_base, b_scratch, m.b_rows_k ? d->N : d->K, (uint32_t)(m.P * m.b_rows), 1,
+        plan_wg_map(&L.map[1], op->dt, m.es, b_base, b_scratch, m.b_rows_k ? d->N : d->K, (uint32_t)(m.P * m.b_rows), 1,
                     m.b_rows_k ? XMR_GEMM_BF16_BK : xmr_gemm_b_box(pair));
         break;
     }

@@ -260,6 +260,12 @@ __device__ __forceinline__ void wgmma_u8_m64n64k32(uint32_t (&d)[32], uint64_t d
         : "l"(da), "l"(db));
 }
 
+template <class X, class Y> struct Same { static constexpr bool value = false; };
+template <class X> struct Same<X, X> { static constexpr bool value = true; };
+template <bool OUT_BF16> struct CElem { using T = float; };
+template <> struct CElem<true> { using T = uint16_t; };
+__device__ __forceinline__ uint32_t acc_word(float x) { return __float_as_uint(x); }     // an accumulator's 32-bit word
+__device__ __forceinline__ uint32_t acc_word(int32_t x) { return (uint32_t)x; }
 // Epilogue of one consumer thread: vote the NC accumulators of its fragment element by element with the reference's select
 // voter / `fcmp oeq`, count, ONE store of the voted value.  Columns [n0 + 128 sub, ...) for sub < nsub_t.
 // GROUPED: C starts at row ro[0] (c_grp) and rows from row_end on belong to the next product: no vote, tally, flip or store.
@@ -270,16 +276,13 @@ __device__ __forceinline__ void wgmma_u8_m64n64k32(uint32_t (&d)[32], uint64_t d
 // of a scale (-noMemReplication's load rule), after the main loop, so nothing of it is live next to the accumulators.
 // OUT_BF16 (xmr_o16_*, COAST_MM_OUT_BF16; not with SCALED): C holds bfloat16.  Each replica rounds its thread's two values
 // (after the fault hook) into one bf16x2 with cvt.rn, the vote and the tally run on the 16-bit halves (`fcmp oeq` on the widened
-// values, the majority voter bitwise on the pair), and one 4-byte store writes the voted pair.  Its own branch, so that the fp32
-// epilogue's code is not touched.
+// values, the majority voter bitwise on the pair), and one 4-byte store writes the voted pair: its own branch, with its own pair vote.
 // Integer accumulators (AccT int32_t, xmr_gemm_i8*; neither SCALED nor OUT_BF16): the vote is integer equality (`icmp eq`) on the
 // two's-complement words, with the select or the bitwise majority voter.  The fp32 vote would be wrong on them: `fcmp oeq` takes a
-// bit-31 flip of a zero C (0x80000000, -0.0) as equal to +0.0, and every C whose pattern is a NaN as a disagreement.  Its own
-// branch as well; C is written with the same 8-byte pair stores.
-template <class X, class Y> struct Same { static constexpr bool value = false; };
-template <class X> struct Same<X, X> { static constexpr bool value = true; };
-template <bool OUT_BF16> struct CElem { using T = float; };
-template <> struct CElem<true> { using T = uint16_t; };
+// bit-31 flip of a zero C (0x80000000, -0.0) as equal to +0.0, and every C whose pattern is a NaN as a disagreement.  It shares
+// the fp32 branch -- word read, fault hook, vote and tally -- but for the compare; C is written with the same 8-byte pair stores.
+// The fault hook and the word reads stay written out in each branch: as inline helpers shared by the branches (over arrays,
+// over scalar references, with the vote or without), they changed the SASS of the TMR kernels (DESIGN.md §5.2).
 template <int NC, int NSUB, bool INJECT, bool GROUPED = false, bool SCALED = false, bool ROWWISE = false, bool OUT_BF16 = false,
           class AccT = float>
 __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (&acc)[NC][NSUB][64], uint32_t row0, uint32_t n0, uint32_t nsub_t,
@@ -317,36 +320,7 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (
                 const uint32_t row = row0 + 8 * h, col = n0 + sub * WG_N + 8 * j + 2 * (lane & 3);
                 if constexpr (GROUPED) { if (row >= row_end) continue; }
                 const unsigned long long local0 = (unsigned long long)row * a.N + col;
-                if constexpr (INT_ACC) {
-                    uint32_t o[2];
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int i = 4 * j + 2 * h + e;
-                        uint32_t r0 = (uint32_t)acc[0][sub][i];
-                        uint32_t r1 = NC > 1 ? (uint32_t)acc[NC > 1 ? 1 : 0][sub][i] : r0;
-                        uint32_t r2 = NC > 2 ? (uint32_t)acc[NC > 2 ? 2 : 0][sub][i] : r0;
-                        if (INJECT) {
-                            Fault f = fault_for_unit(a, NC, local0 + e, [](uint32_t) { return 32u; });
-                            if (f.active) {
-                                tally.injected++;
-                                uint32_t mk = 1u << f.bit;
-                                if (f.replica == 0) r0 ^= mk; else if (f.replica == 1) r1 ^= mk; else r2 ^= mk;
-                            }
-                        }
-                        uint32_t vote = r0, bad = 0;
-                        if (NC == 2) bad = (r0 == r1) ? 0u : 1u;
-                        if (NC == 3) {
-                            const bool c01 = (r0 == r1), c02 = (r0 == r2);       // icmp eq
-                            vote = majority ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
-                            bad = (c01 && c02) ? 0u : 1u;
-                        }
-                        o[e] = vote;
-                        tally.unit_exit<NC>(bad, 1u, flags, a.unit_base + local0 + e);
-                    }
-                    CT* dst = C + local0;
-                    if (hints) st_v2_hint(dst, o[0], o[1], pol_c);
-                    else *reinterpret_cast<uint2*>(dst) = make_uint2(o[0], o[1]);
-                } else if constexpr (OUT_BF16) {
+                if constexpr (OUT_BF16) {
                     uint32_t x[3][2];                            // [replica][element]: the accumulators after the fault hook
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
@@ -390,9 +364,9 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const int i = 4 * j + 2 * h + e;
-                        uint32_t r0 = __float_as_uint(acc[0][sub][i]);
-                        uint32_t r1 = NC > 1 ? __float_as_uint(acc[NC > 1 ? 1 : 0][sub][i]) : r0;
-                        uint32_t r2 = NC > 2 ? __float_as_uint(acc[NC > 2 ? 2 : 0][sub][i]) : r0;
+                        uint32_t r0 = acc_word(acc[0][sub][i]);
+                        uint32_t r1 = NC > 1 ? acc_word(acc[NC > 1 ? 1 : 0][sub][i]) : r0;
+                        uint32_t r2 = NC > 2 ? acc_word(acc[NC > 2 ? 2 : 0][sub][i]) : r0;
                         if (INJECT) {
                             Fault f = fault_for_unit(a, NC, local0 + e, [](uint32_t) { return 32u; });
                             if (f.active) {
@@ -409,16 +383,16 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (
                         }
                         const float f0 = __uint_as_float(r0), f1 = __uint_as_float(r1), f2 = __uint_as_float(r2);
                         uint32_t vote = r0, bad = 0;
-                        if (NC == 2) bad = (f0 == f1) ? 0u : 1u;
+                        if (NC == 2) bad = (INT_ACC ? r0 == r1 : f0 == f1) ? 0u : 1u;
                         if (NC == 3) {
-                            const bool c01 = (f0 == f1), c02 = (f0 == f2);       // fcmp oeq
+                            const bool c01 = INT_ACC ? r0 == r1 : f0 == f1, c02 = INT_ACC ? r0 == r2 : f0 == f2;   // icmp eq / fcmp oeq
                             vote = majority ? ((r0 & r1) | (r0 & r2) | (r1 & r2)) : (c01 ? r0 : r2);
                             bad = (c01 && c02) ? 0u : 1u;
                         }
                         o[e] = vote;
                         tally.unit_exit<NC>(bad, 1u, flags, a.unit_base + local0 + e);
                     }
-                    float* dst = C + local0;
+                    CT* dst = C + local0;
                     if (hints) st_v2_hint(dst, o[0], o[1], pol_c);
                     else *reinterpret_cast<uint2*>(dst) = make_uint2(o[0], o[1]);
                 }
@@ -582,36 +556,34 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
                     for (int sub = 0; sub < NSUB; ++sub) wg_fence_regs(acc[r][sub]);
                 if (t == 0) for (uint32_t c = 0; c < CTAS; ++c) mbar_arrive_rank(&empty[s], c);
             }
+            // the tile's first row and column for this thread, C's first row (grouped: ro[0], which also indexes the row-wise A
+            // scales), the rows it may write and its product (which places its row-wise B scales)
+            uint32_t row0, n_t, row_end = 0, prod = 0;
+            unsigned long long c_row = 0;
             if constexpr (GROUPED) {
                 // found here rather than before the main loop: nothing of it stays live next to the accumulators
                 const unsigned long long r0 = __ldg(ro);
                 const grp::Tile x = grp::tile_of(ro, r0, R, ts, n_grp, tiles_n, group_m, tile);
-                const uint32_t row0 = x.start + x.tm * TM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
-                using CT = typename CElem<OUT_BF16>::T;
-                if constexpr (SCALED) {                         // row-wise: rows are d_in's (from ro[0]), columns product x.g's
-                    if (a.mode & XMR_MODE_SCALE_ROWWISE)
-                        epilogue<NC, NSUB, INJECT, true, true, true, OUT_BF16>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
-                                                                     static_cast<CT*>(a.out) + r0 * a.N, x.end, sa + r0,
-                                                                     sb + (unsigned long long)x.g * a.N);
-                    else
-                        epilogue<NC, NSUB, INJECT, true, true, false, OUT_BF16>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
-                                                               static_cast<CT*>(a.out) + r0 * a.N, x.end, sa, sb);
-                } else {
-                    epilogue<NC, NSUB, INJECT, true, false, false, OUT_BF16>(a, tally, acc, row0, x.tn * BN, nsub_t, hints, pol_c,
-                                                                             static_cast<CT*>(a.out) + r0 * a.N, x.end);
-                }
+                row0 = x.start + x.tm * TM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
+                n_t = x.tn * BN;
+                c_row = r0;
+                row_end = x.end;
+                prod = x.g;
             } else {
-                const uint32_t row0 = tm * TM + rank * BM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
-                if constexpr (SCALED) {                         // row-wise: the stacked rows index sa, the tile's product sb
-                    if (a.mode & XMR_MODE_SCALE_ROWWISE)
-                        epilogue<NC, NSUB, INJECT, false, true, true, OUT_BF16>(a, tally, acc, row0, n0, nsub_t, hints, pol_c, nullptr, 0u, sa,
-                                                                      sb + (unsigned long long)((tm * TM) / a.M) * a.N);
-                    else
-                        epilogue<NC, NSUB, INJECT, false, true, false, OUT_BF16>(a, tally, acc, row0, n0, nsub_t, hints, pol_c, nullptr, 0u, sa, sb);
-                } else {
-                    epilogue<NC, NSUB, INJECT, false, false, false, OUT_BF16>(a, tally, acc, row0, n0, nsub_t, hints, pol_c);
-                }
+                row0 = tm * TM + rank * BM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
+                n_t = n0;
             }
+            using CT = typename CElem<OUT_BF16>::T;
+            CT* const c_grp = GROUPED ? static_cast<CT*>(a.out) + c_row * a.N : nullptr;
+            // the two scale layouts are two instances: one epilogue that chose at run time spilled (DESIGN.md §10 item 11).  The
+            // row-wise offsets are computed in the row-wise call only.
+            if (SCALED && (a.mode & XMR_MODE_SCALE_ROWWISE))
+                epilogue<NC, NSUB, INJECT, GROUPED, SCALED, true, OUT_BF16>(a, tally, acc, row0, n_t, nsub_t, hints, pol_c, c_grp, row_end,
+                                                                            sa + c_row,
+                                                                            sb + (unsigned long long)(GROUPED ? prod : (tm * TM) / a.M) * a.N);
+            else
+                epilogue<NC, NSUB, INJECT, GROUPED, SCALED, false, OUT_BF16>(a, tally, acc, row0, n_t, nsub_t, hints, pol_c, c_grp, row_end,
+                                                                             sa, sb);
         }
         tally.flush(a.counters);
     }
@@ -666,228 +638,74 @@ xmr_gemm_bt_u8(const uint8_t* __restrict__ B, uint8_t* __restrict__ Bt, unsigned
     }
 }
 
-#define XMR_GEMM_KERNEL(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER) XMR_GEMM_KERNEL_C(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER, false)
-#define XMR_GEMM_KERNEL_C(OP, NAME, NC, INJ, WIDE, PAIR, CLUSTER, O16)                                    \
-    extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                      \
-    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b) { \
-        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, PAIR, false, false, O16>(a, &map_a, &map_b);     \
-    }
+// ---- the entry points -------------------------------------------------------------------------------------------
+// XMR_GEMM_FAMILY(OP, SCALED, OUT_BF16, STEM, BT, ORDER, GN1, XP, XA) declares one family's 20 kernels on gemm_body<OP, ...>,
+// at inj 0 and 1 each (<i>):
+//   STEM BT <nc>            NC 1-3: 128 x 256 tiles at NC 1 (unprotected, N % 256 == 0), 128 x 128 at NC 2-3
+//   STEM n BT <nc1>         NC 1: 128 x 128 tiles (N a multiple of 128 but not of 256)
+//   STEM p BT <nc>          NC 1-3: CTA pairs (cluster 2 x 1 x 1), 256 x 256 (unprotected) / 256 x 128 pair tiles
+//   STEM GN1 BT _grp_inj<i>_nc1, STEM BT _grp_inj<i>_nc<2,3>
+//                           grouped (COAST_MM_GROUPED): single CTAs, 128 x 128 tiles; after the maps they take `ro`, the
+//                           caller's row offsets, and `grp`, the group block the pre-pass wrote (xmr_mm_grp.cuh)
+// <nc> is _inj<i>_nc<n> (ORDER IN) or, for TF32's kernels that came before the grouped ones, _nc<n>_inj<i> (ORDER NI).  BT is
+// _bt for BF16's B^T kernels, GN1 is the n that the grouped NC 1 kernels of TF32 and BF16 carry.  XP and XA are the extra
+// parameters after the maps (grouped: after ro and grp) and their arguments to gemm_body, each list opening with its comma:
+// () or, scaled, (, const float* sa, const float* sb) and (, sa, sb).  For example, FP8 is xmr_gemm_fp8_inj<i>_nc<1,2,3>,
+// xmr_gemm_fp8n_inj<i>_nc1, xmr_gemm_fp8p_inj<i>_nc<1,2,3> and xmr_gemm_fp8_grp_inj<i>_nc<1,2,3>; TF32 is
+// xmr_gemm_tf32{,p}_nc<1,2,3>_inj<i>, xmr_gemm_tf32n_nc1_inj<i>, xmr_gemm_tf32n_grp_inj<i>_nc1 and xmr_gemm_tf32_grp_inj<i>_nc<2,3>.
+#define XMR_LIST(...) __VA_ARGS__
+#define XMR_GEMM_NAME_IN(STEM, V, BT, NC, INJ) STEM##V##BT##_inj##INJ##_nc##NC
+#define XMR_GEMM_NAME_NI(STEM, V, BT, NC, INJ) STEM##V##BT##_nc##NC##_inj##INJ
+#define XMR_GEMM_NAME_GRP(STEM, V, BT, NC, INJ) STEM##V##BT##_grp_inj##INJ##_nc##NC
 #define XMR_NO_CLUSTER
 #define XMR_PAIR_CLUSTER __cluster_dims__(2, 1, 1)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc1_inj0, 1, 0, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc2_inj0, 2, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc3_inj0, 3, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc1_inj1, 1, 1, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc2_inj1, 2, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32_nc3_inj1, 3, 1, false, false, XMR_NO_CLUSTER)
-// unprotected, N a multiple of 128 but not of 256: 128 x 128 tiles
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32n_nc1_inj0, 1, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32n_nc1_inj1, 1, 1, false, false, XMR_NO_CLUSTER)
-// CTA pairs: 256 x 256 (unprotected) / 256 x 128 pair tiles
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc1_inj0, 1, 0, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc2_inj0, 2, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc3_inj0, 3, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc1_inj1, 1, 1, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc2_inj1, 2, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Tf32, xmr_gemm_tf32p_nc3_inj1, 3, 1, false, true, XMR_PAIR_CLUSTER)
-
-// grouped (COAST_MM_GROUPED): single CTAs and 128 x 128 tiles (tf32n unprotected); `ro` = the caller's row offsets, `grp` = the
-// group block the pre-pass wrote (xmr_mm_grp.cuh)
-#define XMR_GEMM_GRP_KERNEL(OP, NAME, NC, INJ, WIDE) XMR_GEMM_GRP_KERNEL_C(OP, NAME, NC, INJ, WIDE, false)
-#define XMR_GEMM_GRP_KERNEL_C(OP, NAME, NC, INJ, WIDE, O16)                                                \
-    extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
-    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, \
-         const unsigned long long* ro, const uint8_t* grp) {                                             \
-        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, false, true, false, O16>(a, &map_a, &map_b, ro, grp); \
+#define XMR_GEMM_ENTRY(NAME, CLUSTER, OP, NC, INJ, WIDE, PAIR, GROUPED, SCALED, OUT_BF16, PARAMS, ARGS)                      \
+    extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                                       \
+    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a,                                   \
+         const __grid_constant__ CUtensorMap map_b XMR_LIST PARAMS) {                                                     \
+        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, PAIR, GROUPED, SCALED, OUT_BF16>(a, &map_a, &map_b XMR_LIST ARGS); \
     }
-XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj0_nc2, 2, 0, false)
-XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj0_nc3, 3, 0, false)
-XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj1_nc2, 2, 1, false)
-XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32_grp_inj1_nc3, 3, 1, false)
-XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32n_grp_inj0_nc1, 1, 0, false)
-XMR_GEMM_GRP_KERNEL(Tf32, xmr_gemm_tf32n_grp_inj1_nc1, 1, 1, false)
+#define XMR_GEMM_ONE(V, NC, INJ, WIDE, PAIR, CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                         \
+    XMR_GEMM_ENTRY(XMR_GEMM_NAME_##ORDER(STEM, V, BT, NC, INJ), CLUSTER, OP, NC, INJ, WIDE, PAIR, false, SCALED, OUT_BF16, \
+                   XP, (, nullptr, nullptr XMR_LIST XA))
+#define XMR_GEMM_GRP(V, NC, INJ, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                   \
+    XMR_GEMM_ENTRY(XMR_GEMM_NAME_GRP(STEM, V, BT, NC, INJ), XMR_NO_CLUSTER, OP, NC, INJ, false, false, true, SCALED, OUT_BF16, \
+                   (, const unsigned long long* ro, const uint8_t* grp XMR_LIST XP), (, ro, grp XMR_LIST XA))
+#define XMR_GEMM_FAMILY(OP, SCALED, OUT_BF16, STEM, BT, ORDER, GN1, XP, XA)                                                \
+    XMR_GEMM_ONE(, 1, 0, true, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                      \
+    XMR_GEMM_ONE(, 2, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                     \
+    XMR_GEMM_ONE(, 3, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                     \
+    XMR_GEMM_ONE(, 1, 1, true, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                      \
+    XMR_GEMM_ONE(, 2, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                     \
+    XMR_GEMM_ONE(, 3, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                     \
+    XMR_GEMM_ONE(n, 1, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                    \
+    XMR_GEMM_ONE(n, 1, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                    \
+    XMR_GEMM_ONE(p, 1, 0, true, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                    \
+    XMR_GEMM_ONE(p, 2, 0, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                   \
+    XMR_GEMM_ONE(p, 3, 0, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                   \
+    XMR_GEMM_ONE(p, 1, 1, true, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                    \
+    XMR_GEMM_ONE(p, 2, 1, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                   \
+    XMR_GEMM_ONE(p, 3, 1, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                   \
+    XMR_GEMM_GRP(GN1, 1, 0, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                       \
+    XMR_GEMM_GRP(, 2, 0, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                          \
+    XMR_GEMM_GRP(, 3, 0, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                          \
+    XMR_GEMM_GRP(GN1, 1, 1, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                       \
+    XMR_GEMM_GRP(, 2, 1, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                          \
+    XMR_GEMM_GRP(, 3, 1, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)
 
-// BF16 operands: the same variants (wide / narrow / pair / grouped), B read in place; named _inj<i>_nc<n> like the grouped kernels
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16, xmr_gemm_bf16p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj0_nc2, 2, 0, false)
-XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj0_nc3, 3, 0, false)
-XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj1_nc2, 2, 1, false)
-XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16_grp_inj1_nc3, 3, 1, false)
-XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16n_grp_inj0_nc1, 1, 0, false)
-XMR_GEMM_GRP_KERNEL(Bf16, xmr_gemm_bf16n_grp_inj1_nc1, 1, 1, false)
-// BF16 with B^T read in place, K-major (COAST_MM_B_TRANSPOSED): the same variants
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16_bt_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16n_bt_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16n_bt_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Bf16T, xmr_gemm_bf16p_bt_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj0_nc2, 2, 0, false)
-XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj0_nc3, 3, 0, false)
-XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj1_nc2, 2, 1, false)
-XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16_bt_grp_inj1_nc3, 3, 1, false)
-XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16n_bt_grp_inj0_nc1, 1, 0, false)
-XMR_GEMM_GRP_KERNEL(Bf16T, xmr_gemm_bf16n_bt_grp_inj1_nc1, 1, 1, false)
-// FP8 (E4M3) operands: the variants of TF32, one set for B and B^T (B^T from the byte pre-pass or the caller); named
-// _inj<i>_nc<n>, the grouped nc1 kernel without the n (grouped tiles are always 128 x 128)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(Fp8, xmr_gemm_fp8p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj0_nc1, 1, 0, false)
-XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj0_nc2, 2, 0, false)
-XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj0_nc3, 3, 0, false)
-XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc1, 1, 1, false)
-XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc2, 2, 1, false)
-XMR_GEMM_GRP_KERNEL(Fp8, xmr_gemm_fp8_grp_inj1_nc3, 3, 1, false)
-// INT8 (s8) operands, s32 C: GEMM_FP8's variants and names, B^T K-major from the byte pre-pass or the caller; integer vote
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_KERNEL(I8, xmr_gemm_i8p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj0_nc1, 1, 0, false)
-XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj0_nc2, 2, 0, false)
-XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj0_nc3, 3, 0, false)
-XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj1_nc1, 1, 1, false)
-XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj1_nc2, 2, 1, false)
-XMR_GEMM_GRP_KERNEL(I8, xmr_gemm_i8_grp_inj1_nc3, 3, 1, false)
-
-// Scaled FP8 (COAST_MM_SCALE_TENSOR / COAST_MM_SCALE_ROWWISE): the GEMM_FP8 variants with the scale pointers after the maps
-// (grouped: after ro and the group block); every replica multiplies its accumulator by the A and B scales before the vote
-#define XMR_SCALED_KERNEL(NAME, NC, INJ, WIDE, PAIR, CLUSTER)                                                \
-    extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                      \
-    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, \
-         const float* sa, const float* sb) {                                                             \
-        xmr::gemm::gemm_body<xmr::gemm::Fp8, NC, INJ != 0, WIDE, PAIR, false, true>(a, &map_a, &map_b, nullptr, nullptr, sa, sb); \
-    }
-#define XMR_SCALED_GRP_KERNEL(NAME, NC, INJ)                                                                 \
-    extern "C" __global__ void __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                              \
-    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, \
-         const unsigned long long* ro, const uint8_t* grp, const float* sa, const float* sb) {           \
-        xmr::gemm::gemm_body<xmr::gemm::Fp8, NC, INJ != 0, false, false, true, true>(a, &map_a, &map_b, ro, grp, sa, sb); \
-    }
-XMR_SCALED_KERNEL(xmr_scaled_fp8_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_SCALED_KERNEL(xmr_scaled_fp8p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER)
-XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj0_nc1, 1, 0)
-XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj0_nc2, 2, 0)
-XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj0_nc3, 3, 0)
-XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc1, 1, 1)
-XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc2, 2, 1)
-XMR_SCALED_GRP_KERNEL(xmr_scaled_fp8_grp_inj1_nc3, 3, 1)
-
-// BF16 output (COAST_MM_OUT_BF16): every GEMM_BF16 and GEMM_FP8 variant once more, named xmr_o16_ + the name without its
+// fp32 C: TF32 (B^T from the transposing pre-pass or the caller), BF16 with B read in place and with B^T read in place, FP8
+// (E4M3; B^T from the byte pre-pass or the caller), INT8 (s8, s32 C, integer vote; FP8's layout)
+XMR_GEMM_FAMILY(Tf32, false, false, xmr_gemm_tf32, , NI, n, (), ())
+XMR_GEMM_FAMILY(Bf16, false, false, xmr_gemm_bf16, , IN, n, (), ())
+XMR_GEMM_FAMILY(Bf16T, false, false, xmr_gemm_bf16, _bt, IN, n, (), ())
+XMR_GEMM_FAMILY(Fp8, false, false, xmr_gemm_fp8, , IN, , (), ())
+XMR_GEMM_FAMILY(I8, false, false, xmr_gemm_i8, , IN, , (), ())
+// Scaled FP8 (COAST_MM_SCALE_TENSOR / COAST_MM_SCALE_ROWWISE): the scale pointers follow the maps (grouped: ro and grp); every
+// replica multiplies its accumulator by the A and B scales before the vote
+XMR_GEMM_FAMILY(Fp8, true, false, xmr_scaled_fp8, , IN, , (, const float* sa, const float* sb), (, sa, sb))
+// BF16 output (COAST_MM_OUT_BF16): every GEMM_BF16 and GEMM_FP8 kernel once more, named xmr_o16_ + the name without its
 // xmr_gemm_ prefix; C holds bfloat16, each replica rounds its values before the vote (see epilogue).  Scaled GEMM_FP8 has no
 // BF16-output set: its TMR and DWC kernels spilled 104-296 bytes with it (DESIGN.md §10 item 12)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16, xmr_o16_bf16p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16_grp_inj0_nc2, 2, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16_grp_inj0_nc3, 3, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16_grp_inj1_nc2, 2, 1, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16_grp_inj1_nc3, 3, 1, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16n_grp_inj0_nc1, 1, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16, xmr_o16_bf16n_grp_inj1_nc1, 1, 1, false, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16_bt_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16n_bt_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16n_bt_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Bf16T, xmr_o16_bf16p_bt_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16_bt_grp_inj0_nc2, 2, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16_bt_grp_inj0_nc3, 3, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16_bt_grp_inj1_nc2, 2, 1, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16_bt_grp_inj1_nc3, 3, 1, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16n_bt_grp_inj0_nc1, 1, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Bf16T, xmr_o16_bf16n_bt_grp_inj1_nc1, 1, 1, false, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj0_nc1, 1, 0, true, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj0_nc2, 2, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj0_nc3, 3, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj1_nc1, 1, 1, true, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj1_nc2, 2, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8_inj1_nc3, 3, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8n_inj0_nc1, 1, 0, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8n_inj1_nc1, 1, 1, false, false, XMR_NO_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj0_nc1, 1, 0, true, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj0_nc2, 2, 0, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj0_nc3, 3, 0, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj1_nc1, 1, 1, true, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj1_nc2, 2, 1, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_KERNEL_C(Fp8, xmr_o16_fp8p_inj1_nc3, 3, 1, false, true, XMR_PAIR_CLUSTER, true)
-XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj0_nc1, 1, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj0_nc2, 2, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj0_nc3, 3, 0, false, true)
-XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj1_nc1, 1, 1, false, true)
-XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj1_nc2, 2, 1, false, true)
-XMR_GEMM_GRP_KERNEL_C(Fp8, xmr_o16_fp8_grp_inj1_nc3, 3, 1, false, true)
+XMR_GEMM_FAMILY(Bf16, false, true, xmr_o16_bf16, , IN, n, (), ())
+XMR_GEMM_FAMILY(Bf16T, false, true, xmr_o16_bf16, _bt, IN, n, (), ())
+XMR_GEMM_FAMILY(Fp8, false, true, xmr_o16_fp8, , IN, , (), ())

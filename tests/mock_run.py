@@ -1,10 +1,12 @@
 """What every host-logic test shares: libcoast_rt.so runs in a child process (tests/mock_cuda/*_child.py) against the mock
 driver (tests/mock_cuda/mock_cuda.c, test infrastructure: it runs no workload, it records and bounds-checks driver calls),
 and the test reads back the child's results and the driver calls, one JSON event per line.  Kernel ids, mode bits and error
-codes are the runtime's own (coast_b200/runtime.py imports no torch at module level)."""
+codes are the runtime's own (coast_b200/runtime.py imports no torch at module level).  The cuobjdump readers of the embedded
+cubin are here too: its functions, each function's SASS and each function's resource usage."""
 import ctypes as C
 import json
 import os
+import re
 import subprocess
 import sys
 
@@ -14,14 +16,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 from coast_b200.runtime import (ERR_BAD_ARG as BAD_ARG, ERR_UNSUPPORTED as UNSUPPORTED, K_AES128, K_CHSTONE_AES,  # noqa: E402,F401
-                                K_CHSTONE_SHA, K_CRC16, K_GEMM_BF16, K_GEMM_FP8, K_GEMM_TF32, K_MM_U32, K_QSORT, K_SHA256,
-                                MM_B_TRANSPOSED, MM_BATCHED, MM_ELEM_BYTES, MM_GROUPED, UNIT_OFFSETS)
+                                K_CHSTONE_SHA, K_CRC16, K_GEMM_BF16, K_GEMM_FP8, K_GEMM_I8, K_GEMM_TF32, K_MM_U32, K_QSORT,
+                                K_SHA256, MM_B_TRANSPOSED, MM_BATCHED, MM_ELEM_BYTES, MM_GROUPED, MM_OUT_BF16, UNIT_OFFSETS)
 
 # every environment switch of libcoast_rt.so: a child starts with none of them, so only a test's env_extra sets one
 KNOBS = ("COAST_DEVICE", "COAST_GEMM_GROUP_M", "COAST_GEMM_L2_HINTS", "COAST_GEMM_PAIR", "COAST_GEMM_TAIL_SPLIT",
          "COAST_HOST_CHUNK_BYTES", "COAST_HOST_PATH", "COAST_MM_PATH", "COAST_NUMA_BIND", "COAST_OPT_PASSES", "COAST_QSORT_PATH",
          "COAST_REPORT_COUNTERS", "COAST_STRICT_FLAGS")
 SMS = 132                                                # the mock device's multiprocessor count
+CUBIN = os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")
 GRP_BYTES = lambda G: 128 + 4 * (G + 1)                  # noqa: E731  (xmr_mm_grp_bytes)
 
 
@@ -94,3 +97,24 @@ def scratch(ev, sizes):
 def spans(ev, op, base, size):
     """(host offset, bytes, stream, device offset) of every copy of kind op whose host side lies in [base, base + size)"""
     return [(e["host"] - base, e["bytes"], e["stream"], e["offset"]) for e in ev if e["op"] == op and base <= e["host"] < base + size]
+
+
+def cuobjdump(*args):
+    return subprocess.run(["cuobjdump", *args, CUBIN], capture_output=True, text=True).stdout
+
+
+def cubin_functions():
+    """the names of the cubin's xmr_* functions"""
+    return set(re.findall(r"\.text\.(xmr_\w+)", cuobjdump("-elf")))
+
+
+def sass_by_function():
+    """function name -> its SASS text"""
+    parts = re.split(r"\n\s*Function : (\S+)\n", cuobjdump("-sass"))
+    return dict(zip(parts[1::2], parts[2::2]))
+
+
+def res_usage():
+    """function name -> {REG, STACK, SHARED, LOCAL, ...}: the cuobjdump -res-usage line of every function"""
+    return {name: {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", body)}
+            for name, body in re.findall(r"Function (\S+):\s*\n\s*(REG:.*)", cuobjdump("-res-usage"))}

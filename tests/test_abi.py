@@ -31,38 +31,42 @@ def test_library_exports_everything_the_header_declares(built_lib):
 
 
 def test_sm90a_cubin_is_embedded(built_lib):
-    import subprocess
-    out = subprocess.run(["cuobjdump", "-lelf", os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")],
-                         capture_output=True, text=True).stdout
-    assert "sm_90a" in out
+    from mock_run import CUBIN, cuobjdump
+    assert "sm_90a" in cuobjdump("-lelf")
     blob = open(built_lib, "rb").read()
-    cubin = open(os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin"), "rb").read()
+    cubin = open(CUBIN, "rb").read()
     assert cubin[:4] == b"\x7fELF" and cubin in blob
 
 
-def test_every_non_matmul_kernel_name_format_is_in_the_cubin(built_lib):
-    """coast_rt.c builds kernel names with snprintf; a typo would only show up as a launch failure on a GPU box.  The matmul
-    kernels' names follow one rule from their stems (mm_kernel_name); tests/test_mm_plan_sweep.py launches every one of them."""
+def test_every_kernel_name_format_and_matmul_stem_is_in_the_cubin(built_lib):
+    """coast_rt.c builds kernel names with snprintf; a typo would only show up as a launch failure on a GPU box.  Every name
+    format of the non-matmul kernels expands to functions of the cubin.  The matmul kernels' names follow one rule
+    (mm_kernel_name) from the rows of MM_OPS: each row's xmr_<prefix>_<stem> starts functions of the cubin, as do the scaled
+    and bfloat16-output prefixes of the types that have them; tests/test_mm_plan_sweep.py launches every matmul function."""
     import itertools
-    import re
-    import subprocess
+    from mock_run import cubin_functions
     src = open(os.path.join(ROOT, "coast_b200", "csrc", "coast_rt.c")).read()
     fmts = set(re.findall(r'"(xmr_[A-Za-z0-9_%]+)"', src))
     stems = {"xmr_qsort", "xmr_qsortn", "xmr_aes128_enc", "xmr_aes128_dec", "xmr_aes128_enck", "xmr_aes128_deck",
              "xmr_chaes_enc", "xmr_chaes_dec"}               # stems of a "%s_nc%u_inj%d"
-    mm_stems = {"xmr_mm_u32", "xmr_gemm_tf32", "xmr_gemm_bf16"}
-    assert stems <= fmts and mm_stems <= fmts
-    fmts = (fmts - stems - mm_stems) | {s + "_nc%u_inj%d" for s in stems}
+    mm_rule = "xmr_%s_%s%s%s%s_%s%u_%s%u"                   # mm_kernel_name's one format
+    assert stems <= fmts and mm_rule in fmts
+    fmts = (fmts - stems - {mm_rule}) | {s + "_nc%u_inj%d" for s in stems}
     names = set()
     for f in fmts:
         opts = [["tc"] if tok == "%s" else ["1", "2", "3"] if tok == "%u" else ["0", "1"] for tok in re.findall(r"%[sud]", f)]
         for combo in itertools.product(*opts):
             it = iter(combo)
             names.add(re.sub(r"%[sud]", lambda m: next(it), f))
-    sass = subprocess.run(["cuobjdump", "-elf", os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")],
-                          capture_output=True, text=True).stdout
-    have = set(re.findall(r"\.text\.(xmr_\w+)", sass))
+    have = cubin_functions()
     assert len(names) > 100 and not (names - have), sorted(names - have)
+    rows = {k: (p, s) for k, p, s in re.findall(r'\[COAST_K_(\w+)\]\s*=\s*\{\s*"\w+",\s*"(\w+)",\s*"(\w+)"', src)}
+    assert rows == {"MM_U32": ("mm", "u32"), "GEMM_TF32": ("gemm", "tf32"), "GEMM_BF16": ("gemm", "bf16"),
+                    "GEMM_FP8": ("gemm", "fp8"), "GEMM_I8": ("gemm", "i8")}, rows
+    prefixes = {f"xmr_{p}_{s}" for p, s in rows.values()} | {"xmr_scaled_fp8", "xmr_o16_bf16", "xmr_o16_fp8"}
+    assert {"xmr_mm_u32", "xmr_gemm_tf32", "xmr_gemm_bf16"} <= prefixes
+    missing = sorted(p for p in prefixes if not any(f.startswith(p) for f in have))
+    assert not missing, missing
 
 
 @pytest.mark.parametrize("s,nc,fl", [
@@ -179,9 +183,8 @@ def test_flags_honoured_says_what_each_kernel_really_does(built_lib):
 
 
 def _sass(fun):
-    import subprocess
-    cubin = os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")
-    return subprocess.run(["cuobjdump", "-sass", "-fun", fun, cubin], capture_output=True, text=True, timeout=300).stdout
+    from mock_run import cuobjdump
+    return cuobjdump("-sass", "-fun", fun)
 
 
 def test_sass_carries_the_hopper_instructions_the_design_claims(built_lib):

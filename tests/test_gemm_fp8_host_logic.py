@@ -5,17 +5,14 @@ wide / narrow, CTA pair, grouped), grid and shared memory, both UINT8 tensor map
 every refusal with its message, that a batch of one is the unbatched launch, the bytes the host call copies per chunk (1-byte A
 and B, 4-byte C), that every xmr_gemm_fp8 function of the cubin runs the E4M3 wgmma, and that none keeps more stack than its
 TF32 or BF16 twin.  tests/test_mm_plan_sweep.py shows that each is reached."""
-import os
 import re
-import subprocess
 
 import pytest
 
-from mock_run import (BAD_ARG, GRP_BYTES, K_CRC16, K_GEMM_FP8, MM_B_TRANSPOSED as MM_BT, MM_BATCHED, MM_GROUPED, ROOT, SMS,  # noqa: F401
-                      UNSUPPORTED, arg0_ptr, args_of, maps, mock_dir, run, spans, work)
+from mock_run import (BAD_ARG, GRP_BYTES, K_CRC16, K_GEMM_FP8, MM_B_TRANSPOSED as MM_BT, MM_BATCHED, MM_GROUPED, SMS,  # noqa: F401
+                      UNSUPPORTED, arg0_ptr, args_of, maps, mock_dir, res_usage, run, sass_by_function, spans, work)
 
 SMEM = 6 * (128 * 128 + 128 * 128) + 1024 + 256          # xmr_gemm_smem: the same bytes wide and narrow
-CUBIN = os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")
 
 
 # (id, nc, M, N, K, batch or None, environment, kernel, grid)
@@ -217,12 +214,6 @@ def test_host_call_groups_per_chunk(mock_dir, tmp_path, pinned):
 
 
 # ------------------------------------------------------------------------------------------ the cubin's FP8 functions
-def sass_by_function():
-    sass = subprocess.run(["cuobjdump", "-sass", CUBIN], capture_output=True, text=True).stdout
-    parts = re.split(r"\n\s*Function : (\S+)\n", sass)
-    return dict(zip(parts[1::2], parts[2::2]))
-
-
 def test_fp8_functions_run_the_e4m3_wgmma_and_the_pre_pass_none(built_lib):
     sass = sass_by_function()
     fns = sorted(f for f in sass if f.startswith("xmr_gemm_fp8"))
@@ -245,10 +236,7 @@ def twins(f):
 def test_no_fp8_function_keeps_more_stack_than_its_twins(built_lib):
     """spills show as stack: an FP8 kernel holds the same 64-register accumulator fragments as BF16, so it may keep no more
     local memory than the TF32 or BF16 kernel of its variant"""
-    usage = subprocess.run(["cuobjdump", "-res-usage", CUBIN], capture_output=True, text=True).stdout
-    res = {}
-    for name, body in re.findall(r"Function (\S+):\s*\n\s*(REG:.*)", usage):
-        res[name] = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", body)}
+    res = res_usage()
     fns = sorted(f for f in res if f.startswith("xmr_gemm_fp8"))
     assert len(fns) == 20
     for f in fns:

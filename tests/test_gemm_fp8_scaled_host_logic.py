@@ -4,8 +4,8 @@ launch) through tests/mock_cuda/mm_scaled_child.py.  Pinned here: the xmr_scaled
 launch -- the pre-pass, grid, block, shared memory, tensor maps, scratch and argument block -- is the unscaled launch's; that the
 scale pointers are the last two parameters (after the maps, and for groups after ro and the group block) and reach the kernel
 unchanged; the internal row-wise mode bit and no caller scale bit in the argument block; every refusal; the scale bytes the host
-call copies per chunk for row blocks, whole products and groups, tensorwise and row-wise; that all 20 functions are reached; that
-they run the E4M3 wgmma; and that none keeps more stack than its unscaled twin."""
+call copies per chunk for row blocks, whole products and groups, tensorwise and row-wise; that the 20 functions run the E4M3
+wgmma; and that none keeps more stack than its unscaled twin.  That all 20 are reached is tests/test_mm_plan_sweep.py's."""
 import os
 import re
 import subprocess
@@ -13,11 +13,10 @@ import subprocess
 import pytest
 
 import mock_run
-from mock_run import BAD_ARG, K_CRC16, K_GEMM_BF16, K_GEMM_FP8, K_GEMM_TF32, ROOT, args_of, maps, run, spans
+from mock_run import BAD_ARG, K_CRC16, K_GEMM_BF16, K_GEMM_FP8, K_GEMM_TF32, ROOT, args_of, maps, res_usage, run, sass_by_function, spans
 from coast_b200.runtime import MM_SCALE_ROWWISE, MM_SCALE_TENSOR
 
 CHILD = "mm_scaled_child.py"
-CUBIN = os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")
 ROWWISE_BIT = 0x400                                       # XMR_MODE_SCALE_ROWWISE (coast_b200/csrc/xmr_args.h)
 RO = [3, 3, 100, 101, 101, 500, 700]
 
@@ -226,30 +225,7 @@ def test_host_call_groups(mock_dir, tmp_path, pinned, scale):
         assert k["sa"] + 4 * ro[f] == device_address(ev, c) and k["sb"] % 8 == 0, (f, e)
 
 
-# ------------------------------------------------------------------------------------------ every function, its SASS and its stack
-def test_every_scaled_function_is_reached(mock_dir, tmp_path):
-    launched = set()
-    shapes = [(512, 512, 128), (384, 512, 128), (512, 384, 128)]
-    for env in ({}, {"COAST_GEMM_PAIR": "0"}, {"COAST_GEMM_PAIR": "1"}):
-        ops = []
-        for nc in (1, 2, 3):
-            for p in (0, 0.3):
-                for scale in ("tensor", "row"):
-                    base = dict(op="launch", kernel=K_GEMM_FP8, nc=nc, p=p, scale=scale, unit_base=(1 << 32) - 5)
-                    ops += [dict(base, M=M, N=N, K=K) for M, N, K in shapes] + [dict(base, N=256, K=128, ro=RO)]
-        res, ev, _ = run(mock_dir, tmp_path, ops, child=CHILD, env_extra=env)
-        assert [r["err"] for r in res["ops"] if r["rc"]] == []
-        launched |= {e["name"] for e in work(ev) if e["name"].startswith("xmr_scaled")}
-    have = {f for f in sass_by_function() if f.startswith("xmr_scaled")}
-    assert len(have) == 20 and launched == have, (sorted(have - launched), sorted(launched - have))
-
-
-def sass_by_function():
-    sass = subprocess.run(["cuobjdump", "-sass", CUBIN], capture_output=True, text=True).stdout
-    parts = re.split(r"\n\s*Function : (\S+)\n", sass)
-    return dict(zip(parts[1::2], parts[2::2]))
-
-
+# ------------------------------------------------------------------------------------------ every function's SASS and stack
 def test_scaled_functions_run_the_e4m3_wgmma_and_round_to_nearest(built_lib):
     sass = sass_by_function()
     fns = sorted(f for f in sass if f.startswith("xmr_scaled_fp8"))
@@ -260,10 +236,7 @@ def test_scaled_functions_run_the_e4m3_wgmma_and_round_to_nearest(built_lib):
 
 
 def test_no_scaled_function_keeps_more_stack_than_its_twin(built_lib):
-    usage = subprocess.run(["cuobjdump", "-res-usage", CUBIN], capture_output=True, text=True).stdout
-    res = {}
-    for name, body in re.findall(r"Function (\S+):\s*\n\s*(REG:.*)", usage):
-        res[name] = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", body)}
+    res = res_usage()
     fns = sorted(f for f in res if f.startswith("xmr_scaled_fp8"))
     assert len(fns) == 20
     for f in fns:

@@ -3,21 +3,18 @@ tests/mock_cuda/mm_child.py, whose A and B buffers hold 1-byte elements.  GEMM_I
 here: over GEMM_FP8's plan space of tests/test_mm_plan_sweep.py (one product, a batch, groups, with and without B^T, NC 1-3 with
 and without a plan, every COAST_GEMM_PAIR setting), every GEMM_I8 launch makes exactly the driver calls of its GEMM_FP8 twin --
 grid, block, shared memory, UINT8 tensor maps, the byte-transposing pre-pass, scratch and argument block -- except for the kernel's
-name, xmr_gemm_i8 for xmr_gemm_fp8; so do coast_run_host calls, pinned or not; all twenty xmr_gemm_i8* functions are reached;
-scales, bfloat16 output and unassigned ids are refused with their messages; every xmr_gemm_i8* function runs the s8 wgmma and
-keeps the register, stack and local budget of its FP8 twin."""
-import os
+name, xmr_gemm_i8 for xmr_gemm_fp8; so do coast_run_host calls, pinned or not; scales, bfloat16 output and unassigned ids are
+refused with their messages; every xmr_gemm_i8* function runs the s8 wgmma and keeps the register, stack and local budget of its
+FP8 twin.  That all twenty xmr_gemm_i8* functions are reached is tests/test_mm_plan_sweep.py's."""
 import re
-import subprocess
 
 import pytest
 
-from mock_run import BAD_ARG, K_CRC16, K_GEMM_FP8, ROOT, SMS, args_of, maps, mock_dir, run, work  # noqa: F401
+from mock_run import BAD_ARG, K_CRC16, K_GEMM_FP8, SMS, args_of, maps, mock_dir, res_usage, run, sass_by_function, work  # noqa: F401
 from coast_b200.runtime import K_GEMM_I8, MM_OUT_BF16, MM_SCALE_ROWWISE, MM_SCALE_TENSOR
 from test_gemm_out_bf16_host_logic import mode_of, normalised
 from test_mm_plan_sweep import ENVS, RO, SHAPES
 
-CUBIN = os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")
 I8, FP8 = "xmr_gemm_i8", "xmr_gemm_fp8"
 
 
@@ -69,11 +66,6 @@ def sweep_ops():
     return ops
 
 
-def cubin_functions():
-    elf = subprocess.run(["cuobjdump", "-elf", CUBIN], capture_output=True, text=True).stdout
-    return set(re.findall(r"\.text\.(xmr_\w+)", elf))
-
-
 @pytest.mark.parametrize("env", ENVS, ids=["default", "mm_tiled", "mm_naive", "pair0", "pair1"])
 def test_every_launch_is_its_fp8_twin_but_for_the_name(mock_dir, tmp_path, env):
     ops = sweep_ops()
@@ -85,18 +77,6 @@ def test_every_launch_is_its_fp8_twin_but_for_the_name(mock_dir, tmp_path, env):
     assert len(names1) == len(ops) and [twin(n) for n in names1] == names0
     assert not [e for e in work(ev1) if e["name"].startswith(FP8)]
     assert compared(renamed(ev1)) == compared(ev0)
-
-
-def test_every_i8_function_is_reached_and_no_name_is_missing(mock_dir, tmp_path):
-    launched = set()
-    for env in ENVS:
-        res, ev, _ = run(mock_dir, tmp_path, as_i8(sweep_ops()), env_extra=env)
-        assert [r["err"] for r in res["ops"] if r["rc"]] == []               # a name missing from the cubin is a mock error
-        launched |= {e["name"] for e in work(ev) if e["name"].startswith(I8)}
-    functions = cubin_functions()
-    have = {f for f in functions if f.startswith(I8)}
-    assert len(have) == 20 and launched == have, (sorted(have - launched), sorted(launched - have))
-    assert all(twin(f) in functions for f in have)
 
 
 # (id, op): row blocks, one shot, whole products per chunk (B and B^T), groups per chunk
@@ -172,12 +152,6 @@ def test_store_vote_flags_warn_with_the_kernel_name(mock_dir, tmp_path):
 
 
 # ------------------------------------------------------------------------------------------ SASS and resources
-def sass_by_function():
-    sass = subprocess.run(["cuobjdump", "-sass", CUBIN], capture_output=True, text=True).stdout
-    parts = re.split(r"\n\s*Function : (\S+)\n", sass)
-    return dict(zip(parts[1::2], parts[2::2]))
-
-
 def test_every_i8_function_runs_the_s8_wgmma(built_lib):
     sass = sass_by_function()
     fns = sorted(f for f in sass if f.startswith(I8))
@@ -190,10 +164,7 @@ def test_every_i8_function_runs_the_s8_wgmma(built_lib):
 def test_every_i8_function_keeps_the_budget_of_its_fp8_twin(built_lib):
     """168 registers, as every wgmma GEMM kernel (the s32 accumulators take the registers fp32 ones do), and no more stack or
     local memory than the FP8 kernel of the same variant, NC and injection"""
-    usage = subprocess.run(["cuobjdump", "-res-usage", CUBIN], capture_output=True, text=True).stdout
-    res = {}
-    for name, body in re.findall(r"Function (\S+):\s*\n\s*(REG:.*)", usage):
-        res[name] = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", body)}
+    res = res_usage()
     fns = sorted(f for f in res if f.startswith(I8))
     assert len(fns) == 20
     for f in fns:

@@ -13,7 +13,7 @@ import sys
 import pytest
 
 from mock_run import (ROOT, XmrArgs, K_AES128, K_CHSTONE_SHA, K_CRC16, K_GEMM_TF32, K_MM_U32, K_QSORT, K_SHA256, args_of,  # noqa: F401
-                      mock_dir, run)
+                      cuobjdump, mock_dir, run)
 
 
 def test_argument_block_mirror_matches_the_header():
@@ -182,8 +182,7 @@ def test_tf32_gemm_kernel_selection_pairs_and_single(mock_dir, tmp_path, nc, M, 
 
 def _declared_bounds():
     """{kernel: (EIATTR_MAX_THREADS, EIATTR_CTA_PER_CLUSTER)} of the built cubin: its __launch_bounds__ and __cluster_dims__"""
-    elf = subprocess.run(["cuobjdump", "-elf", os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")],
-                         capture_output=True, text=True, check=True).stdout
+    elf = cuobjdump("-elf")
     bounds = {}
     for sec in re.split(r"^(?=\.)", elf, flags=re.M):
         m = re.match(r"\.nv\.info\.(xmr_\w+)", sec)

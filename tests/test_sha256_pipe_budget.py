@@ -4,7 +4,6 @@ The segmented kernel is bound by ALU-pipe issue.  Its round and schedule additio
 in the constant bank; a ptxas upgrade or a source change that folds them back into IADD3 would quietly give that back, so
 the SASS of the embedded cubin is held to a budget here."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -13,8 +12,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import sha_pipe_rates as spr  # noqa: E402
-
-CUBIN = os.path.join(ROOT, "coast_b200", "csrc", "coast_kernels.cubin")
+from mock_run import CUBIN, res_usage  # noqa: E402
 
 # whole-function SASS counts (the tile loop is nearly all of them): ALU-pipe instructions at most, IMAD-pipe at least.
 # With every addition on the ALU pipe the fault-free kernel issued 2235 ALU and 234 IMAD instructions, the injecting one
@@ -39,12 +37,10 @@ def test_segmented_kernel_keeps_its_pipe_split(built_lib, fun):
 
 @pytest.mark.parametrize("fun", sorted(BUDGET))
 def test_segmented_kernel_has_no_local_memory(built_lib, fun):
-    cuobjdump = os.path.join(os.path.dirname(spr.nvcc()), "cuobjdump")
-    out = subprocess.run([cuobjdump, "-res-usage", "-fun", fun, CUBIN], capture_output=True, text=True, check=True).stdout
-    fields = dict(kv.split(":", 1) for kv in out.split(fun + ":")[1].split() if ":" in kv)
-    assert int(fields["STACK"]) == 0 and int(fields["LOCAL"]) == 0, fields
+    fields = res_usage()[fun]
+    assert fields["STACK"] == 0 and fields["LOCAL"] == 0, fields
     if fun.endswith("inj0"):
-        assert int(fields["REG"]) <= MAX_REGS_INJ0, fields
+        assert fields["REG"] <= MAX_REGS_INJ0, fields
     assert not [op for _, op, _ in spr.sass_ops(CUBIN, fun) if op.startswith(("LDL", "STL"))]
 
 

@@ -6,7 +6,8 @@ so that two builds of libcoast_rt.so can be compared with diff:
 The sweep is tests/test_mm_plan_sweep.py's, plus refusals (zero dimensions, n_units off the shape, the 2^31 row bounds,
 misaligned or null buffers and row offsets, too many groups, combined mode bits, store votes) and host calls (pageable and
 pinned buffers, several chunks, COAST_HOST_PATH=one-shot).  It runs <checkout>/coast_b200/libcoast_rt.so against this tree's
-mock driver (tests/mock_cuda/mock_cuda.c) through tests/mock_cuda/mm_child.py, one op per init, with a marker in the log between ops.  Pointers are made
+mock driver (tests/mock_cuda/mock_cuda.c) through tests/mock_cuda/mm_child.py (scaled ops: mm_scaled_child.py), one op per init,
+with a marker in the log between ops, CHUNK_OPS ops per child process.  Pointers are made
 comparable across processes: an 8-byte word of an argument block, a tensor-map base or a copy's device side that points into
 a live allocation becomes a<id>+<offset>, a host-call chunk's biased d_in / d_out an offset from the slot buffer it is copied
 through, and a pageable host address an offset into the op's buffers.  After each op its rc, error text and coast_last_host_path()."""
@@ -22,10 +23,11 @@ import tempfile
 HERE = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(HERE, "tests"))
 import test_mm_plan_sweep as S  # noqa: E402
-from mock_run import (KNOBS, K_CRC16, K_GEMM_BF16, K_GEMM_FP8, K_GEMM_TF32, K_MM_U32, K_SHA256, MM_B_TRANSPOSED as BT,  # noqa: E402
-                      MM_BATCHED as BATCHED, MM_GROUPED as GROUPED, UNIT_OFFSETS)
+from mock_run import (KNOBS, K_CRC16, K_GEMM_BF16, K_GEMM_FP8, K_GEMM_I8, K_GEMM_TF32, K_MM_U32, K_SHA256,  # noqa: E402
+                      MM_B_TRANSPOSED as BT, MM_BATCHED as BATCHED, MM_GROUPED as GROUPED, UNIT_OFFSETS)
 
-MM = (K_MM_U32, K_GEMM_TF32, K_GEMM_BF16, K_GEMM_FP8)
+MM = (K_MM_U32, K_GEMM_TF32, K_GEMM_BF16, K_GEMM_FP8, K_GEMM_I8)
+CHUNK_OPS = 128                  # ops per child process: the mock driver keeps at most 4096 allocation records per process
 
 
 def edge_ops():
@@ -70,24 +72,26 @@ def edge_ops():
             ({"COAST_HOST_PATH": "one-shot"}, host)]
 
 
-def child(root, ops):
-    """runs each op as its own init .. shutdown of root's library, a marker line in the mock's log before it"""
+def child(root, ops, start):
+    """runs each op as its own init .. shutdown of root's library, a marker line with its index (from start) in the mock's log
+    before it"""
     sys.path.insert(0, os.path.join(HERE, "tests", "mock_cuda"))
     import mm_child
+    import mm_scaled_child
     mm_child.R.lib_path = lambda: os.path.join(root, "coast_b200", "libcoast_rt.so")
     results = []
     for i, op in enumerate(ops):
         with open(os.environ["MOCK_CUDA_LOG"], "a") as f:
-            f.write(json.dumps({"op": "begin", "index": i}) + "\n")
+            f.write(json.dumps({"op": "begin", "index": start + i}) + "\n")
         sys.argv = ["mm_child.py", json.dumps({"ops": [op]})]
         buf = io.StringIO()
         with contextlib.redirect_stdout(buf):
-            mm_child.main()
+            (mm_scaled_child if S.child_of(op) == "mm_scaled_child.py" else mm_child).main()
         results.append(json.loads(buf.getvalue().strip().splitlines()[-1])["ops"][0])
     print(json.dumps(results))
 
 
-def normalise(events, results):
+def normalise(events, results, start):
     live = {}                                                       # id -> (base, bytes)
     lines, op = [], -1
 
@@ -125,8 +129,8 @@ def normalise(events, results):
         if kind == "begin":
             if op >= 0:
                 lines.append("result " + json.dumps({k: results[op].get(k) for k in ("rc", "err", "path")}))
-            op = e["index"]
-            lines.append(f"op {op}")
+            op = e["index"] - start
+            lines.append(f"op {e['index']}")
         elif kind == "alloc":
             live[e["id"]] = (e["ptr"], e["bytes"])
             lines.append(f"alloc a{e['id']} {e['bytes']} host={e['host']}")
@@ -152,33 +156,38 @@ def normalise(events, results):
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--root", required=True, help="checkout whose coast_b200/libcoast_rt.so is traced")
-    ap.add_argument("--child", help=argparse.SUPPRESS)
+    ap.add_argument("--child", help=argparse.SUPPRESS)          # a JSON file: the first op's index and the ops
     a = ap.parse_args()
     if a.child:
-        return child(a.root, json.loads(a.child))
+        job = json.load(open(a.child))
+        return child(a.root, job["ops"], job["start"])
     root = os.path.abspath(a.root)
     n_ops = n_events = 0
     with tempfile.TemporaryDirectory() as tmp:
         subprocess.run(["gcc", "-O1", "-shared", "-fPIC", "-Wall", "-I/usr/local/cuda/include", "-o", os.path.join(tmp, "libcuda.so.1"),
                         os.path.join(HERE, "tests", "mock_cuda", "mock_cuda.c")], check=True)
-        log = os.path.join(tmp, "mock.log")
-        for env_extra, ops in S.SWEEP + edge_ops():
-            if os.path.exists(log):
-                os.unlink(log)
+        log, ops_file = os.path.join(tmp, "mock.log"), os.path.join(tmp, "ops.json")
+        for env_extra, all_ops in S.SWEEP + edge_ops():
+            print("env " + json.dumps(env_extra, sort_keys=True))
             env = dict(os.environ, LD_LIBRARY_PATH=f"{tmp}:" + os.environ.get("LD_LIBRARY_PATH", ""), MOCK_CUDA_LOG=log)
             for k in KNOBS:
                 env.pop(k, None)
             env.update(env_extra)
-            res = subprocess.run([sys.executable, os.path.abspath(__file__), "--root", root, "--child", json.dumps(ops)],
-                                 capture_output=True, text=True, env=env, timeout=3600)
-            if res.returncode:
-                sys.exit(res.stdout + res.stderr)
-            events = [json.loads(ln) for ln in open(log)]
-            print("env " + json.dumps(env_extra, sort_keys=True))
-            for ln in normalise(events, json.loads(res.stdout.strip().splitlines()[-1])):
-                print(ln)
-            n_ops += len(ops)
-            n_events += sum(e["op"] != "begin" for e in events)
+            for start in range(0, len(all_ops), CHUNK_OPS):
+                ops = all_ops[start:start + CHUNK_OPS]
+                if os.path.exists(log):
+                    os.unlink(log)
+                with open(ops_file, "w") as f:
+                    json.dump({"start": start, "ops": ops}, f)
+                res = subprocess.run([sys.executable, os.path.abspath(__file__), "--root", root, "--child", ops_file],
+                                     capture_output=True, text=True, env=env, timeout=3600)
+                if res.returncode:
+                    sys.exit(res.stdout + res.stderr)
+                events = [json.loads(ln) for ln in open(log)]
+                for ln in normalise(events, json.loads(res.stdout.strip().splitlines()[-1]), start):
+                    print(ln)
+                n_ops += len(ops)
+                n_events += sum(e["op"] != "begin" for e in events)
     print(f"{n_ops} ops, {n_events} events", file=sys.stderr)
 
 
