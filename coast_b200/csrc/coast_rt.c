@@ -410,8 +410,9 @@ static const struct kernel_info {
     [COAST_K_GEMM_BF16]   = { "gemm_bf16",   4,  1,  0,             0,  0, 0, 2 },
     [COAST_K_GEMM_FP8]    = { "gemm_fp8",    4,  1,  0,             0,  0, 0, 1 },
     [COAST_K_GEMM_I8]     = { "gemm_i8",     4,  1,  0,             0,  0, 0, 1 },
+    [COAST_K_GEMM_F16]    = { "gemm_f16",    4,  1,  0,             0,  0, 0, 2 },
 };
-/* an id with a row above; the ids between are unassigned (9, 11) and unknown like those past the table */
+/* an id with a row above; the ids between are unassigned (9, 11, 13) and unknown like those past the table */
 static int known_kernel(uint32_t kernel) { return kernel < COAST_K_COUNT_ && KINFO[kernel].name; }
 static int is_matmul(uint32_t kernel) { return known_kernel(kernel) && KINFO[kernel].mm_elem != 0; }
 
@@ -455,6 +456,7 @@ uint32_t coast_fault_sites(uint32_t kernel, uint32_t unit_bytes, uint32_t K) {
     case COAST_K_GEMM_BF16: return 1u;
     case COAST_K_GEMM_FP8:  return 1u;
     case COAST_K_GEMM_I8:   return 1u;
+    case COAST_K_GEMM_F16:  return 1u;
     case COAST_K_QSORT:     return 33u * (unit_bytes / 4u);
     case COAST_K_CHSTONE_SHA: return 421u * (unit_bytes / 64u + 1u);
     case COAST_K_CHSTONE_AES: return 176u;
@@ -506,19 +508,24 @@ static int encode_map(const map_desc* want, CUdeviceptr scratch, int cached, CUt
 /* One row per matmul operand type: what the GEMM launch and the kernel names need to know about it (MM_U32: its names only). */
 static const struct mm_op {
     const char* ty;                         /* the type in messages: GEMM_<ty> */
-    const char* prefix, * stem;             /* kernel names: xmr_<prefix>_<stem>...; scaled and BF16-output GEMMs swap the prefix */
+    const char* prefix, * stem;             /* kernel names: xmr_<prefix>_<stem>...; scaled and 16-bit-output GEMMs swap the prefix */
     unsigned bk;                            /* elements per k-block (one 128-byte swizzle row) */
     CUtensorMapDataType dt;                 /* A's and B's tensor-map element type */
     int b_in_place;                         /* B (K x N) is read in place, MN-major: no transposing pre-pass, no scratch */
     int bt_kernels;                         /* a caller's B^T has kernels of its own (_bt); else the same kernels read it */
     int nc_first;                           /* _nc<n>_inj<i> on the kernels that are neither grouped nor _bt (they came first) */
     int grp_variant;                        /* grouped kernels keep the path variant (the n of NC 1); else they carry none */
+    const char* c16;                        /* the prefix of the kernels with a 2-byte C: o16 (bfloat16), h16 (f16); NULL: none */
 } MM_OPS[COAST_K_COUNT_] = {
     [COAST_K_MM_U32]    = { "U32",  "mm",   "u32",  0,                0,                                0, 1, 1, 1 },
     [COAST_K_GEMM_TF32] = { "TF32", "gemm", "tf32", XMR_GEMM_BK,      CU_TENSOR_MAP_DATA_TYPE_FLOAT32,  0, 0, 1, 1 },
-    [COAST_K_GEMM_BF16] = { "BF16", "gemm", "bf16", XMR_GEMM_BF16_BK, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 1, 1, 0, 1 },
-    [COAST_K_GEMM_FP8]  = { "FP8",  "gemm", "fp8",  XMR_GEMM_FP8_BK,  CU_TENSOR_MAP_DATA_TYPE_UINT8,    0, 0, 0, 0 },
+    [COAST_K_GEMM_BF16] = { "BF16", "gemm", "bf16", XMR_GEMM_BF16_BK, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 1, 1, 0, 1, "o16" },
+    [COAST_K_GEMM_FP8]  = { "FP8",  "gemm", "fp8",  XMR_GEMM_FP8_BK,  CU_TENSOR_MAP_DATA_TYPE_UINT8,    0, 0, 0, 0, "o16" },
     [COAST_K_GEMM_I8]   = { "I8",   "gemm", "i8",   XMR_GEMM_FP8_BK,  CU_TENSOR_MAP_DATA_TYPE_UINT8,    0, 0, 0, 0 },
+    /* written with designators: GEMM_BF16's layout with IEEE binary16 elements.  (tests/test_abi.py pins the positional rows
+     * above; tests/test_gemm_f16_host_logic.py checks this one.) */
+    [COAST_K_GEMM_F16]  = { .ty = "F16", .prefix = "gemm", .stem = "f16", .bk = XMR_GEMM_BF16_BK, .dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                            .b_in_place = 1, .bt_kernels = 1, .nc_first = 0, .grp_variant = 1, .c16 = "h16" },
 };
 
 /* The shape of a matmul launch, read off its descriptor once.  Batched (COAST_MM_BATCHED): the stacked A and C are one
@@ -526,7 +533,7 @@ static const struct mm_op {
  * the stacked A and C are one R-row matrix from row ro[0] (R = n_units / N) and B is G matrices end to end. */
 typedef struct {
     unsigned es;                  /* bytes per element of A and B */
-    unsigned ces;                 /* bytes per element of C: 4, or 2 with COAST_MM_OUT_BF16 (bfloat16) */
+    unsigned ces;                 /* bytes per element of C: 4, or 2 with COAST_MM_OUT_BF16 (bfloat16) or COAST_MM_OUT_F16 (f16) */
     int batched, grouped, bt;     /* the mode bits */
     uint64_t P;                   /* products: 1, the batch or G */
     uint64_t rows;                /* stacked rows of A and C: batch*M or R */
@@ -612,8 +619,14 @@ static int mm_scale_check(const coast_launch_desc* d) {
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_SCALE_ROWWISE: d_scale_b must be 8-byte aligned (column scales are read in pairs)");
     return COAST_OK;
 }
-/* BF16 output (GEMM_BF16 and GEMM_FP8 only; not with a scale bit) */
+/* BF16 output (GEMM_BF16 and GEMM_FP8 only; not with a scale bit) and FP16 output (GEMM_F16 only; not with BF16 output) */
 static int mm_out_check(const coast_launch_desc* d) {
+    if (d->mode & COAST_MM_OUT_F16) {
+        if (d->kernel != COAST_K_GEMM_F16)
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_OUT_F16: float16 output exists for GEMM_F16 only (kernel %u)", d->kernel);
+        if (d->mode & COAST_MM_OUT_BF16)
+            return fail(COAST_ERR_BAD_ARG, "COAST_MM_OUT_F16 and COAST_MM_OUT_BF16 cannot be combined: one C type per launch");
+    }
     if (!(d->mode & COAST_MM_OUT_BF16)) return COAST_OK;
     if (d->kernel != COAST_K_GEMM_BF16 && d->kernel != COAST_K_GEMM_FP8)
         return fail(COAST_ERR_BAD_ARG, "COAST_MM_OUT_BF16: bfloat16 output exists for GEMM_BF16 and GEMM_FP8 only (kernel %u)", d->kernel);
@@ -630,7 +643,7 @@ static int mm_check(const coast_launch_desc* d, mm_shape* m) {
         (rc = mm_bit_refused(d, COAST_MM_B_TRANSPOSED)) || (rc = mm_scale_check(d)) || (rc = mm_out_check(d)))
         return rc;
     if (!is_matmul(d->kernel)) return COAST_OK;
-    m->ces = (d->mode & COAST_MM_OUT_BF16) ? 2u : KINFO[d->kernel].out_bytes;
+    m->ces = (d->mode & (COAST_MM_OUT_BF16 | COAST_MM_OUT_F16)) ? 2u : KINFO[d->kernel].out_bytes;
     m->scaled = (d->mode & (COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE)) != 0;
     m->rowwise = (d->mode & COAST_MM_SCALE_ROWWISE) != 0;
     m->es = KINFO[d->kernel].mm_elem;
@@ -674,13 +687,13 @@ static int mm_check(const coast_launch_desc* d, mm_shape* m) {
 static uint64_t mm_row_tiles(const mm_shape* m, unsigned bm) { return m->rows / bm + (m->grouped ? m->P : 0); }
 
 /* A matmul kernel's name: xmr_<prefix>_<stem><variant>[_bt][_grp], then _inj<i>_nc<n>, or _nc<n>_inj<i> where the row says so.
- * The prefix is scaled for COAST_MM_SCALE_* and o16 for COAST_MM_OUT_BF16 (2-byte C elements); the variant is the path ("n",
- * "p", "_tc", "_tiled" or ""). */
-static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, int scaled, int o16, uint32_t nc, int inj) {
+ * The prefix is scaled for COAST_MM_SCALE_* and the row's c16 for a 2-byte C (o16: COAST_MM_OUT_BF16, h16: COAST_MM_OUT_F16); the
+ * variant is the path ("n", "p", "_tc", "_tiled" or ""). */
+static void mm_kernel_name(char* name, uint32_t kernel, const char* variant, int bt, int grouped, int scaled, int c16, uint32_t nc, int inj) {
     const struct mm_op* op = &MM_OPS[kernel];
     bt = bt && op->bt_kernels;
     const int ni = op->nc_first && !bt && !grouped;
-    snprintf(name, 64, "xmr_%s_%s%s%s%s_%s%u_%s%u", scaled ? "scaled" : o16 ? "o16" : op->prefix, op->stem,
+    snprintf(name, 64, "xmr_%s_%s%s%s%s_%s%u_%s%u", scaled ? "scaled" : c16 ? op->c16 : op->prefix, op->stem,
              grouped && !op->grp_variant ? "" : variant, bt ? "_bt" : "", grouped ? "_grp" : "", ni ? "nc" : "inj", ni ? nc : (unsigned)inj,
              ni ? "inj" : "nc", ni ? (unsigned)inj : nc);
 }
@@ -826,7 +839,8 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     /* the kernels find a batch from n_units / N (rows of the stacked problem) and a.M (rows per product): a batch of one is
      * an unbatched launch, argument block included */
     a.unit_bytes = d->unit_bytes; a.flags = d->flags; a.mode = d->mode & ~(COAST_MM_BATCHED | COAST_MM_GROUPED | COAST_MM_B_TRANSPOSED |
-                                                                      COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE | COAST_MM_OUT_BF16);
+                                                                      COAST_MM_SCALE_TENSOR | COAST_MM_SCALE_ROWWISE | COAST_MM_OUT_BF16 |
+                                                                      COAST_MM_OUT_F16);
     if (m.rowwise) a.mode |= XMR_MODE_SCALE_ROWWISE;
     a.M = d->M; a.N = d->N; a.K = d->K;
     memcpy(a.key, d->key, 16);
@@ -985,9 +999,10 @@ static int launch_impl(const coast_launch_desc* d, void* stream) {
     case COAST_K_GEMM_TF32:
     case COAST_K_GEMM_BF16:
     case COAST_K_GEMM_FP8:
-    case COAST_K_GEMM_I8: {
+    case COAST_K_GEMM_I8:
+    case COAST_K_GEMM_F16: {
         /* one body for every operand type (xmr_gemm_tf32.cuh): fp32 operands read as TF32, B^T K-major from a transposing pre-pass
-         * into scratch; bfloat16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch); or E4M3 or s8
+         * into scratch; bfloat16 or float16 operands, 64-element k-blocks and B read in place (no pre-pass, no scratch); or E4M3 or s8
          * operands, 128-element k-blocks and, as for TF32, B^T K-major from a byte-transposing pre-pass (the type's MM_OPS row) */
         const struct mm_op* op = &MM_OPS[d->kernel];
         const unsigned bk = op->bk;

@@ -25,6 +25,8 @@
 // a caller's B^T (COAST_MM_B_TRANSPOSED) is read in place by the same kernels.
 // And INT8 operands (xmr_gemm_i8*, operand type I8): s8 A and B laid out as FP8's, wgmma m64n128k32 into s32 accumulators that
 // wrap, so C = A . B mod 2^32 exactly; the epilogue votes the int32 words with integer equality.
+// And FP16 operands (xmr_gemm_f16*, operand types F16 and F16T): IEEE binary16 A and B in BF16's layout (B in place MN-major, or
+// the caller's B^T K-major), wgmma m64n128k16 f16 x f16 into fp32 accumulators.
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, 64 rows of the 128-row tile each.
 // Persistent CTAs, one per SM.  Tiles: 128 x 256 unprotected (N % 256 == 0), 128 x 128 otherwise; the accumulators of a
 // replica are 64 x 128 wgmma fragments (64 fp32 registers per thread), so TMR holds 192 accumulator registers per thread.
@@ -100,6 +102,18 @@ __device__ __forceinline__ uint32_t pack_bf16x2_rn(uint32_t lo, uint32_t hi) {
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "r"(hi), "r"(lo));
     return d;
 }
+// the same into one f16x2 (IEEE binary16): finite values of 65520 or more in magnitude become infinities
+__device__ __forceinline__ uint32_t pack_f16x2_rn(uint32_t lo, uint32_t hi) {
+    uint32_t d;
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "r"(hi), "r"(lo));
+    return d;
+}
+// an f16 (the low 16 bits of h) as the fp32 of the same value, exactly
+__device__ __forceinline__ float f16_widen(uint32_t h) {
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"((unsigned short)h));
+    return f;
+}
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -170,6 +184,14 @@ __device__ __forceinline__ void wgmma_bf16_m64n128k16(float (&d)[64], uint64_t d
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(da), "l"(db), "n"(TRANS_B));
 }
+// the same with IEEE binary16 operands
+template <int TRANS_B = 1>
+__device__ __forceinline__ void wgmma_f16_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, %66;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "n"(TRANS_B));
+}
 
 // D (+)= A . B^T with both operands K-major, E4M3 x E4M3 (the 8-bit wgmma takes no transpose immediates); D's fragment layout as above
 __device__ __forceinline__ void wgmma_e4m3_m64n128k32(float (&d)[64], uint64_t da, uint64_t db) {
@@ -222,6 +244,13 @@ struct Bf16T {
     static __device__ __forceinline__ uint64_t desc_b(uint32_t saddr) { return wg_desc(saddr); }
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_bf16_m64n128k16<0>(d, da, db); }
 };
+//   F16, F16T: IEEE binary16 operands in Bf16's and Bf16T's layouts; only the wgmma's operand type differs.
+struct F16 : Bf16 {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_f16_m64n128k16(d, da, db); }
+};
+struct F16T : Bf16T {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) { wgmma_f16_m64n128k16<0>(d, da, db); }
+};
 //   Fp8: E4M3 operands, B^T K-major like Tf32's (the pre-pass's scratch or the caller's B^T): a k-block is 128 elements, the same
 //        128-byte row, and a k32 step is 32 bytes, the same descriptor step as Tf32's.  The accumulator is the wgmma's own
 //        (DESIGN.md §6: for FP8 it is narrower than fp32), as with torch._scaled_mm(use_fast_accum=True).
@@ -262,8 +291,10 @@ __device__ __forceinline__ void wgmma_u8_m64n64k32(uint32_t (&d)[32], uint64_t d
 
 template <class X, class Y> struct Same { static constexpr bool value = false; };
 template <class X> struct Same<X, X> { static constexpr bool value = true; };
-template <bool OUT_BF16> struct CElem { using T = float; };
-template <> struct CElem<true> { using T = uint16_t; };
+// C's element type (the OUT parameter of the epilogue and gemm_body): fp32 (I8: its s32 words), bfloat16 or f16
+enum COut : int { C_F32 = 0, C_BF16 = 1, C_F16 = 2 };
+template <int OUT> struct CElem { using T = uint16_t; };
+template <> struct CElem<C_F32> { using T = float; };
 __device__ __forceinline__ uint32_t acc_word(float x) { return __float_as_uint(x); }     // an accumulator's 32-bit word
 __device__ __forceinline__ uint32_t acc_word(int32_t x) { return (uint32_t)x; }
 // Epilogue of one consumer thread: vote the NC accumulators of its fragment element by element with the reference's select
@@ -274,24 +305,25 @@ __device__ __forceinline__ uint32_t acc_word(int32_t x) { return (uint32_t)x; }
 // `col` is sb[col] or sb[0] (the caller offsets both to the tile's product).  The two layouts are two instances, so neither
 // carries the other's loads and branches next to the accumulators.  Every replica reads the one copy
 // of a scale (-noMemReplication's load rule), after the main loop, so nothing of it is live next to the accumulators.
-// OUT_BF16 (xmr_o16_*, COAST_MM_OUT_BF16; not with SCALED): C holds bfloat16.  Each replica rounds its thread's two values
+// OUT C_BF16 (xmr_o16_*, COAST_MM_OUT_BF16; not with SCALED): C holds bfloat16.  Each replica rounds its thread's two values
 // (after the fault hook) into one bf16x2 with cvt.rn, the vote and the tally run on the 16-bit halves (`fcmp oeq` on the widened
 // values, the majority voter bitwise on the pair), and one 4-byte store writes the voted pair: its own branch, with its own pair vote.
-// Integer accumulators (AccT int32_t, xmr_gemm_i8*; neither SCALED nor OUT_BF16): the vote is integer equality (`icmp eq`) on the
+// OUT C_F16 (xmr_h16_*, COAST_MM_OUT_F16) is the same branch with cvt.rn.f16x2.f32 and cvt.f32.f16 for the widening.
+// Integer accumulators (AccT int32_t, xmr_gemm_i8*; neither SCALED nor 16-bit C): the vote is integer equality (`icmp eq`) on the
 // two's-complement words, with the select or the bitwise majority voter.  The fp32 vote would be wrong on them: `fcmp oeq` takes a
 // bit-31 flip of a zero C (0x80000000, -0.0) as equal to +0.0, and every C whose pattern is a NaN as a disagreement.  It shares
 // the fp32 branch -- word read, fault hook, vote and tally -- but for the compare; C is written with the same 8-byte pair stores.
 // The fault hook and the word reads stay written out in each branch: as inline helpers shared by the branches (over arrays,
 // over scalar references, with the vote or without), they changed the SASS of the TMR kernels (DESIGN.md §5.2).
-template <int NC, int NSUB, bool INJECT, bool GROUPED = false, bool SCALED = false, bool ROWWISE = false, bool OUT_BF16 = false,
+template <int NC, int NSUB, bool INJECT, bool GROUPED = false, bool SCALED = false, bool ROWWISE = false, int OUT = C_F32,
           class AccT = float>
 __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (&acc)[NC][NSUB][64], uint32_t row0, uint32_t n0, uint32_t nsub_t,
-                                         bool hints, uint64_t pol_c, typename CElem<OUT_BF16>::T* c_grp = nullptr, uint32_t row_end = 0,
+                                         bool hints, uint64_t pol_c, typename CElem<OUT>::T* c_grp = nullptr, uint32_t row_end = 0,
                                          const float* sa = nullptr, const float* sb = nullptr) {
-    static_assert(!(SCALED && OUT_BF16), "scaled GEMM_FP8 has no bfloat16-output epilogue");
+    static_assert(!(SCALED && OUT != C_F32), "scaled GEMM_FP8 has no 16-bit-output epilogue");
     constexpr bool INT_ACC = !Same<AccT, float>::value;
-    static_assert(!INT_ACC || (Same<AccT, int32_t>::value && !SCALED && !OUT_BF16), "integer accumulators: s32, unscaled, 4-byte C");
-    using CT = typename CElem<OUT_BF16>::T;
+    static_assert(!INT_ACC || (Same<AccT, int32_t>::value && !SCALED && OUT == C_F32), "integer accumulators: s32, unscaled, 4-byte C");
+    using CT = typename CElem<OUT>::T;
     const uint32_t flags = a.flags;
     const bool majority = flags & COAST_F_MAJORITY_VOTER;
     CT* C = GROUPED ? c_grp : static_cast<CT*>(a.out);
@@ -320,7 +352,7 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (
                 const uint32_t row = row0 + 8 * h, col = n0 + sub * WG_N + 8 * j + 2 * (lane & 3);
                 if constexpr (GROUPED) { if (row >= row_end) continue; }
                 const unsigned long long local0 = (unsigned long long)row * a.N + col;
-                if constexpr (OUT_BF16) {
+                if constexpr (OUT != C_F32) {
                     uint32_t x[3][2];                            // [replica][element]: the accumulators after the fault hook
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
@@ -337,16 +369,28 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (
                             }
                         }
                     }
-                    const uint32_t p0 = pack_bf16x2_rn(x[0][0], x[0][1]);         // every replica rounds its own pair
-                    const uint32_t p1 = NC > 1 ? pack_bf16x2_rn(x[1][0], x[1][1]) : p0;
-                    const uint32_t p2 = NC > 2 ? pack_bf16x2_rn(x[2][0], x[2][1]) : p0;
+                    uint32_t p0, p1, p2;                                           // every replica rounds its own pair
+                    if constexpr (OUT == C_F16) {
+                        p0 = pack_f16x2_rn(x[0][0], x[0][1]);
+                        p1 = NC > 1 ? pack_f16x2_rn(x[1][0], x[1][1]) : p0;
+                        p2 = NC > 2 ? pack_f16x2_rn(x[2][0], x[2][1]) : p0;
+                    } else {
+                        p0 = pack_bf16x2_rn(x[0][0], x[0][1]);
+                        p1 = NC > 1 ? pack_bf16x2_rn(x[1][0], x[1][1]) : p0;
+                        p2 = NC > 2 ? pack_bf16x2_rn(x[2][0], x[2][1]) : p0;
+                    }
                     uint32_t o = p0;
                     if (NC == 3 && majority) o = (p0 & p1) | (p0 & p2) | (p1 & p2);
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        const uint32_t half = e ? 0xFFFF0000u : 0x0000FFFFu;       // element e's bfloat16
-                        const float f0 = __uint_as_float(e ? p0 & half : p0 << 16), f1 = __uint_as_float(e ? p1 & half : p1 << 16),
-                                    f2 = __uint_as_float(e ? p2 & half : p2 << 16);
+                        const uint32_t half = e ? 0xFFFF0000u : 0x0000FFFFu;       // element e's bfloat16 / f16
+                        float f0, f1, f2;
+                        if constexpr (OUT == C_F16) {
+                            f0 = f16_widen(e ? p0 >> 16 : p0); f1 = f16_widen(e ? p1 >> 16 : p1); f2 = f16_widen(e ? p2 >> 16 : p2);
+                        } else {
+                            f0 = __uint_as_float(e ? p0 & half : p0 << 16); f1 = __uint_as_float(e ? p1 & half : p1 << 16);
+                            f2 = __uint_as_float(e ? p2 & half : p2 << 16);
+                        }
                         uint32_t bad = 0;
                         if (NC == 2) bad = (f0 == f1) ? 0u : 1u;
                         if (NC == 3) {
@@ -406,8 +450,8 @@ __device__ __forceinline__ void epilogue(const xmr_args& a, Tally& tally, AccT (
 // GROUPED (single CTAs with 128 x 128 tiles, xmr_mm_grp.cuh): a.M products of their own row counts, `ro` their row offsets and
 // `grp` the group block: the tiles come from its tile_start table, A through its rebased map, B^T rows from g N (Bf16: B rows from g K).
 // SCALED (xmr_scaled_fp8*): sa and sb are the caller's scales (see epilogue); a row-wise B scale vector holds N entries per product.
-// OUT_BF16 (xmr_o16_*): C holds bfloat16 at the same element offsets (see epilogue).
-template <class OP, int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false, bool SCALED = false, bool OUT_BF16 = false>
+// OUT (xmr_o16_*, xmr_h16_*): C holds bfloat16 or f16 at the same element offsets (see epilogue).
+template <class OP, int NC, bool INJECT, bool WIDE, bool PAIR, bool GROUPED = false, bool SCALED = false, int OUT = C_F32>
 __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* map_a, const CUtensorMap* map_b,
                                           const unsigned long long* ro = nullptr, const uint8_t* grp = nullptr,
                                           const float* sa = nullptr, const float* sb = nullptr) {
@@ -573,16 +617,16 @@ __device__ __forceinline__ void gemm_body(const xmr_args& a, const CUtensorMap* 
                 row0 = tm * TM + rank * BM + (uint32_t)(wg - 1) * 64u + 16u * (t >> 5) + ((t & 31) >> 2);
                 n_t = n0;
             }
-            using CT = typename CElem<OUT_BF16>::T;
+            using CT = typename CElem<OUT>::T;
             CT* const c_grp = GROUPED ? static_cast<CT*>(a.out) + c_row * a.N : nullptr;
             // the two scale layouts are two instances: one epilogue that chose at run time spilled (DESIGN.md §10 item 11).  The
             // row-wise offsets are computed in the row-wise call only.
             if (SCALED && (a.mode & XMR_MODE_SCALE_ROWWISE))
-                epilogue<NC, NSUB, INJECT, GROUPED, SCALED, true, OUT_BF16>(a, tally, acc, row0, n_t, nsub_t, hints, pol_c, c_grp, row_end,
+                epilogue<NC, NSUB, INJECT, GROUPED, SCALED, true, OUT>(a, tally, acc, row0, n_t, nsub_t, hints, pol_c, c_grp, row_end,
                                                                             sa + c_row,
                                                                             sb + (unsigned long long)(GROUPED ? prod : (tm * TM) / a.M) * a.N);
             else
-                epilogue<NC, NSUB, INJECT, GROUPED, SCALED, false, OUT_BF16>(a, tally, acc, row0, n_t, nsub_t, hints, pol_c, c_grp, row_end,
+                epilogue<NC, NSUB, INJECT, GROUPED, SCALED, false, OUT>(a, tally, acc, row0, n_t, nsub_t, hints, pol_c, c_grp, row_end,
                                                                              sa, sb);
         }
         tally.flush(a.counters);
@@ -639,7 +683,7 @@ xmr_gemm_bt_u8(const uint8_t* __restrict__ B, uint8_t* __restrict__ Bt, unsigned
 }
 
 // ---- the entry points -------------------------------------------------------------------------------------------
-// XMR_GEMM_FAMILY(OP, SCALED, OUT_BF16, STEM, BT, ORDER, GN1, XP, XA) declares one family's 20 kernels on gemm_body<OP, ...>,
+// XMR_GEMM_FAMILY(OP, SCALED, OUT, STEM, BT, ORDER, GN1, XP, XA) declares one family's 20 kernels on gemm_body<OP, ...>,
 // at inj 0 and 1 each (<i>):
 //   STEM BT <nc>            NC 1-3: 128 x 256 tiles at NC 1 (unprotected, N % 256 == 0), 128 x 128 at NC 2-3
 //   STEM n BT <nc1>         NC 1: 128 x 128 tiles (N a multiple of 128 but not of 256)
@@ -659,53 +703,59 @@ xmr_gemm_bt_u8(const uint8_t* __restrict__ B, uint8_t* __restrict__ Bt, unsigned
 #define XMR_GEMM_NAME_GRP(STEM, V, BT, NC, INJ) STEM##V##BT##_grp_inj##INJ##_nc##NC
 #define XMR_NO_CLUSTER
 #define XMR_PAIR_CLUSTER __cluster_dims__(2, 1, 1)
-#define XMR_GEMM_ENTRY(NAME, CLUSTER, OP, NC, INJ, WIDE, PAIR, GROUPED, SCALED, OUT_BF16, PARAMS, ARGS)                      \
-    extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                                       \
-    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a,                                   \
-         const __grid_constant__ CUtensorMap map_b XMR_LIST PARAMS) {                                                     \
-        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, PAIR, GROUPED, SCALED, OUT_BF16>(a, &map_a, &map_b XMR_LIST ARGS); \
+#define XMR_GEMM_ENTRY(NAME, CLUSTER, OP, NC, INJ, WIDE, PAIR, GROUPED, SCALED, OUT, PARAMS, ARGS)                         \
+    extern "C" __global__ void CLUSTER __launch_bounds__(xmr::gemm::CTA_THREADS, 1)                                        \
+    NAME(const __grid_constant__ xmr_args a, const __grid_constant__ CUtensorMap map_a,                                    \
+         const __grid_constant__ CUtensorMap map_b XMR_LIST PARAMS) {                                                      \
+        xmr::gemm::gemm_body<xmr::gemm::OP, NC, INJ != 0, WIDE, PAIR, GROUPED, SCALED, xmr::gemm::OUT>(a, &map_a, &map_b XMR_LIST ARGS); \
     }
-#define XMR_GEMM_ONE(V, NC, INJ, WIDE, PAIR, CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                         \
-    XMR_GEMM_ENTRY(XMR_GEMM_NAME_##ORDER(STEM, V, BT, NC, INJ), CLUSTER, OP, NC, INJ, WIDE, PAIR, false, SCALED, OUT_BF16, \
+#define XMR_GEMM_ONE(V, NC, INJ, WIDE, PAIR, CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                            \
+    XMR_GEMM_ENTRY(XMR_GEMM_NAME_##ORDER(STEM, V, BT, NC, INJ), CLUSTER, OP, NC, INJ, WIDE, PAIR, false, SCALED, OUT,      \
                    XP, (, nullptr, nullptr XMR_LIST XA))
-#define XMR_GEMM_GRP(V, NC, INJ, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                   \
-    XMR_GEMM_ENTRY(XMR_GEMM_NAME_GRP(STEM, V, BT, NC, INJ), XMR_NO_CLUSTER, OP, NC, INJ, false, false, true, SCALED, OUT_BF16, \
+#define XMR_GEMM_GRP(V, NC, INJ, OP, SCALED, OUT, STEM, BT, XP, XA)                                                        \
+    XMR_GEMM_ENTRY(XMR_GEMM_NAME_GRP(STEM, V, BT, NC, INJ), XMR_NO_CLUSTER, OP, NC, INJ, false, false, true, SCALED, OUT,  \
                    (, const unsigned long long* ro, const uint8_t* grp XMR_LIST XP), (, ro, grp XMR_LIST XA))
-#define XMR_GEMM_FAMILY(OP, SCALED, OUT_BF16, STEM, BT, ORDER, GN1, XP, XA)                                                \
-    XMR_GEMM_ONE(, 1, 0, true, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                      \
-    XMR_GEMM_ONE(, 2, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                     \
-    XMR_GEMM_ONE(, 3, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                     \
-    XMR_GEMM_ONE(, 1, 1, true, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                      \
-    XMR_GEMM_ONE(, 2, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                     \
-    XMR_GEMM_ONE(, 3, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                     \
-    XMR_GEMM_ONE(n, 1, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                    \
-    XMR_GEMM_ONE(n, 1, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                    \
-    XMR_GEMM_ONE(p, 1, 0, true, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                    \
-    XMR_GEMM_ONE(p, 2, 0, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                   \
-    XMR_GEMM_ONE(p, 3, 0, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                   \
-    XMR_GEMM_ONE(p, 1, 1, true, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                    \
-    XMR_GEMM_ONE(p, 2, 1, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                   \
-    XMR_GEMM_ONE(p, 3, 1, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT_BF16, STEM, BT, ORDER, XP, XA)                   \
-    XMR_GEMM_GRP(GN1, 1, 0, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                       \
-    XMR_GEMM_GRP(, 2, 0, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                          \
-    XMR_GEMM_GRP(, 3, 0, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                          \
-    XMR_GEMM_GRP(GN1, 1, 1, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                       \
-    XMR_GEMM_GRP(, 2, 1, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)                                                          \
-    XMR_GEMM_GRP(, 3, 1, OP, SCALED, OUT_BF16, STEM, BT, XP, XA)
+#define XMR_GEMM_FAMILY(OP, SCALED, OUT, STEM, BT, ORDER, GN1, XP, XA)                                                     \
+    XMR_GEMM_ONE(, 1, 0, true, false, XMR_NO_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                            \
+    XMR_GEMM_ONE(, 2, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                           \
+    XMR_GEMM_ONE(, 3, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                           \
+    XMR_GEMM_ONE(, 1, 1, true, false, XMR_NO_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                            \
+    XMR_GEMM_ONE(, 2, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                           \
+    XMR_GEMM_ONE(, 3, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                           \
+    XMR_GEMM_ONE(n, 1, 0, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                          \
+    XMR_GEMM_ONE(n, 1, 1, false, false, XMR_NO_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                          \
+    XMR_GEMM_ONE(p, 1, 0, true, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                          \
+    XMR_GEMM_ONE(p, 2, 0, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                         \
+    XMR_GEMM_ONE(p, 3, 0, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                         \
+    XMR_GEMM_ONE(p, 1, 1, true, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                          \
+    XMR_GEMM_ONE(p, 2, 1, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                         \
+    XMR_GEMM_ONE(p, 3, 1, false, true, XMR_PAIR_CLUSTER, OP, SCALED, OUT, STEM, BT, ORDER, XP, XA)                         \
+    XMR_GEMM_GRP(GN1, 1, 0, OP, SCALED, OUT, STEM, BT, XP, XA)                                                             \
+    XMR_GEMM_GRP(, 2, 0, OP, SCALED, OUT, STEM, BT, XP, XA)                                                                \
+    XMR_GEMM_GRP(, 3, 0, OP, SCALED, OUT, STEM, BT, XP, XA)                                                                \
+    XMR_GEMM_GRP(GN1, 1, 1, OP, SCALED, OUT, STEM, BT, XP, XA)                                                             \
+    XMR_GEMM_GRP(, 2, 1, OP, SCALED, OUT, STEM, BT, XP, XA)                                                                \
+    XMR_GEMM_GRP(, 3, 1, OP, SCALED, OUT, STEM, BT, XP, XA)
 
 // fp32 C: TF32 (B^T from the transposing pre-pass or the caller), BF16 with B read in place and with B^T read in place, FP8
-// (E4M3; B^T from the byte pre-pass or the caller), INT8 (s8, s32 C, integer vote; FP8's layout)
-XMR_GEMM_FAMILY(Tf32, false, false, xmr_gemm_tf32, , NI, n, (), ())
-XMR_GEMM_FAMILY(Bf16, false, false, xmr_gemm_bf16, , IN, n, (), ())
-XMR_GEMM_FAMILY(Bf16T, false, false, xmr_gemm_bf16, _bt, IN, n, (), ())
-XMR_GEMM_FAMILY(Fp8, false, false, xmr_gemm_fp8, , IN, , (), ())
-XMR_GEMM_FAMILY(I8, false, false, xmr_gemm_i8, , IN, , (), ())
+// (E4M3; B^T from the byte pre-pass or the caller), INT8 (s8, s32 C, integer vote; FP8's layout), FP16 (BF16's layout)
+XMR_GEMM_FAMILY(Tf32, false, C_F32, xmr_gemm_tf32, , NI, n, (), ())
+XMR_GEMM_FAMILY(Bf16, false, C_F32, xmr_gemm_bf16, , IN, n, (), ())
+XMR_GEMM_FAMILY(Bf16T, false, C_F32, xmr_gemm_bf16, _bt, IN, n, (), ())
+XMR_GEMM_FAMILY(Fp8, false, C_F32, xmr_gemm_fp8, , IN, , (), ())
+XMR_GEMM_FAMILY(I8, false, C_F32, xmr_gemm_i8, , IN, , (), ())
+XMR_GEMM_FAMILY(F16, false, C_F32, xmr_gemm_f16, , IN, n, (), ())
+XMR_GEMM_FAMILY(F16T, false, C_F32, xmr_gemm_f16, _bt, IN, n, (), ())
 // Scaled FP8 (COAST_MM_SCALE_TENSOR / COAST_MM_SCALE_ROWWISE): the scale pointers follow the maps (grouped: ro and grp); every
 // replica multiplies its accumulator by the A and B scales before the vote
-XMR_GEMM_FAMILY(Fp8, true, false, xmr_scaled_fp8, , IN, , (, const float* sa, const float* sb), (, sa, sb))
+XMR_GEMM_FAMILY(Fp8, true, C_F32, xmr_scaled_fp8, , IN, , (, const float* sa, const float* sb), (, sa, sb))
 // BF16 output (COAST_MM_OUT_BF16): every GEMM_BF16 and GEMM_FP8 kernel once more, named xmr_o16_ + the name without its
 // xmr_gemm_ prefix; C holds bfloat16, each replica rounds its values before the vote (see epilogue).  Scaled GEMM_FP8 has no
 // BF16-output set: its TMR and DWC kernels spilled 104-296 bytes with it (DESIGN.md §10 item 12)
-XMR_GEMM_FAMILY(Bf16, false, true, xmr_o16_bf16, , IN, n, (), ())
-XMR_GEMM_FAMILY(Bf16T, false, true, xmr_o16_bf16, _bt, IN, n, (), ())
-XMR_GEMM_FAMILY(Fp8, false, true, xmr_o16_fp8, , IN, , (), ())
+XMR_GEMM_FAMILY(Bf16, false, C_BF16, xmr_o16_bf16, , IN, n, (), ())
+XMR_GEMM_FAMILY(Bf16T, false, C_BF16, xmr_o16_bf16, _bt, IN, n, (), ())
+XMR_GEMM_FAMILY(Fp8, false, C_BF16, xmr_o16_fp8, , IN, , (), ())
+// FP16 output (COAST_MM_OUT_F16, GEMM_F16 only): every GEMM_F16 kernel once more, named xmr_h16_ + the name without its
+// xmr_gemm_ prefix; C holds f16, each replica rounds its values before the vote
+XMR_GEMM_FAMILY(F16, false, C_F16, xmr_h16_f16, , IN, n, (), ())
+XMR_GEMM_FAMILY(F16T, false, C_F16, xmr_h16_f16, _bt, IN, n, (), ())

@@ -15,29 +15,32 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 K_CRC16, K_SHA256, K_AES128, K_MM_U32, K_GEMM_TF32, K_QSORT, K_CHSTONE_SHA, K_CHSTONE_AES, K_GEMM_BF16 = range(9)
 K_GEMM_FP8 = 10                              # FP8 E4M3 operands, fp32 out; id 9 is unassigned
 K_GEMM_I8 = 12                               # int8 operands, int32 out, exact mod 2^32, integer vote; id 11 is unassigned
+K_GEMM_F16 = 14                              # float16 operands, fp32 out (MM_OUT_F16: float16); GEMM_BF16's layout; id 13 is unassigned
 F_COUNT_ERRORS, F_COUNT_SYNCS, F_NO_MEM_REPLICATION = 0x1, 0x2, 0x4
 F_INTERLEAVE, F_SEGMENT, F_VERBOSE, F_MAJORITY_VOTER = 0x8, 0x10, 0x20, 0x100
 F_STORE_DATA_SYNC, F_NO_STORE_DATA_SYNC, F_NO_LOAD_SYNC, F_NO_STORE_ADDR_SYNC = 0x200, 0x400, 0x800, 0x1000
 PLAN_NONE, PLAN_BERNOULLI, PLAN_TABLE = 0, 1, 2
 AES_DECRYPT, AES_KEY_PER_UNIT, AES_KEY_WRITEBACK = 1, 2, 4
 UNIT_OFFSETS = COAST_UNIT_OFFSETS = 0x10000  # ragged CRC16 / SHA256 / QSORT batches: aux = n_units + 1 u64 byte offsets into inp
-MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8: n_units = batch*M*N, inp / aux / out hold batch A / B / C
-MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
-MM_B_TRANSPOSED = COAST_MM_B_TRANSPOSED = 0x80000  # MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8: aux holds B^T, N x K per product (nn.Linear.weight)
+MM_BATCHED = COAST_MM_BATCHED = 0x20000      # batched MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8 / GEMM_F16: n_units = batch*M*N, inp / aux / out hold batch A / B / C
+MM_GROUPED = COAST_MM_GROUPED = 0x40000      # grouped MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8 / GEMM_F16: M = G products, rows = G + 1 u64 row offsets, n_units = R*N
+MM_B_TRANSPOSED = COAST_MM_B_TRANSPOSED = 0x80000  # MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8 / GEMM_F16: aux holds B^T, N x K per product (nn.Linear.weight)
 MM_SCALE_TENSOR = COAST_MM_SCALE_TENSOR = 0x100000    # GEMM_FP8: one fp32 scale of A and one of B, applied by every replica before the vote
 MM_SCALE_ROWWISE = COAST_MM_SCALE_ROWWISE = 0x200000  # GEMM_FP8: one fp32 scale per row of the stacked A and per column of each product's B
 MM_OUT_BF16 = COAST_MM_OUT_BF16 = 0x400000            # GEMM_BF16 / GEMM_FP8: C is bfloat16, every replica rounds before the vote
+MM_OUT_F16 = COAST_MM_OUT_F16 = 0x800000              # GEMM_F16: C is float16, every replica rounds before the vote
 NO_FAULT_UNIT = 0xFFFFFFFFFFFFFFFF
 ERR_NO_DRIVER, ERR_NOT_INIT, ERR_BAD_ARG, ERR_UNSUPPORTED, ERR_BUSY = -100001, -100002, -100003, -100004, -100005
 
 OUT_BYTES = {K_CRC16: 2, K_SHA256: 32, K_AES128: 16, K_MM_U32: 4, K_GEMM_TF32: 4, K_CHSTONE_SHA: 20, K_CHSTONE_AES: 64, K_GEMM_BF16: 4,
-             K_GEMM_FP8: 4, K_GEMM_I8: 4}
-MM_ELEM_BYTES = {K_GEMM_BF16: 2, K_GEMM_FP8: 1, K_GEMM_I8: 1}   # bytes per A and B element of the matmuls; 4 for MM_U32 and GEMM_TF32
+             K_GEMM_FP8: 4, K_GEMM_I8: 4, K_GEMM_F16: 4}
+MM_ELEM_BYTES = {K_GEMM_BF16: 2, K_GEMM_FP8: 1, K_GEMM_I8: 1, K_GEMM_F16: 2}   # bytes per A and B element of the matmuls; 4 for MM_U32 and GEMM_TF32
 
 
 def out_bytes(kernel: int, unit_bytes: int = 0, mode: int = 0) -> int:
-    """bytes of output per unit; with MM_OUT_BF16, GEMM_BF16 and GEMM_FP8 write 2-byte bfloat16 C elements"""
-    if mode & MM_OUT_BF16 and kernel in (K_GEMM_BF16, K_GEMM_FP8):
+    """bytes of output per unit; with MM_OUT_BF16, GEMM_BF16 and GEMM_FP8 write 2-byte bfloat16 C elements, and with
+    MM_OUT_F16 GEMM_F16 writes 2-byte float16 ones"""
+    if mode & MM_OUT_BF16 and kernel in (K_GEMM_BF16, K_GEMM_FP8) or mode & MM_OUT_F16 and kernel == K_GEMM_F16:
         return 2
     return unit_bytes if kernel == K_QSORT else OUT_BYTES[kernel]
 
@@ -297,7 +300,9 @@ class Runtime:
         scale_b one per column of each product's B.  With MM_OUT_BF16 (K_GEMM_BF16, K_GEMM_FP8) the result is bfloat16 bytes, two
         per element: view it as torch.bfloat16.
         K_GEMM_I8: inp and aux are torch.int8 tensors (or their uint8 views); the result is int32, 4 bytes per element: view it as
-        torch.int32.  It takes no scales and no MM_OUT_BF16."""
+        torch.int32.  It takes no scales and no MM_OUT_BF16.
+        K_GEMM_F16: inp and aux are torch.float16 tensors (or their int16 / uint16 views); the result is fp32, or with MM_OUT_F16
+        float16 bytes, two per element: view it as torch.float16.  It takes no scales and no MM_OUT_BF16 (the library refuses them)."""
         torch = self.torch
         self._check_i8(kernel, mode, scale_a, scale_b)
         if mode & MM_GROUPED:
@@ -404,7 +409,8 @@ class Runtime:
                  abort_on_dwc: bool = False, h_rows=None, scale_a=None, scale_b=None) -> Stats:
         """h_in/h_out/h_aux: CPU torch tensors or numpy arrays (pinned memory makes the copies async); scale_a / scale_b: the
         host float32 scales of a MM_SCALE_TENSOR or MM_SCALE_ROWWISE call.  With MM_OUT_BF16, h_out receives bfloat16 bytes, two
-        per element.  K_GEMM_I8: int8 operands, h_out receives int32 elements; no scales and no MM_OUT_BF16."""
+        per element.  K_GEMM_I8: int8 operands, h_out receives int32 elements; no scales and no MM_OUT_BF16.  K_GEMM_F16: float16
+        operands (or their 16-bit integer views); with MM_OUT_F16, h_out receives float16 bytes, two per element."""
         self._check_i8(kernel, mode, scale_a, scale_b)
 
         def ptr(x):

@@ -76,7 +76,10 @@ typedef enum coast_kernel_id {
                                COAST_MM_B_TRANSPOSED) */
     /* 11 is not assigned either */
     COAST_K_GEMM_I8   = 12, /* int8 (s8) in, int32 out, exact mod 2^32, wgmma s8; B^T read K-major as for GEMM_FP8; integer vote */
-    COAST_K_COUNT_    = 13
+    /* 13 is not assigned either */
+    COAST_K_GEMM_F16  = 14, /* float16 (IEEE binary16) in, fp32 accumulate and out (f16 with COAST_MM_OUT_F16), wgmma f16;
+                               GEMM_BF16's layout: B read in place */
+    COAST_K_COUNT_    = 15
 } coast_kernel_id;
 
 /* numClones of dataflowProtection::run: 3 = -TMR, 2 = -DWC, 1 = unprotected
@@ -193,7 +196,15 @@ typedef struct coast_fault_plan {
  *            for -0.0 == +0.0, so TMR's select voter would store INT_MIN silently and DWC would miss the flip; and every C in
  *            [-8388607, -1] or [2139095041, 2147483647] is a NaN pattern, which `fcmp oeq` would count as a disagreement.
  *            COAST_MM_SCALE_* and COAST_MM_OUT_BF16 are refused (COAST_ERR_BAD_ARG).
- *   MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8 with COAST_MM_B_TRANSPOSED: aux: B^T, N x K row-major per product (see below).
+ *   GEMM_F16 in : A, M x K float16 (IEEE binary16) row-major; aux: B, K x N float16 row-major   out: C, M x N float: the
+ *            fp32-accumulated sum of the exact f16 x f16 products (float16 with COAST_MM_OUT_F16, see below).  Every rule of
+ *            GEMM_BF16 holds unchanged: M%128 == N%128 == K%64 == 0 (grouped: N and K only), buffers 16-byte aligned, B read in
+ *            place MN-major with no pre-pass and no scratch, B^T (COAST_MM_B_TRANSPOSED) read in place K-major, COAST_MM_BATCHED
+ *            and COAST_MM_GROUPED with element offsets counting 2-byte elements in d_in and d_aux, and the 2^31 bounds.  A unit is
+ *            one C element with one fault site of width 32 on the accumulator and one `fcmp oeq` vote, as GEMM_TF32, so a plan
+ *            draws the faults of a GEMM_BF16 launch of the same shape.  COAST_MM_SCALE_* and COAST_MM_OUT_BF16 are refused
+ *            (COAST_ERR_BAD_ARG).
+ *   MM_U32 / GEMM_TF32 / GEMM_BF16 / GEMM_FP8 / GEMM_I8 / GEMM_F16 with COAST_MM_B_TRANSPOSED: aux: B^T, N x K row-major per product (see below).
  *   QSORT    in : n_units x unit_bytes, arrays of L = unit_bytes/4 int32 (L <= 1024)   out: the sorted arrays
  *   CHSTONE_SHA in : n_units x unit_bytes stream bytes (unit_bytes a multiple of 64, 64 <= unit_bytes < 2^29)
  *            out: n_units x 5 uint32 = sha_info_digest[5] (sha.h:38)
@@ -222,42 +233,42 @@ typedef struct coast_fault_plan {
  * SHA256, whose d_out is indexed by the shard's own units) and unit_base = lo.  COAST_QSORT_PATH=nested gives
  * COAST_ERR_UNSUPPORTED: a ragged batch runs the state-machine scheduling only. */
 #define COAST_UNIT_OFFSETS      0x10000u
-/* Batched matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8 and GEMM_I8 only): with COAST_MM_BATCHED in `mode`, M, N and K are the shape of ONE product and
+/* Batched matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8 and GEMM_F16 only): with COAST_MM_BATCHED in `mode`, M, N and K are the shape of ONE product and
  * n_units = batch x M x N.  d_in holds `batch` A matrices (M x K) end to end, d_aux `batch` B matrices (K x N) and d_out
  * receives `batch` C matrices (M x N), all dense and row-major.  The launch equals `batch` single launches, matrix b with
  * d_in + b*M*K, d_aux + b*K*N, d_out + b*M*N (elements) and unit_base + b*M*N: the same output bytes, summed counters and
  * minimum first_fault_unit.  Fault plans stay keyed by the global unit index (a TABLE plan has n_units entries), and the
  * in-loop store votes keep their meaning (K + 1 votes per unit on the plain kernel).  Each path's shape rules apply to the
- * per-matrix M, N and K; a TF32 / BF16 / FP8 / I8 CTA pair needs the per-matrix M to be a multiple of 256.  COAST_ERR_BAD_ARG for the bit on
- * any other kernel, for n_units zero or not a multiple of M*N, and for batch*M or batch*N (GEMM_BF16 without COAST_MM_B_TRANSPOSED:
+ * per-matrix M, N and K; a TF32 / BF16 / FP8 / I8 / F16 CTA pair needs the per-matrix M to be a multiple of 256.  COAST_ERR_BAD_ARG for the bit on
+ * any other kernel, for n_units zero or not a multiple of M*N, and for batch*M or batch*N (GEMM_BF16 and GEMM_F16 without COAST_MM_B_TRANSPOSED:
  * batch*K) at or above 2^31.  Without the
  * bit n_units must be M*N; with batch = 1 the launch is identical to an unbatched one.  A shard takes whole matrices
  * [b_lo, b_hi): the three pointers and unit_base offset as above, n_units = (b_hi - b_lo) x M x N. */
 #define COAST_MM_BATCHED        0x20000u
-/* Grouped matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8 and GEMM_I8 only): with COAST_MM_GROUPED in `mode`, M is the number of products G (at least 1) and N
+/* Grouped matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8 and GEMM_F16 only): with COAST_MM_GROUPED in `mode`, M is the number of products G (at least 1) and N
  * and K are shared by all of them.  d_rows points to G + 1 non-decreasing uint64_t row offsets ro[] (8-byte aligned; a device
  * pointer for coast_launch, a host pointer for coast_run_host): product g has M_g = ro[g+1] - ro[g] rows (zero is allowed),
  * its A at d_in + ro[g]*K, its B at d_aux + g*K*N and its C at d_out + ro[g]*N (elements); d_aux holds the G dense K x N
  * matrices end to end.  n_units = R*N with R = ro[G] - ro[0] the rows of all products.  The launch equals G single launches,
  * product g with M = M_g and unit_base + (ro[g] - ro[0])*N: the same output elements, summed counters, minimum
  * first_fault_unit and d_status bytes (coast_launch).  Fault plans stay keyed by the global unit index (a TABLE plan has n_units
- * entries); the sites are those of the kernel (K for MM_U32, 1 for GEMM_TF32, GEMM_BF16, GEMM_FP8 and GEMM_I8) and the in-loop store votes keep K + 1 votes per
+ * entries); the sites are those of the kernel (K for MM_U32, 1 for GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8 and GEMM_F16) and the in-loop store votes keep K + 1 votes per
  * unit.  Each path's shape rules apply to N and K only: every M_g is allowed on every path.  The kernels clamp every offset to
  * [ro[0], ro[0] + R] and count a decreasing pair as zero rows, so a malformed table never reads or writes outside
  * [ro[0], ro[0] + R) rows of the buffers; coast_run_host (and Runtime.run) refuse a table that decreases or whose last offset is
  * not ro[0] + R.  COAST_ERR_BAD_ARG for the bit on any other kernel or with COAST_MM_BATCHED or COAST_UNIT_OFFSETS, for G = 0
- * or above 2^20, for n_units not a multiple of N, for R or G*N (GEMM_BF16 without COAST_MM_B_TRANSPOSED: G*K) at or above 2^31,
+ * or above 2^20, for n_units not a multiple of N, for R or G*N (GEMM_BF16 and GEMM_F16 without COAST_MM_B_TRANSPOSED: G*K) at or above 2^31,
  * and for a null or misaligned d_rows.  A shard
  * takes whole products [g_lo, g_hi): d_rows + g_lo with the same d_in and d_out, d_aux + g_lo*K*N, M = g_hi - g_lo,
  * n_units = (ro[g_hi] - ro[g_lo])*N and unit_base + (ro[g_lo] - ro[0])*N. */
 #define COAST_MM_GROUPED        0x40000u
-/* Transposed B (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8 and GEMM_I8 only), the layout of a linear layer's weight: with COAST_MM_B_TRANSPOSED in
+/* Transposed B (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8 and GEMM_F16 only), the layout of a linear layer's weight: with COAST_MM_B_TRANSPOSED in
  * `mode`, d_aux holds B^T, each product's B stored as N rows of K elements, row-major: element (k, n) of product p is at
  * d_aux[p*N*K + n*K + k].  It combines with COAST_MM_BATCHED and COAST_MM_GROUPED; the product offsets into d_aux (p*K*N
  * elements) and the shard rules stay as documented there.  The launch equals the same launch without the bit whose d_aux holds
  * every product's B = (B^T)^T: the same output bytes, summed counters, minimum first_fault_unit and d_status bytes.  Fault sites,
  * their widths, TABLE plans and the in-loop store votes are unchanged.  B^T is read in place: GEMM_TF32 runs no transposing
- * pre-pass and needs no B^T scratch, GEMM_BF16 reads B^T K-major, GEMM_FP8 and GEMM_I8 run no byte-transposing pre-pass and need no
+ * pre-pass and needs no B^T scratch, GEMM_BF16 and GEMM_F16 read B^T K-major, GEMM_FP8 and GEMM_I8 run no byte-transposing pre-pass and need no
  * scratch (a grouped launch still allocates its group block), MM_U32's limb path splits B^T like A.  Each path's shape
  * rules are unchanged; the 2^31 bound on B's stacked rows is on batch*N (grouped: G*N) for every kernel with the bit.
  * COAST_ERR_BAD_ARG for the bit on any other kernel. */
@@ -301,6 +312,16 @@ typedef struct coast_fault_plan {
  * coast_run_host stages and downloads C at 2 bytes per element.  coast_out_bytes() does not see the mode and returns the fp32
  * size (4); a caller sizes a bf16 C at 2 bytes per unit. */
 #define COAST_MM_OUT_BF16       0x400000u
+/* FP16 output (GEMM_F16 only): with COAST_MM_OUT_F16 in `mode`, C is float16 (IEEE binary16), what torch.matmul returns for
+ * half tensors.  Everything COAST_MM_OUT_BF16 says above holds with f16 for bf16: the same layout and element offsets (2-byte
+ * elements), the same fault sites, and each replica rounds its accumulator after the fault hook, v_r = f16(x_r), to nearest even
+ * (cvt.rn.f16x2.f32: subnormals are kept, finite values of 65520 or more in magnitude become infinities, a NaN becomes 0x7FFF).
+ * The vote (`fcmp oeq` on the widened values; the majority voter bitwise on the 16-bit patterns), the counters and d_status
+ * work on the rounded values.  With at most one flip per unit, the f16 C equals the fp32 C of the same launch and plan rounded
+ * to nearest even, except for the sign of a zero where TMR's select voter meets a sign flip on replica 0 of a value that rounds
+ * to zero (DESIGN.md §3.15).  COAST_ERR_BAD_ARG for the bit on any other kernel and together with COAST_MM_OUT_BF16.
+ * coast_run_host stages and downloads C at 2 bytes per element; coast_out_bytes() returns the fp32 size (4). */
+#define COAST_MM_OUT_F16        0x800000u
 #define COAST_AES_DECRYPT       0x1u
 #define COAST_AES_KEY_PER_UNIT  0x2u
 #define COAST_AES_KEY_WRITEBACK 0x4u   /* with KEY_PER_UNIT: store what aes_enc_dec() leaves in key[] (TI_aes_128.c:214-221 mutates
@@ -316,7 +337,7 @@ typedef struct coast_launch_desc {
     uint64_t n_units;      /* units in THIS launch                                */
     uint64_t unit_base;    /* global index of this launch's unit 0 (fault plans)  */
     uint32_t unit_bytes;   /* CRC16/SHA256: message length of every unit          */
-    uint32_t M, N, K;      /* the matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8) */
+    uint32_t M, N, K;      /* the matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8, GEMM_F16) */
     const void* d_in;
     void*       d_out;
     const void* d_aux;
@@ -441,7 +462,7 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  *     ONE launch reads the mapped host memory and writes the voted output straight back; the
  *     default when the output is at most 1/8 of the input (CRC16, CHSTONE_SHA);
  *   hybrid: the staged chunks' kernels read a pinned input in place, outputs are staged;
- *   matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8): B goes up once and C comes down in row blocks (one-shot: one
+ *   matmuls (MM_U32, GEMM_TF32, GEMM_BF16, GEMM_FP8, GEMM_I8, GEMM_F16): B goes up once and C comes down in row blocks (one-shot: one
  *     block for small or oddly shaped problems).
  * COAST_HOST_PATH=staged|hybrid|zerocopy forces a path, and for matmuls one-shot forces one block
  * (INTEGRATION.md §config).  Ragged calls (COAST_UNIT_OFFSETS, d_aux = host offsets, which must never
@@ -455,7 +476,7 @@ int  coast_fill_philox(void* d_dst, uint64_t n_words, uint64_t word_base, uint32
  * biased by ro[first] rows.  Scaled GEMM_FP8 (COAST_MM_SCALE_*) keeps the chunks of the unscaled call: tensorwise, the two
  * floats go up once; row-wise, row blocks send B's column scales once with B and each block its rows' A scales, batched chunks
  * the A rows and B columns of their products, grouped chunks A scales [ro[first], ro[end]) biased like d_in and B scales
- * [first*N, end*N).  With COAST_MM_OUT_BF16 the same schedules move C at 2 bytes per element.  On any failure every copy already queued on
+ * [first*N, end*N).  With COAST_MM_OUT_BF16 or COAST_MM_OUT_F16 the same schedules move C at 2 bytes per element.  On any failure every copy already queued on
  * the caller's buffers is drained before the call returns. */
 int  coast_run_host(const coast_launch_desc* desc_with_host_ptrs, coast_stats* out);
 /* What the last host call did: "staged", "hybrid" or "zerocopy"; unbatched matmuls: "row-blocks" or "one-shot"; grouped: "groups". */
